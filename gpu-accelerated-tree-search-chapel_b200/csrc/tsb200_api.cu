@@ -2188,6 +2188,11 @@ void* tsb_pfsp_stream(const tsb_pfsp* h) { return h ? static_cast<void*>(h->stre
 
 uint64_t tsb_pfsp_slow_rounds(const tsb_pfsp* h) { return h ? h->slow_rounds : 0; }
 
+int tsb_pfsp_route(const tsb_pfsp* h) {
+  if (!h) return TSB_EINVAL;
+  return h->mt | (h->simd16 ? TSB_ROUTE_SIMD16 : 0) | (h->pairs > 0 ? TSB_ROUTE_LB2 : 0) | (h->lb2u ? TSB_ROUTE_LB2U : 0);
+}
+
 int tsb_pfsp_expand_device(tsb_pfsp* h, int lb_kind, const void* parents_d, int count, int64_t* best,
                            void* children_d, uint64_t* n_children, uint64_t* n_solutions, void* stream) {
   if (h && h->wide) return TSB_EUNSUPPORTED;  // (the fused expand / device pool exist for MAX_JOBS = 20 only)

@@ -11,8 +11,8 @@ meaning (`size` = N*poolSize resp. jobs*poolSize, results in `labels` / `bounds`
 arrays standing for the Chapel records.  There is no CPU fallback: without libtsb200.so or a CUDA
 device every call raises.
 """
-from ._lib import (LB1, LB1_D, LB2, XFER_AUTO, XFER_MEMCPY, XFER_ZEROCOPY, PfspTables, SearchStats, TsbError,
-                   check, lib)
+from ._lib import (LB1, LB1_D, LB2, ROUTE_LB2, ROUTE_LB2U, ROUTE_MT_MASK, ROUTE_SIMD16, XFER_AUTO, XFER_MEMCPY,
+                   XFER_ZEROCOPY, PfspTables, PfspTables50, SearchStats, TsbError, check, lib)
 from .nqueens import (NQ_NODE_DTYPE, NQueensEvaluator, nqueens_search, nqueens_search_device,
                       nqueens_pool_run_multi, nqueens_search_device_part, nqueens_warmup)
 from .pfsp import (PFSP_NODE_DTYPE, PFSP_NODE50_DTYPE, LB_NAMES, LB2_VARIANTS, PfspEvaluator, taillard_tables50, pfsp_search, pfsp_search_device,
@@ -22,4 +22,5 @@ __all__ = ["NQueensEvaluator", "PfspEvaluator", "nqueens_warmup", "nqueens_pool_
            "pfsp_search_device_part",
            "taillard_tables",
            "NQ_NODE_DTYPE", "PFSP_NODE_DTYPE", "PFSP_NODE50_DTYPE", "LB2_VARIANTS", "taillard_tables50", "LB_NAMES", "LB1", "LB1_D", "LB2", "TsbError", "lib", "check",
-           "PfspTables", "SearchStats", "XFER_AUTO", "XFER_MEMCPY", "XFER_ZEROCOPY"]
+           "PfspTables", "PfspTables50", "SearchStats", "XFER_AUTO", "XFER_MEMCPY", "XFER_ZEROCOPY",
+           "ROUTE_MT_MASK", "ROUTE_SIMD16", "ROUTE_LB2", "ROUTE_LB2U"]

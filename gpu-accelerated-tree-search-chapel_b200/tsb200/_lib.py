@@ -15,6 +15,8 @@ MAX_PAIRS = 190
 OK, EINVAL, ECUDA, ENOMEM, ENODEV, EALIGN, EUNSUPPORTED = 0, -1, -2, -3, -4, -5, -6
 LB1_D, LB1, LB2 = 0, 1, 2
 XFER_AUTO, XFER_MEMCPY, XFER_ZEROCOPY = 0, 1, 2
+# tsb_pfsp_route: template machine count in the low byte, and which kernel specialisations the handle uses
+ROUTE_MT_MASK, ROUTE_SIMD16, ROUTE_LB2, ROUTE_LB2U = 0xFF, 0x100, 0x200, 0x400
 
 
 class TsbError(RuntimeError):
@@ -106,6 +108,7 @@ SYMBOLS = {
     "tsb_pfsp_pool_step": (_i, [_vp, _i, _i, _i, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_u64), C.POINTER(_u64)]),
     "tsb_pfsp_pool_drain": (_i, [_vp, _vp, _i64, C.POINTER(_i64)]),
     "tsb_pfsp_slow_rounds": (_u64, [_vp]),
+    "tsb_pfsp_route": (_i, [_vp]),
     "tsb_pfsp_register_host": (_i, [_vp, _vp, C.c_size_t]),
     "tsb_pfsp_unregister_host": (_i, [_vp, _vp]),
     "tsb_pfsp_set_xfer": (_i, [_vp, _i]),

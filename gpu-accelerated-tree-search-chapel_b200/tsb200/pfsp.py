@@ -129,6 +129,13 @@ class PfspEvaluator:
     def slow_rounds(self) -> int:
         return int(lib().tsb_pfsp_slow_rounds(self._h))
 
+    @property
+    def route(self) -> int:
+        """tsb_pfsp_route: template machine count | ROUTE_SIMD16 | ROUTE_LB2 | ROUTE_LB2U"""
+        r = int(lib().tsb_pfsp_route(self._h))
+        check(min(r, 0), "tsb_pfsp_route")
+        return r
+
     def pool_step(self, lb, m: int, M: int, best: int):
         """(parents popped, children appended, solutions, best_after) of one device-side offload round"""
         kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)

@@ -190,7 +190,11 @@ typedef struct tsb_pfsp tsb_pfsp;
  * lb2_bound_data (lib/pfsp/Bound_johnson.chpl:11-48):
  *   p_times[machines*jobs] machine-major (k*jobs + job); min_heads/min_tails[machines];
  *   johnson[nb_pairs*jobs], lags[nb_pairs*jobs]; mp0/mp1/mp_order[nb_pairs].
- * jobs <= 20 (the reference's MAX_JOBS), machines <= 20, nb_pairs <= 190. */
+ * jobs <= 20 (the reference's MAX_JOBS), machines <= 20, nb_pairs <= 190.
+ * lb2 keeps its tables in packed words, so a handle refuses lb2 (every TSB_LB2 call on it returns TSB_EINVAL;
+ * lb1 / lb1_d are unaffected) when nb_pairs == 0 (one machine), when any p_times entry of a paired machine is
+ * outside 0..127, any lag outside 0..8191 (0..4095 on a tsb_pfsp_create_wide handle), or any min_tails entry of a
+ * paired machine outside 0..2047.  tsb_pfsp_route tells which case a handle is in. */
 int tsb_pfsp_create(tsb_pfsp** h, int device, int jobs, int machines, int M_max, const int32_t* p_times,
                     const int32_t* min_heads, const int32_t* min_tails, int nb_pairs,
                     const int32_t* johnson, const int32_t* lags, const int32_t* mp0, const int32_t* mp1,
@@ -240,6 +244,14 @@ int tsb_pfsp_set_xfer(tsb_pfsp* h, int mode);
 uint64_t tsb_pfsp_kernel_launches(const tsb_pfsp* h);
 void* tsb_pfsp_stream(const tsb_pfsp* h);
 uint64_t tsb_pfsp_slow_rounds(const tsb_pfsp* h); /* expand rounds redone on the host because a leaf improved best */
+/* diagnostics: which kernel specialisations tsb_pfsp_create chose for the handle's tables.  The low byte is the
+ * template machine count (5, 10 or 20: fewer machines are zero-padded up to it); TSB_ROUTE_SIMD16: lb1 / lb1_d
+ * evaluate two children per register (all values >= 0, min_tails non-increasing, sum of p_times + largest
+ * min_heads + largest min_tails < 65536; env TSB200_NO_SIMD16 turns it off); TSB_ROUTE_LB2: lb2 is available (see
+ * tsb_pfsp_create); TSB_ROUTE_LB2U: lb2 uses the one-word-per-use table (<= 10 machines with TSB_ROUTE_SIMD16; env
+ * TSB200_NO_LB2U=1 turns it off), else the packed one.  TSB_EINVAL for a NULL handle. */
+enum { TSB_ROUTE_MT_MASK = 0xFF, TSB_ROUTE_SIMD16 = 0x100, TSB_ROUTE_LB2 = 0x200, TSB_ROUTE_LB2U = 0x400 };
+int tsb_pfsp_route(const tsb_pfsp* h);
 
 /* ------------------------------------------------------------------ host-side problem data
  * (CPU code the Chapel drivers already own — lib/pfsp/Taillard.chpl, fill_* in Bound_*.chpl —

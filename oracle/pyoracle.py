@@ -84,6 +84,7 @@ def lib() -> C.CDLL:
         L.or_taillard_processing_times.argtypes = [vp, i32]
         L.or_pfsp_tables_build.argtypes = [C.POINTER(Tables), i32, i32]
         L.or_pfsp_tables_build_variant.argtypes = [C.POINTER(Tables), i32, i32, i32]
+        L.or_pfsp_tables_from_ptimes.argtypes = [C.POINTER(Tables), i32, i32, vp, i32, i32]
         L.or_eval_solution.argtypes = [C.POINTER(Tables), vp]
         L.or_eval_solution.restype = C.c_int32
         L.or_lb1_bound.argtypes = [C.POINTER(Tables), vp, C.c_int32, C.c_int32]
@@ -121,6 +122,17 @@ def tables(inst: int, heads_mode: int = 0, variant: int = 0) -> Tables:
     rc = lib().or_pfsp_tables_build_variant(C.byref(t), inst, heads_mode, variant)
     if rc != 0:
         raise ValueError(f"or_pfsp_tables_build({inst}) -> {rc}")
+    return t
+
+
+def tables_from_ptimes(p_times, heads_mode: int = 0, variant: int = 0, L=None, cls=Tables):
+    """the tables fill_* build from a processing-time matrix p_times[machines, jobs] (any values)"""
+    p = np.ascontiguousarray(p_times, dtype=np.int32)
+    machines, jobs = p.shape
+    t = cls()
+    rc = (L or lib()).or_pfsp_tables_from_ptimes(C.byref(t), jobs, machines, _ptr(p), heads_mode, variant)
+    if rc != 0:
+        raise ValueError(f"or_pfsp_tables_from_ptimes({jobs} jobs, {machines} machines) -> {rc}")
     return t
 
 

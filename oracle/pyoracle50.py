@@ -42,6 +42,7 @@ def lib() -> C.CDLL:
             po.build(ref=False)
         L = C.CDLL(path)
         L.or_pfsp_tables_build_variant.argtypes = [C.POINTER(Tables), C.c_int, C.c_int, C.c_int]
+        L.or_pfsp_tables_from_ptimes.argtypes = [C.POINTER(Tables), C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
         L.or_pfsp_evaluate.argtypes = [C.POINTER(Tables), C.c_int, C.c_void_p, C.c_int, C.c_int64, C.c_void_p]
         L.or_taillard_best_ub.restype = C.c_int64
         _lib = L
@@ -54,6 +55,11 @@ def tables(inst: int, heads_mode: int = 0, variant: int = 0) -> Tables:
     if rc != 0:
         raise ValueError(f"or_pfsp_tables_build({inst}) -> {rc}")
     return t
+
+
+def tables_from_ptimes(p_times, heads_mode: int = 0, variant: int = 0) -> Tables:
+    """the tables fill_* build from a processing-time matrix p_times[machines, 50] (any values)"""
+    return po.tables_from_ptimes(p_times, heads_mode, variant, L=lib(), cls=Tables)
 
 
 def pfsp_evaluate(t: Tables, lb_kind: int, parents: np.ndarray, best: int, fill: int = -0x32323233) -> np.ndarray:

@@ -195,19 +195,29 @@ static void fill_johnson_schedules(or_pfsp_tables* t) {
   }
 }
 
-/* pfsp_chpl.chpl:31-38 (module-scope table construction) */
-int or_pfsp_tables_build_variant(or_pfsp_tables* t, int inst, int heads_mode, int variant) {
-  if (inst < 1 || inst > 120) return -1;
+/* the fill_* precompute of pfsp_chpl.chpl:31-38 on any machine-major processing-time matrix p_times[k*jobs + j] */
+int or_pfsp_tables_from_ptimes(or_pfsp_tables* t, int jobs, int machines, const int32_t* p_times, int heads_mode,
+                               int variant) {
+  if (jobs < 1 || jobs > OR_MAX_JOBS || machines < 1 || machines > OR_MAX_MACHINES) return -2;
   memset(t, 0, sizeof(*t));
-  t->jobs = or_taillard_nb_jobs(inst);
-  t->machines = or_taillard_nb_machines(inst);
-  if (t->jobs > OR_MAX_JOBS) return -2; /* MAX_JOBS (20: only ta001..ta030, SURVEY A.2; 50: up to ta060) */
-  or_taillard_processing_times(t->p_times, inst);
+  t->jobs = jobs;
+  t->machines = machines;
+  memcpy(t->p_times, p_times, (size_t)jobs * machines * sizeof(int32_t));
   fill_min_heads_tails(t, heads_mode);
   fill_machine_pairs(t, variant);
   fill_lags(t);
   fill_johnson_schedules(t);
   return 0;
+}
+
+/* pfsp_chpl.chpl:31-38 (module-scope table construction) */
+int or_pfsp_tables_build_variant(or_pfsp_tables* t, int inst, int heads_mode, int variant) {
+  if (inst < 1 || inst > 120) return -1;
+  const int jobs = or_taillard_nb_jobs(inst), machines = or_taillard_nb_machines(inst);
+  if (jobs > OR_MAX_JOBS) return -2; /* MAX_JOBS (20: only ta001..ta030, SURVEY A.2; 50: up to ta060) */
+  int32_t p_times[OR_MAX_MACHINES * OR_MAX_JOBS];
+  or_taillard_processing_times(p_times, inst);
+  return or_pfsp_tables_from_ptimes(t, jobs, machines, p_times, heads_mode, variant);
 }
 int or_pfsp_tables_build(or_pfsp_tables* t, int inst, int heads_mode) {
   return or_pfsp_tables_build_variant(t, inst, heads_mode, 0);

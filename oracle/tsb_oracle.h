@@ -67,6 +67,10 @@ int or_pfsp_tables_build(or_pfsp_tables* t, int inst, int heads_mode);
  * (all pairs, what the reference compiles), 1 LB2_NABESHIMA (adjacent machines), 2 LB2_LAGEWEG (each machine with
  * the last one) */
 int or_pfsp_tables_build_variant(or_pfsp_tables* t, int inst, int heads_mode, int variant);
+/* the same precompute on a given machine-major matrix p_times[machines*jobs] (any values, any 1..OR_MAX_JOBS jobs
+ * and 1..OR_MAX_MACHINES machines): 0, or -2 for dimensions out of range */
+int or_pfsp_tables_from_ptimes(or_pfsp_tables* t, int jobs, int machines, const int32_t* p_times, int heads_mode,
+                               int variant);
 
 /* ---- bounds ---- */
 int32_t or_eval_solution(const or_pfsp_tables* t, const int32_t* prmu);

@@ -54,15 +54,21 @@ def check_nq(ev, parents, N):
     return got
 
 
+def copy_tables(src, cls):
+    """the same PFSP tables in another ctypes mirror of the layout: oracle Tables <-> tsb200.PfspTables (20 jobs),
+    pyoracle50.Tables <-> tsb200.PfspTables50"""
+    t = cls()
+    for name in ("jobs", "machines", "pairs"):
+        setattr(t, name, getattr(src, name))
+    for name in ("p_times", "min_heads", "min_tails", "johnson", "lags", "mp0", "mp1", "mp_order"):
+        np.ctypeslib.as_array(getattr(t, name))[:] = np.ctypeslib.as_array(getattr(src, name))
+    return t
+
+
 def check_pfsp(ev, parents, lb, best):
     jobs = ev.jobs
     got = ev.evaluate(parents, lb, best).reshape(-1, jobs)
-    t = po.Tables()
-    # the oracle gets the very same tables the device got (tables are an input of the kernels)
-    for name in ("jobs", "machines", "pairs"):
-        setattr(t, name, getattr(ev.tables, name))
-    for name in ("p_times", "min_heads", "min_tails", "johnson", "lags", "mp0", "mp1", "mp_order"):
-        np.ctypeslib.as_array(getattr(t, name))[:] = np.ctypeslib.as_array(getattr(ev.tables, name))
+    t = copy_tables(ev.tables, po.Tables)  # the oracle gets the very same tables the device got (an input of the kernels)
     kind = tsb200.LB_NAMES[lb]
     want = po.pfsp_evaluate(t, kind, parents.view(po.PFSP_NODE_DTYPE), best).reshape(-1, jobs)
     live = po.pfsp_live_mask(parents.view(po.PFSP_NODE_DTYPE), jobs)

@@ -254,3 +254,90 @@ def test_max_jobs_50_oracle_matches_reference(golden_dir, inst):
     np.testing.assert_array_equal(po50.pfsp_evaluate(t, 0, parents, best), gold[f"{tag}_lb1_d"])
     np.testing.assert_array_equal(po50.pfsp_evaluate(t, 2, parents, best), gold[f"{tag}_lb2_best"])
     np.testing.assert_array_equal(po50.pfsp_evaluate(t, 2, parents, INT_MAX), gold[f"{tag}_lb2_inf"])
+
+
+# ------------------------------------------------------------------------------------------ synthetic shapes
+# tests/golden/pfsp_shapes.npz (tests/golden/make_golden_shapes.py): the reference's tables and bounds for synthetic
+# processing-time matrices on 1..20 machines, in value classes that each select one kernel route of the device library
+SHAPES = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pfsp_shapes.npz")
+SHAPE_TAGS = [str(x) for x in np.load(SHAPES)["tags"]]
+
+
+def shape_tables(gold, tag, heads_mode=0):
+    """oracle tables of fixture instance `tag` from its processing times (with its overwritten min_tails, if any)"""
+    from oracle import pyoracle50 as po50
+    jobs, machines, _ = (int(x) for x in gold[f"{tag}_dims"])
+    mod = po50 if jobs > po.MAX_JOBS else po
+    t = mod.tables_from_ptimes(gold[f"{tag}_p_times"].reshape(machines, jobs), heads_mode)
+    if gold[f"{tag}_tails_set"][0]:
+        np.ctypeslib.as_array(t.min_tails)[:machines] = gold[f"{tag}_min_tails"]
+    return t
+
+
+def shape_parents(gold, tag):
+    from oracle import pyoracle50 as po50
+    jobs = int(gold[f"{tag}_dims"][0])
+    return gold[f"{tag}_parents"].view(po50.PFSP_NODE_DTYPE if jobs > po.MAX_JOBS else po.PFSP_NODE_DTYPE)
+
+
+def shape_evaluate(t, kind, parents, best):
+    """the oracle's bounds on the live slots (k >= limit1 + 1, row-major), the layout of the fixture"""
+    from oracle import pyoracle50 as po50
+    mod = po50 if t.jobs > po.MAX_JOBS else po
+    got = mod.pfsp_evaluate(t, kind, parents, best).reshape(-1, t.jobs)
+    return got[mod.pfsp_live_mask(parents, t.jobs)]
+
+
+@pytest.fixture(scope="module")
+def shapes():
+    return np.load(SHAPES)
+
+
+@pytest.mark.parametrize("tag", SHAPE_TAGS)
+def test_tables_from_ptimes_match_reference(shapes, tag):
+    """or_pfsp_tables_from_ptimes runs the same fill_* as the reference on any matrix (C min_heads semantics with
+    heads_mode 1, the Chapel statement with heads_mode 0)"""
+    g = shapes
+    jobs, machines, pairs = (int(x) for x in g[f"{tag}_dims"])
+    t = shape_tables(g, tag, heads_mode=1)
+    assert (t.jobs, t.machines, t.pairs) == (jobs, machines, pairs)
+    np.testing.assert_array_equal(t.arr("p_times", jobs * machines), g[f"{tag}_p_times"])
+    np.testing.assert_array_equal(t.arr("min_heads", machines), g[f"{tag}_min_heads_C"])
+    np.testing.assert_array_equal(t.arr("min_tails", machines), g[f"{tag}_min_tails"])
+    np.testing.assert_array_equal(t.arr("lags", pairs * jobs), g[f"{tag}_lags"])
+    np.testing.assert_array_equal(t.arr("mp0", pairs), g[f"{tag}_mp0"])
+    np.testing.assert_array_equal(t.arr("mp1", pairs), g[f"{tag}_mp1"])
+    if f"{tag}_min_heads_chapel" in g:
+        np.testing.assert_array_equal(shape_tables(g, tag, 0).arr("min_heads", machines), g[f"{tag}_min_heads_chapel"])
+    # Johnson order: a permutation per pair, sorted by the reference's key (ties may permute)
+    ours = t.arr("johnson", pairs * jobs).reshape(pairs, jobs)
+    ref = g[f"{tag}_johnson_qsort"].reshape(pairs, jobs)
+    p = g[f"{tag}_p_times"].reshape(machines, jobs).astype(np.int64)
+    lags = g[f"{tag}_lags"].reshape(pairs, jobs).astype(np.int64)
+    for k in range(pairs):
+        assert sorted(ours[k]) == list(range(jobs))
+        a = p[g[f"{tag}_mp0"][k]] + lags[k]
+        b = p[g[f"{tag}_mp1"][k]] + lags[k]
+        key = lambda j: (0, a[j]) if a[j] < b[j] else (1, -b[j])  # noqa: E731
+        assert [key(j) for j in ours[k]] == [key(j) for j in ref[k]]
+
+
+@pytest.mark.parametrize("tag", SHAPE_TAGS)
+def test_bounds_from_ptimes_match_reference(shapes, tag):
+    """the oracle's lb1 / lb1_d / lb2 (every incumbent of the fixture) on these tables = the reference's, and lb1_d of
+    the root with the Chapel min_heads = the reference built with the Chapel statement"""
+    g = shapes
+    parents = shape_parents(g, tag)
+    for heads_mode in (0, 1):  # min_heads is never read when limit1 >= 0
+        t = shape_tables(g, tag, heads_mode)
+        np.testing.assert_array_equal(shape_evaluate(t, 1, parents, INT_MAX), g[f"{tag}_lb1"])
+        np.testing.assert_array_equal(shape_evaluate(t, 0, parents, INT_MAX), g[f"{tag}_lb1_d"])
+        for i, best in enumerate(g[f"{tag}_lb2_bests"] if t.pairs else ()):
+            np.testing.assert_array_equal(shape_evaluate(t, 2, parents, int(best)), g[f"{tag}_lb2"][i],
+                                          err_msg=f"lb2 best={best}")
+    if f"{tag}_root_lb1_d" in g:
+        t = shape_tables(g, tag, 0)
+        root = np.zeros(1, dtype=po.PFSP_NODE_DTYPE)
+        root["limit1"] = -1
+        root["prmu"][0, : t.jobs] = np.arange(t.jobs)
+        np.testing.assert_array_equal(shape_evaluate(t, 0, root, INT_MAX), g[f"{tag}_root_lb1_d"])
