@@ -5,12 +5,18 @@
 // most of a round is spent waiting on them.  Here the pool lives, while the kernel runs, in a SELF-VALIDATING format
 // (the "LL" idea of NCCL's low-latency protocol):
 //
-//   fat node = 8 x 8-byte words; word i = data32[i] | epoch << 32            (64 B per node, 16-byte aligned)
-//   data32[0..5] = the 21 node bytes (depth, board[0..19]),  data32[6..7] = the node's aux word (nq_rounds.cuh:
-//   diagonal masks, child mask, leaf flag)
+//   fat node = 4 x 8-byte words; word i = data32[i] | epoch << 32     (32 B per node = one sector, 32-byte aligned)
+//   data32[0..3] = the node packed in 125 bits (any N <= 20: every board value is below 32):
+//     board[i] in bits 5 (i % 6) .. +4 of data32[i / 6]            (six values per word; board[18], [19] in data32[3])
+//     depth in the 2-bit tails (bits 30..31) of data32[0], [1], [2]: bits 0-1, 2-3 and 4 of the depth
+//     data32[3] bits 10..29: the node's child mask (slot k set <=> k >= depth and board[k] is not attacked: evaluate_gpu's
+//     label for slot k, nqueens_gpu_chpl.chpl:97-123), bit 30: leaf (depth == N)
+//   The diagonal masks of a parent (what its next row attacks) are not stored: a round recomputes them from the placed
+//   prefix, O(depth), for the parents that have children, while the child counts are on their way; a child's masks
+//   follow from its parent's in O(1) as in nq_rounds.cuh, and its child mask is evaluated when it is built.
 //
 // Every 8-byte word is written by one store (an element of a st.v2.u64) and is therefore seen whole or not at all;
-// a reader that expects the children of round r polls the words of its slice until all eight carry r's epoch.  No
+// a reader that expects the children of round r polls the words of its slice until all four carry r's epoch.  No
 // fence, no "done" flags: the data is its own flag, and a round costs ONE flag exchange (the child counts) plus one
 // store -> L2 -> poll hop for the nodes.  Epochs are 32 bits and never repeat, so stale words cannot alias.
 //
@@ -49,15 +55,29 @@ constexpr int LL_T = 256;                    // threads per CTA
 __host__ __device__ constexpr int ll_slice(int ppt) { return LL_T * ppt; }          // parents per CTA per round
 static_assert(ll_slice(2) == LL_SLICE2 && ll_slice(3) == LL_SLICE3 && RND_MAX_CTAS == LL_MAX_SMS, "ll_tiers.h");
 // children per window of the staging buffer (a CTA's share of a round averages ~0.8 children per parent; a dense
-// share takes several windows); 512 in the three-CTAs-per-SM build (MINB = 3: 64 KB of shared memory per CTA)
-__host__ __device__ constexpr int ll_cap(int ppt, int minb) { return minb >= 3 ? 512 : ppt <= 2 ? 2048 : 1024; }
-constexpr int LL_WORDS = 8;                  // 8-byte words per fat node
+// share takes several windows)
+constexpr int LL_CAP = 2048;
+constexpr int LL_WORDS = 4;                  // 8-byte words per fat node
 constexpr int LL_LAYERS = 1024;              // layers of the pool a CTA tracks (more: the kernel leaves and is relaunched)
 constexpr unsigned LL_TRUSTED = 0u;          // layer epoch of the nodes that were in the pool at launch (epochs start at 1)
 
-struct FatNode {
+struct alignas(32) FatNode {
   unsigned long long w[LL_WORDS];
 };
+// the packed node (data32[0..3], see above)
+constexpr int LL_CM_SHIFT = 10;          // child mask: data32[3] bits 10..29
+constexpr uint32_t LL_LEAF = 1u << 30;   // leaf flag: data32[3] bit 30
+__host__ __device__ constexpr int ll_fw(int i) { return i / 6; }        // data word of board[i]
+__host__ __device__ constexpr int ll_fs(int i) { return 5 * (i % 6); }  // its first bit
+__device__ __forceinline__ uint32_t ll_depth(uint32_t d0, uint32_t d1, uint32_t d2) {
+  return d0 >> 30 | (d1 >> 30) << 2 | (d2 >> 30) << 4;
+}
+// data32[0..2] with their depth tails replaced by those of `depth`
+__device__ __forceinline__ void ll_set_depth(uint32_t (&d)[4], uint32_t depth) {
+  d[0] = (d[0] & 0x3FFFFFFFu) | (depth & 3u) << 30;
+  d[1] = (d[1] & 0x3FFFFFFFu) | (depth >> 2 & 3u) << 30;
+  d[2] = (d[2] & 0x3FFFFFFFu) | (depth >> 4) << 30;
+}
 struct LlSync {
   unsigned long long slot[2][2 * RND_MAX_CTAS];  // by round parity, one per SUB-slice: epoch << 32 | leaves << 20 | children
   unsigned abort;
@@ -103,18 +123,20 @@ __device__ __forceinline__ void st_fat2(unsigned long long* p, unsigned long lon
   asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(p), "l"(a), "l"(b));
 }
 
-// ---- plain arena <-> fat arena (one thread per node; not performance critical: the whole pool, once per hand-over)
+// ---- plain arena <-> fat arena (one thread per node; not performance critical: the whole pool, once per hand-over).
+// Byte for byte for every node tsb_nq_pool_push admits (depth <= N, board[0..N) < N, bytes past N zero), which
+// are the only nodes a pool holds.
 template <int N>
 __global__ void nq_fat_import_kernel(const uint8_t* __restrict__ arena, FatNode* __restrict__ fat, long long size,
                                      unsigned epoch) {
   const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (p >= size) return;
   const uint8_t* node = arena + p * NQ_REC;
-  uint32_t d[LL_WORDS] = {0, 0, 0, 0, 0, 0, 0, 0};
-  for (int i = 0; i < NQ_REC; i++) d[i >> 2] |= static_cast<uint32_t>(node[i]) << (8 * (i & 3));
+  uint32_t d[LL_WORDS] = {0, 0, 0, 0};
+  for (int i = 0; i < NQ_REC - 1; i++) d[ll_fw(i)] |= static_cast<uint32_t>(node[1 + i]) << ll_fs(i);
+  ll_set_depth(d, node[0]);
   const unsigned long long aux = nq_aux_of_node<N>(node);
-  d[6] = static_cast<uint32_t>(aux);
-  d[7] = static_cast<uint32_t>(aux >> 32);
+  d[3] |= (static_cast<uint32_t>(aux >> 40) & 0xFFFFFu) << LL_CM_SHIFT | ((aux >> 60) & 1u ? LL_LEAF : 0u);
   const unsigned long long e = static_cast<unsigned long long>(epoch) << 32;
   for (int i = 0; i < LL_WORDS; i += 2) st_fat2(&fat[p].w[i], d[i] | e, d[i + 1] | e);
 }
@@ -122,10 +144,10 @@ __global__ void nq_fat_export_kernel(const FatNode* __restrict__ fat, uint8_t* _
   const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (p >= size) return;
   uint8_t* node = arena + p * NQ_REC;
-  for (int i = 0; i < 6; i++) {
-    const uint32_t d = static_cast<uint32_t>(fat[p].w[i]);
-    for (int b = 0; b < 4 && 4 * i + b < NQ_REC; b++) node[4 * i + b] = static_cast<uint8_t>(d >> (8 * b));
-  }
+  uint32_t d[LL_WORDS];
+  for (int i = 0; i < LL_WORDS; i++) d[i] = static_cast<uint32_t>(fat[p].w[i]);
+  node[0] = static_cast<uint8_t>(ll_depth(d[0], d[1], d[2]));
+  for (int i = 0; i < NQ_REC - 1; i++) node[1 + i] = static_cast<uint8_t>(d[ll_fw(i)] >> ll_fs(i) & 31u);
 }
 
 // warp 0: until all n slots carry `epoch`; sums of {leaves << 32 | children} over all slots and over the slots
@@ -163,62 +185,85 @@ __device__ __forceinline__ bool warp_gather_slots2(const unsigned long long* slo
   return true;
 }
 
-template <int T, int PPT, int MINB>
+template <int T, int PPT>
 struct LlSmem {
-  alignas(16) uint32_t parent[T * PPT][8];           // the slice: data32[0..7] of every parent
-  alignas(16) uint32_t stage[ll_cap(PPT, MINB)][8];  // the window's children: data32[0..7]
-  alignas(16) uint16_t item[T * PPT * 20];     // (record << 5) | slot, in child order
+  alignas(16) uint4 parent[T * PPT];   // the slice: data32[0..3] of every parent
+  alignas(16) uint4 stage[LL_CAP];     // the window's children: data32[0..3]
+  alignas(8) uint2 diag[T * PPT];      // {ld, rd} of every parent that has children (ll_parent_diag)
+  alignas(16) uint16_t item[T * PPT * 20];  // (record << 5) | slot, in child order
   unsigned long long warp_tot64[T / 32];
   unsigned long long red[3];
+  long long prof[8], prof_t;       // (prm.prof, CTA 0) cycles per phase, clock at the end of the last one
   long long lay_start[LL_LAYERS];  // the pool's layers, bottom to top: first position ...
   unsigned lay_epoch[LL_LAYERS];   // ... and the epoch its nodes were stored with (LL_TRUSTED: before the launch)
 };
 
-// child `item` of the slice (pure data: no alignment games in the fat format) -> its eight data words
+// the values a parent's next row (row `depth`) attacks along the rising (ld) and falling (rd) diagonals of its placed
+// rows 0 .. depth-1: every row's queen moves one value further per row, as ll_build_child moves its parent's masks
 template <int N>
-__device__ __forceinline__ void ll_build_child(const uint32_t (*parent)[8], int item, uint32_t (&c)[8]) {
-  const int r = item >> 5, k = item & 31;
-  const uint4 lo = *reinterpret_cast<const uint4*>(parent[r]), hi = *reinterpret_cast<const uint4*>(parent[r] + 4);
-  uint32_t P[6] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y & 0xFFu};
-  const uint32_t depth = P[0] & 0xFFu;
-  const uint32_t p1 = 1u + depth, p2 = 1u + static_cast<uint32_t>(k);
-  const uint8_t* pb = reinterpret_cast<const uint8_t*>(parent[r]);
-  const uint32_t v = pb[p2];  // the queen placed on row `depth`
-  const uint32_t D = static_cast<uint32_t>(pb[p1]) ^ v;
-  const uint32_t x1 = D << ((p1 & 3u) * 8u), x2 = D << ((p2 & 3u) * 8u);
-  const uint32_t w1 = p1 >> 2, w2 = p2 >> 2;
+__device__ __forceinline__ uint2 ll_parent_diag(const uint4 p) {
+  const uint32_t P[4] = {p.x, p.y, p.z, p.w};
+  const uint32_t depth = ll_depth(p.x, p.y, p.z);
+  uint32_t ld = 0, rd = 0;
 #pragma unroll
-  for (uint32_t j = 0; j < 6; j++) P[j] ^= (j == w1 ? x1 : 0u) ^ (j == w2 ? x2 : 0u);
-  P[0] += 1u;  // depth + 1
-  const unsigned long long w = static_cast<unsigned long long>(hi.z) | static_cast<unsigned long long>(hi.w) << 32;
-  const uint32_t ld = static_cast<uint32_t>(w) & 0xFFFFFu, rd = static_cast<uint32_t>(w >> 20) & 0xFFFFFu;
-  const uint32_t bit = 1u << (v & 31u);
-  const uint32_t ld2 = ((ld | bit) << 1) & ((1u << N) - 1u), rd2 = (rd | bit) >> 1;
-  NqParent<N, 0, 0> cp;
-  cp.init(P);  // depth + 1, shift amounts = the child's board
-  cp.U = ld2 | rd2;
-  const uint32_t cm = nq_child_mask<N, 0>(cp);  // slots >= depth + 1 whose value is safe (none for a leaf)
-  const unsigned long long ca = nq_aux_pack(ld2, rd2, cm, depth + 1u == static_cast<uint32_t>(N));
+  for (int i = 0; i < N; i++)
+    if (i < depth) {
+      const uint32_t bit = 1u << (P[ll_fw(i)] >> ll_fs(i) & 31u);
+      ld = ((ld | bit) << 1) & ((1u << N) - 1u);
+      rd = (rd | bit) >> 1;
+    }
+  return make_uint2(ld, rd);
+}
+
+// child `item` of the slice -> its four data words: board[depth] and board[k] swapped, depth + 1, its masks from the
+// parent's, its child mask evaluated here
+template <int N>
+__device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2* diag, int item) {
+  const int r = item >> 5;
+  const uint32_t k = static_cast<uint32_t>(item & 31);
+  const uint4 p = parent[r];
+  uint32_t P[4] = {p.x, p.y, p.z, p.w};
+  const uint32_t depth = ll_depth(p.x, p.y, p.z);
+  const auto word = [&](uint32_t w) { return w == 0 ? P[0] : w == 1 ? P[1] : w == 2 ? P[2] : P[3]; };
+  const uint32_t wd = depth / 6u, sd = 5u * (depth - 6u * wd), wk = k / 6u, sk = 5u * (k - 6u * wk);
+  const uint32_t v = word(wk) >> sk & 31u;  // the queen placed on row `depth`
+  const uint32_t D = (word(wd) >> sd & 31u) ^ v;
 #pragma unroll
-  for (int j = 0; j < 6; j++) c[j] = P[j];
-  c[6] = static_cast<uint32_t>(ca);
-  c[7] = static_cast<uint32_t>(ca >> 32);
+  for (uint32_t j = 0; j < 4; j++) P[j] ^= (j == wd ? D << sd : 0u) ^ (j == wk ? D << sk : 0u);
+  const uint32_t cd = depth + 1u;
+  ll_set_depth(P, cd);
+  const uint2 pd = diag[r];
+  const uint32_t bit = 1u << v;
+  const uint32_t S = ~((((pd.x | bit) << 1) & ((1u << N) - 1u)) | ((pd.y | bit) >> 1));  // safe values of row cd
+  uint32_t cm = 0;
+#pragma unroll
+  for (int i = 0; i < N; i++) {
+    const uint32_t x = shf_r_wrap(S, 0u, P[ll_fw(i)] >> ll_fs(i)) & 1u;  // bit board[i] of S (the shift wraps mod 32)
+    asm("mad.lo.u32 %0, %1, %2, %0;" : "+r"(cm) : "r"(x), "r"(1u << i));  // cm |= x << i on the FMA pipe
+  }
+  cm &= shl_clamp(0xFFFFFFFFu, cd);  // only slots i >= depth + 1 exist (none for a leaf)
+  P[3] = (P[3] & 0x3FFu) | cm << LL_CM_SHIFT | (cd == static_cast<uint32_t>(N) ? LL_LEAF : 0u);
+  return make_uint4(P[0], P[1], P[2], P[3]);
 }
 
 template <int N, int T, int MINB, int PPT>
 __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_constant__ LlMultiParams mprm) {
   const LlParams& prm = mprm.pool[blockIdx.y];
-  constexpr int LL_PPT = PPT, LL_CAP = ll_cap(PPT, MINB);
+  constexpr int LL_PPT = PPT;
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  LlSmem<T, PPT, MINB>& sm = *reinterpret_cast<LlSmem<T, PPT, MINB>*>(smem_raw);
+  LlSmem<T, PPT>& sm = *reinterpret_cast<LlSmem<T, PPT>*>(smem_raw);
   const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
   const int k = blockIdx.x, G = gridDim.x;
   LlSync* const sy = prm.sync;
   FatNode* const fat = prm.fat;
+  // the profile lives in shared memory, touched by CTA 0's thread 0 only: no per-thread state, nothing when it is off
+  const bool prof_on = prm.prof != 0 && k == 0 && t == 0;
 
   if (t == 0) {
     sm.lay_start[0] = 0;
     sm.lay_epoch[0] = LL_TRUSTED;
+    if (prof_on)
+      for (int i = 0; i < 8; i++) sm.prof[i] = 0;
   }
   __syncthreads();
   int n_lay = prm.size0 > 0 ? 1 : 0;
@@ -228,13 +273,11 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
   unsigned epoch = prm.epoch0;
   unsigned long long rounds = 0, tot_parents = 0, tot_children = 0, tot_solutions = 0;
   int exit_code = RND_EXIT_PAUSE;
-  long long prof[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tp = 0;
-  const bool prof_on = prm.prof != 0 && k == 0 && t == 0;
 #define TSB_PROF(i)                  \
   if (prof_on) {                     \
     const long long now = clock64(); \
-    prof[i] += now - tp;             \
-    tp = now;                        \
+    sm.prof[i] += now - sm.prof_t;   \
+    sm.prof_t = now;                 \
   }
 
   for (long long r = 0;; r++) {
@@ -258,10 +301,10 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
       break;
     }
     ++epoch;
-    if (prof_on) tp = clock64();
+    if (prof_on) sm.prof_t = clock64();
     // my share of the chunk: TWO sub-slices of n / 2G parents — number k from the bottom and number k from the top.
     // The bottom of a chunk holds the shallow nodes (many children), the top the deep ones (few): a single slice per
-    // CTA left the bottom CTA with 3x the average children, and its build + 64-byte stores were the round's
+    // CTA left the bottom CTA with 3x the average children, and its build + node stores were the round's
     // critical path; pairing k with 2G-1-k evens the load without knowing it in advance.
     const int G2 = 2 * G;
     const unsigned n32 = static_cast<unsigned>(n), uG2 = static_cast<unsigned>(G2), uk = static_cast<unsigned>(k);
@@ -273,20 +316,20 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
     bool ok = true;
     TSB_PROF(0)
 
-    // ---- (2) my slice -> shared memory, 16-byte piece by piece (4 pieces per node, consecutive lanes on consecutive
+    // ---- (2) my slice -> shared memory, 16-byte piece by piece (2 pieces per node, consecutive lanes on consecutive
     // pieces: every warp load is 512 contiguous bytes); a piece is polled until both of its words carry the epoch of
     // the layer its node lies in
     {
       SpinGuard guard;
       const unsigned long long* src0 = fat[s0 + a0].w;
-      const unsigned long long* src1 = fat[s0 + a1].w - 8 * len0;  // (indexed by the concatenated piece number)
+      const unsigned long long* src1 = fat[s0 + a1].w - LL_WORDS * len0;  // (indexed by the concatenated piece number)
       const int top = n_lay - 1;
-      constexpr int PCS = 4 * LL_PPT;  // pieces per thread
+      constexpr int PCS = 2 * LL_PPT;  // pieces per thread
       unsigned long long w0[PCS], w1[PCS];
       unsigned pending = 0;
 #pragma unroll
       for (int j = 0; j < PCS; j++)
-        if (t + j * T < 4 * len) pending |= 1u << j;
+        if (t + j * T < 2 * len) pending |= 1u << j;
       // the epoch node i of my slice was stored with: that of the layer its position lies in (mostly the top one)
       const auto want_of = [&](int i) {
         const long long pos = s0 + (i < len0 ? a0 + i : a1 + (i - len0));
@@ -300,15 +343,15 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
         for (int j = 0; j < PCS; j++)
           if (pending & (1u << j)) {
             const int pc = t + j * T;
-            ld_fat2((pc < 4 * len0 ? src0 : src1) + 2 * pc, w0[j], w1[j]);
+            ld_fat2((pc < 2 * len0 ? src0 : src1) + 2 * pc, w0[j], w1[j]);
           }
 #pragma unroll
         for (int j = 0; j < PCS; j++)
           if (pending & (1u << j)) {
-            const int pc = t + j * T, i = pc >> 2;
+            const int pc = t + j * T, i = pc >> 1;
             const unsigned want = want_of(i);
             if (want == LL_TRUSTED || (static_cast<unsigned>(w0[j] >> 32) == want && static_cast<unsigned>(w1[j] >> 32) == want)) {
-              *reinterpret_cast<uint2*>(&sm.parent[i][2 * (pc & 3)]) =
+              reinterpret_cast<uint2*>(&sm.parent[i])[pc & 1] =
                   make_uint2(static_cast<uint32_t>(w0[j]), static_cast<uint32_t>(w1[j]));
               pending &= ~(1u << j);
             }
@@ -330,10 +373,9 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
       const int i = LL_PPT * t + q;
       cm[q] = 0;
       if (i < len) {
-        const uint2 ax = *reinterpret_cast<const uint2*>(&sm.parent[i][6]);
-        const unsigned long long aux = static_cast<unsigned long long>(ax.x) | static_cast<unsigned long long>(ax.y) << 32;
-        cm[q] = static_cast<uint32_t>(aux >> 40) & 0xFFFFFu;
-        leaves += static_cast<int>(aux >> 60) & 1;
+        const uint32_t w3 = sm.parent[i].w;
+        cm[q] = w3 >> LL_CM_SHIFT & 0xFFFFFu;
+        leaves += (w3 & LL_LEAF) ? 1 : 0;
         mine += __popc(cm[q]);
         if (i < len0) mine0 += __popc(cm[q]);
       }
@@ -376,17 +418,15 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
         }
       }
     }
-    ll_bar(T);  // items complete
+    // ---- (5) the diagonals of my parents that have children (the counts are on their way meanwhile)
+#pragma unroll
+    for (int q = 0; q < LL_PPT; q++)
+      if (cm[q]) sm.diag[LL_PPT * t + q] = ll_parent_diag<N>(sm.parent[LL_PPT * t + q]);
+    ll_bar(T);  // items and diagonals complete
     TSB_PROF(2)
-    // ---- (5) my children (first window), built and evaluated while the other CTAs' counts are on their way
+    // ---- (5b) my children (first window), built and evaluated while the other CTAs' counts are on their way
     auto build_window = [&](int c0, int cnt) {
-      for (int c = t; c < cnt; c += T) {
-        uint32_t ch[8];
-        ll_build_child<N>(sm.parent, sm.item[c0 + c], ch);
-        uint4* dst = reinterpret_cast<uint4*>(sm.stage[c]);
-        dst[0] = make_uint4(ch[0], ch[1], ch[2], ch[3]);
-        dst[1] = make_uint4(ch[4], ch[5], ch[6], ch[7]);
-      }
+      for (int c = t; c < cnt; c += T) sm.stage[c] = ll_build_child<N>(sm.parent, sm.diag, sm.item[c0 + c]);
     };
     build_window(0, min(LL_CAP, my_children));
     TSB_PROF(6)
@@ -424,18 +464,18 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
       // child c of my share goes to position s0 + off0 + c (bottom sub-slice) or s0 + off1 + (c - cnt0) (top one)
       unsigned long long* const dst0 = fat[s0 + off0 + c0].w;
       unsigned long long* const dst1 = fat[s0 + off1 + c0 - cnt0].w;
-      const int npc = 4 * cnt;  // 16-byte pieces, consecutive lanes on consecutive pieces, four in flight per thread
+      const int npc = 2 * cnt;  // 16-byte pieces, consecutive lanes on consecutive pieces, four in flight per thread
       for (int pc = t; pc < npc; pc += 4 * T) {
         uint2 d[4];
 #pragma unroll
         for (int u = 0; u < 4; u++) {
           const int x = min(pc + u * T, npc - 1);
-          d[u] = *reinterpret_cast<const uint2*>(&sm.stage[x >> 2][2 * (x & 3)]);
+          d[u] = reinterpret_cast<const uint2*>(&sm.stage[x >> 1])[x & 1];
         }
 #pragma unroll
         for (int u = 0; u < 4; u++) {
           const int x = pc + u * T;
-          if (x < npc) st_fat2((c0 + (x >> 2) < cnt0 ? dst0 : dst1) + 2 * x, d[u].x | tag, d[u].y | tag);
+          if (x < npc) st_fat2((c0 + (x >> 1) < cnt0 ? dst0 : dst1) + 2 * x, d[u].x | tag, d[u].y | tag);
         }
       }
     }
@@ -473,8 +513,8 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
     st->children = tot_children;
     st->solutions = tot_solutions;
     st->exit_code = exit_code;
-    if (prm.prof)
-      for (int i = 0; i < 8; i++) st->prof[i] = prof[i];
+    if (prof_on)
+      for (int i = 0; i < 8; i++) st->prof[i] = sm.prof[i];
   }
 #undef TSB_PROF
 }

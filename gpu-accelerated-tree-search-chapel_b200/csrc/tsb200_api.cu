@@ -491,13 +491,12 @@ struct RoundsCtx {
   int ctas = 0;       // CTAs per pool (env TSB200_ROUNDS_CTAS; 0 = nq_ll_grid's measured defaults: an all-to-all flag
                       // exchange among all SMs' CTAs costs 2-3x one among half of them (tools/flag_exchange.py), the per-CTA work
                       // grows the other way)
-  int occ = 2;        // env TSB200_ROUNDS_OCC=3: three CTAs per SM (several pools per launch)
   int ppt = 0;        // env TSB200_ROUNDS_PPT=3: the 768-parent slices also where 512 would do (experiments)
   int version = 3;    // 3 = the fence-free kernel on the fat arena (nq_rounds_ll.cuh); 2 = nq_rounds.cuh (env TSB200_ROUNDS_V)
-  tsb::FatNode* d_fat = nullptr;  // the pool in the self-validating 64-byte format, while the LL kernel owns it
+  tsb::FatNode* d_fat = nullptr;  // the pool in the self-validating 32-byte format, while the LL kernel owns it
   long long fat_cap = 0;
   bool in_fat = false;            // the pool currently lives in d_fat (the plain arena is stale)
-  bool attr_llv[4] = {false, false, false, false};
+  bool attr_llv[3] = {false, false, false};
   tsb::LlSync* d_ll = nullptr;
   int ensure_fat(long long cap, cudaStream_t s) {
     if (!d_ll) {
@@ -530,7 +529,6 @@ struct RoundsCtx {
     }
     if (const char* v = std::getenv("TSB200_ROUNDS_CTAS")) ctas = std::max(1, std::atoi(v));
     if (const char* v = std::getenv("TSB200_ROUNDS_PPT")) ppt = std::atoi(v) == 3 ? 3 : 0;
-    if (const char* v = std::getenv("TSB200_ROUNDS_OCC")) occ = std::atoi(v) == 3 ? 3 : 2;
     if (const char* v = std::getenv("TSB200_ROUNDS_V")) version = std::atoi(v) == 2 ? 2 : 3;
   }
   int ensure(cudaStream_t s) {
@@ -1340,11 +1338,23 @@ int nq_aux_ensure(tsb_nq* h) {
   h->aux_ok = true;
   return TSB_OK;
 }
+// what a pool may hold: depth <= N, board[0..N) < N, the bytes past N zero (every node the reference or this library
+// creates; the persistent kernel packs a node into 125 bits on these terms, nq_rounds_ll.cuh)
+bool nq_nodes_valid(int N, const tsb_nq_node* nodes, int64_t n) {
+  for (int64_t i = 0; i < n; i++) {
+    const tsb_nq_node& x = nodes[i];
+    if (x.depth > N) return false;
+    for (int j = 0; j < TSB_MAX_QUEENS; j++)
+      if (x.board[j] >= (j < N ? N : 1)) return false;
+  }
+  return true;
+}
 }  // namespace
 extern "C" {
 
 int tsb_nq_pool_push(tsb_nq* h, const void* nodes, int64_t n) {
   if (!h || n < 0 || (n && !nodes)) return TSB_EINVAL;
+  if (!nq_nodes_valid(h->N, static_cast<const tsb_nq_node*>(nodes), n)) return TSB_EINVAL;
   TSB_CUDA(cudaSetDevice(h->device));
   nq_pool_setup(h);
   int rc = nq_materialize(h);
@@ -1451,17 +1461,12 @@ int nq_rounds_launch(tsb_nq* h, const tsb::RoundsParams& prm, int grid, cudaStre
 template <int N>
 int nq_ll_launch_n(tsb_nq* h, const tsb::LlMultiParams& prm, int grid, int pools, int ppt, cudaStream_t s) {
   // (one pool: the 160-register build, one CTA per SM; several: capped at 128 registers for two CTAs per SM; three
-  // or four pools: 74 CTAs per pool with 768 parents each, see ll_slice)
-  // ppt > 10: the three-CTAs-per-SM build (80 registers, 64 KB of shared memory) with ppt - 10 parents per thread
-  const int var = pools == 1 ? 0 : ppt == 2 ? 1 : ppt == 3 ? 2 : 3;
+  // or four pools: 66 CTAs per pool with 768 parents each on 132 SMs, see ll_slice)
+  const int var = pools == 1 ? 0 : ppt == 2 ? 1 : 2;
   auto kernel = var == 0   ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 2>
                 : var == 1 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 2>
-                : var == 2 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 3>
-                           : tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 3, 2>;
-  const size_t smem = (var == 0   ? sizeof(tsb::LlSmem<tsb::LL_T, 2, 1>)
-                       : var == 1 ? sizeof(tsb::LlSmem<tsb::LL_T, 2, 2>)
-                       : var == 2 ? sizeof(tsb::LlSmem<tsb::LL_T, 3, 2>)
-                                  : sizeof(tsb::LlSmem<tsb::LL_T, 2, 3>)) + 128;
+                           : tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 3>;
+  const size_t smem = (ppt == 2 ? sizeof(tsb::LlSmem<tsb::LL_T, 2>) : sizeof(tsb::LlSmem<tsb::LL_T, 3>)) + 128;
   bool& attr = h->rounds.attr_llv[var];
   if (!attr) {
     TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
@@ -1539,17 +1544,11 @@ int nq_ll_grid(const tsb_nq* h, int M, int pools, int* ppt = nullptr) {
   int most = tsb::ll_ctas_per_pool(sms, pools);  // (ll_tiers.h: the drivers size their warm-up by the same tiers)
   int per = static_cast<long long>(most) * tsb::ll_slice(2) >= M ? 2 : 3;
   if (pools > 1 && h->rounds.ppt == 3) per = 3;
-  bool occ3 = false;
-  if (pools > 1 && h->rounds.occ == 3 && static_cast<long long>(3 * sms / pools) * tsb::ll_slice(2) >= M) {
-    most = 3 * sms / pools;  // three CTAs per SM in all, 512 parents per CTA
-    per = 2;
-    occ3 = true;
-  }
   const int slice = tsb::ll_slice(per);
   int grid = pools == 1 ? std::max(1, (sms * 7 / 8) & ~1) : most;
   if (h->rounds.ctas > 0) grid = std::min(most, h->rounds.ctas);
   while (static_cast<long long>(grid) * slice < M && grid < most) ++grid;  // (M decides)
-  if (ppt) *ppt = occ3 ? 12 : per;
+  if (ppt) *ppt = per;
   return static_cast<long long>(M) <= static_cast<long long>(grid) * slice && (pools > 1 || per == 2) ? grid : 0;
 }
 // Up to `max_rounds` rounds of EACH of the K pools (handles on one device, same N) in launches of the persistent
@@ -1631,7 +1630,7 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
       }
       if (prof)
         std::fprintf(stderr, "[tsb200] LL rounds kernel (pool %d of %d): %llu rounds; CTA 0 cycles per round: build %.0f | fence-check %.0f "
-                     "poll-nodes %.0f scan+items %.0f gather-wait %.0f store %.0f signal %.0f\n", a, n_act,
+                     "poll-nodes %.0f scan+items+diag %.0f gather-wait %.0f store %.0f signal %.0f\n", a, n_act,
                      static_cast<unsigned long long>(st.rounds), 1.0 * st.prof[6] / std::max<unsigned long long>(1, st.rounds),
                      1.0 * st.prof[0] / std::max<unsigned long long>(1, st.rounds), 1.0 * st.prof[1] / std::max<unsigned long long>(1, st.rounds),
                      1.0 * st.prof[2] / std::max<unsigned long long>(1, st.rounds), 1.0 * st.prof[3] / std::max<unsigned long long>(1, st.rounds),

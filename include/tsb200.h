@@ -134,7 +134,9 @@ int tsb_nq_expand_device(tsb_nq* h, const void* parents_d /*16-B aligned*/, int 
  * entirely on the device (two kernels: count + build): popBackBulk(m, M) (nothing below m, else the newest min(size, M)
  * nodes, order preserved, read in place), evaluate, generate_children appended to the pool; drain = move what
  * is left to the host (logical order).  The pool's logical content after every round is byte-identical to
- * the reference's host pool. */
+ * the reference's host pool.
+ * push admits only nodes the search can create: depth <= N, board[0..N) < N and board[N..20) == 0.  Any other
+ * node makes it return TSB_EINVAL with the pool unchanged (the pool is packed to 125 bits per node on these terms). */
 int tsb_nq_pool_push(tsb_nq* h, const void* nodes, int64_t n);
 int64_t tsb_nq_pool_size(const tsb_nq* h);
 int tsb_nq_pool_step(tsb_nq* h, int m, int M, int64_t* n_parents, uint64_t* n_children, uint64_t* n_solutions);
