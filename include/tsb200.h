@@ -166,8 +166,12 @@ int tsb_nq_pool_run_multi(tsb_nq* const* handles, int n_pools, int m, int M, int
  * it; their launches are included in h's tsb_nq_kernel_launches count): what a driver groups with `h` in
  * tsb_nq_pool_run_multi. */
 int tsb_nq_sibling(tsb_nq* h, int index, tsb_nq** sibling);
-/* How many pools one launch of the persistent kernel serves best for chunks of up to M parents on h's device: 4
- * (66 CTAs of 768 parents per pool on an H100), 2 (132 + 132 CTAs of 512), or 1 (M beyond the persistent kernel). */
+/* How many pools one launch of the persistent kernel serves best for chunks of up to M parents on h's device: the
+ * most pools, at most 4, whose CTAs still hold a chunk of M, by the capacities of csrc/ll_tiers.h
+ * (ll_pool_capacity).  On an H100 (132 SMs): 4 up to M = 50 688 (66 CTAs per pool), 3 up to 67 584 (88 CTAs per
+ * pool), 2 up to 101 376 (132 CTAs per pool), else 1 (M beyond the persistent kernel).  The pools' CTAs take 512
+ * parents each while that covers M, else 768.  The search drivers cap this by ll_pools_for (and TSB200_POOLS), which
+ * allows several pools only up to the one-pool capacity, so beyond it they run one pool in two-kernel rounds. */
 int tsb_nq_pools_per_launch(const tsb_nq* h, int M);
 
 /* page-lock + map a caller-owned host array for the lifetime of the handle (see the header comment);
