@@ -5,7 +5,7 @@
 
 namespace tsb {
 
-constexpr int LL_MAX_SMS = 256;  // (RND_MAX_CTAS: the flag slots of a launch)
+constexpr int LL_MAX_SMS = 256;  // CTAs per pool at most (the count slots of a launch, LlSync)
 constexpr int LL_SLICE2 = 512;   // parents per CTA with two parents per thread (256 threads)
 constexpr int LL_SLICE3 = 768;   // ... with three
 

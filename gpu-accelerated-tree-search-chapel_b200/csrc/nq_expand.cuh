@@ -32,7 +32,7 @@ namespace tsb {
 constexpr int EXP_CAP = TSB_EXP_CAP;  // children per pass of the shared staging image (a tile averages ~512; denser tiles take several passes)
 
 template <int N, int Q>
-__device__ __forceinline__ uint32_t nq_child_mask(NqParent<N, Q, 0>& p) {
+__device__ __forceinline__ uint32_t nq_child_mask(NqParent<N, Q>& p) {
   const uint32_t S = ~p.U;
   uint32_t cm = 0;
 #pragma unroll
@@ -43,21 +43,19 @@ __device__ __forceinline__ uint32_t nq_child_mask(NqParent<N, Q, 0>& p) {
   return cm & shl_clamp(0xFFFFFFFFu, p.depth);  // only slots k >= depth exist
 }
 
-// evaluate the four parents of this thread: child masks + number of leaves (depth == N).
-// AUX: the attacked values of each parent's next row come from its side word (ld | rd << 20, written when the parent
-// was built: nq_child_ldrd below) instead of the O(depth) pass over its board.
-template <int N, bool AUX>
-__device__ __forceinline__ void nq_eval_quad(const uint8_t* in_tile, const unsigned long long* aux_tile, long long pos0,
-                                             long long lo, long long hi, uint32_t (&cm)[4], int& leaves) {
+// evaluate the four parents of this thread: child masks + number of leaves (depth == N)
+template <int N>
+__device__ __forceinline__ void nq_eval_quad(const uint8_t* in_tile, long long pos0, long long lo, long long hi,
+                                             uint32_t (&cm)[4], int& leaves) {
   const int t = threadIdx.x;
   const uint32_t* in_w = reinterpret_cast<const uint32_t*>(in_tile) + 21 * t;
   uint32_t w[21];
 #pragma unroll
   for (int i = 0; i < 21; i++) w[i] = in_w[i];
-  NqParent<N, 0, 0> p0;
-  NqParent<N, 1, 0> p1;
-  NqParent<N, 2, 0> p2;
-  NqParent<N, 3, 0> p3;
+  NqParent<N, 0> p0;
+  NqParent<N, 1> p1;
+  NqParent<N, 2> p2;
+  NqParent<N, 3> p3;
   p0.init(w);
   p1.init(w);
   p2.init(w);
@@ -72,18 +70,6 @@ __device__ __forceinline__ void nq_eval_quad(const uint8_t* in_tile, const unsig
     if (valid[q]) dmax = max(dmax, dep[q]);  // records outside the chunk hold arbitrary bytes
   }
   dmax = min(dmax, 20u);
-  if constexpr (AUX) {
-    const ulonglong2* ax = reinterpret_cast<const ulonglong2*>(aux_tile + 4 * t);
-    const ulonglong2 a = ax[0], b = ax[1];
-    const auto attacked = [](unsigned long long w) {
-      return (static_cast<uint32_t>(w) | static_cast<uint32_t>(w >> 20)) & 0xFFFFFu;
-    };
-    p0.U = attacked(a.x);
-    p1.U = attacked(a.y);
-    p2.U = attacked(b.x);
-    p3.U = attacked(b.y);
-    dmax = 0;  // (no rows to walk)
-  }
 #pragma unroll
   for (int j = 0; j < (N + 3) / 4; j++) {
     if (dmax > 4u * j) {
@@ -113,30 +99,27 @@ __device__ __forceinline__ void nq_eval_quad(const uint8_t* in_tile, const unsig
 }
 
 // ------------------------------------------------------------------------------------------- count
-template <bool AUX>
 struct NqCountSmem {
   alignas(128) uint8_t in[2][NQ_TILE * NQ_REC];
-  alignas(128) unsigned long long aux[2][AUX ? NQ_TILE : 2];  // side words of the tile (AUX)
   alignas(8) uint64_t full[2];
   int warp_tot[4];
 };
 
 // items of a tile: one uint16 per child, (record << 5) | slot, in child order, at items[lin * NQ_TILE * N ...]
-template <int N, bool AUX>
+template <int N>
 __global__ void __launch_bounds__(NQ_THREADS) nq_expand_count_kernel(const uint8_t* __restrict__ arena,
-                                                                    const unsigned long long* __restrict__ aux,
                                                                     const __grid_constant__ ExpandParams prm,
                                                                     uint16_t* __restrict__ items,
                                                                     int* __restrict__ tile_sums,
                                                                     ExpandState* __restrict__ st) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  NqCountSmem<AUX>& sm = *reinterpret_cast<NqCountSmem<AUX>*>(smem_raw);
+  NqCountSmem& sm = *reinterpret_cast<NqCountSmem*>(smem_raw);
   const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
   constexpr uint32_t IN_BYTES = NQ_TILE * NQ_REC;
   const int first = blockIdx.x, stride = gridDim.x;
   if (t == 0) {
-    mbar_init(&sm.full[0], AUX ? 2 : 1);
-    mbar_init(&sm.full[1], AUX ? 2 : 1);
+    mbar_init(&sm.full[0], 1);
+    mbar_init(&sm.full[1], 1);
     mbar_fence_init();
   }
   __syncthreads();
@@ -146,11 +129,6 @@ __global__ void __launch_bounds__(NQ_THREADS) nq_expand_count_kernel(const uint8
     const uint32_t nb = tile_load_bytes(at, hi, NQ_TILE, NQ_REC);
     mbar_arrive_expect_tx(&sm.full[s], nb);
     if (nb) bulk_g2s(sm.in[s], arena + at * IN_BYTES, nb, &sm.full[s]);  // default L2 policy: the build kernel re-reads it
-    if constexpr (AUX) {
-      const uint32_t na = tile_load_bytes(at, hi, NQ_TILE, 8);
-      mbar_arrive_expect_tx(&sm.full[s], na);
-      if (na) bulk_g2s(sm.aux[s], aux + at * NQ_TILE, na, &sm.full[s]);
-    }
   };
   if (t == 0) {
     if (first < prm.n_tiles) issue(first, 0);
@@ -165,7 +143,7 @@ __global__ void __launch_bounds__(NQ_THREADS) nq_expand_count_kernel(const uint8
     mbar_wait(&sm.full[s], (it >> 1) & 1u);
     uint32_t cm[4];
     int leaves;
-    nq_eval_quad<N, AUX>(sm.in[s], sm.aux[s], at * NQ_TILE, lo, hi, cm, leaves);
+    nq_eval_quad<N>(sm.in[s], at * NQ_TILE, lo, hi, cm, leaves);
     // block scan of the child counts (leaves ride in the upper bits)
     const int mine = __popc(cm[0]) + __popc(cm[1]) + __popc(cm[2]) + __popc(cm[3]);
     int incl = mine | (leaves << 20);  // children of a tile <= 512*20 < 2^20
@@ -203,23 +181,18 @@ __global__ void __launch_bounds__(NQ_THREADS) nq_expand_count_kernel(const uint8
 }
 
 // ------------------------------------------------------------------------------------------- build
-constexpr int EXP_CAP_AUX = 768;  // (window of the AUX variant: its side words take 8 KB of the CTA's shared memory)
-template <bool AUX>
 struct NqBuildSmem {
-  static constexpr int CAP = AUX ? EXP_CAP_AUX : EXP_CAP;
   alignas(128) uint8_t in[2][NQ_TILE * NQ_REC];
-  alignas(128) unsigned long long aux[2][AUX ? NQ_TILE : 2];  // side words of the tile's parents (AUX)
-  alignas(128) uint16_t item[2][CAP];  // first window of the tile's items
-  alignas(128) uint8_t stage[CAP * NQ_REC + 32];
-  alignas(8) uint64_t full[2];             // one arrival per phase and load: parents, items (, side words)
+  alignas(128) uint16_t item[2][EXP_CAP];  // first window of the tile's items
+  alignas(128) uint8_t stage[EXP_CAP * NQ_REC + 32];
+  alignas(8) uint64_t full[2];             // one arrival per phase and load: parents, items
   alignas(8) uint64_t wbar;                // further item windows of dense tiles
   ScanSmem scan;
 };
 
 // child `c` of the tile -> bytes [B, B + 21) of the staging image (B = image offset of the child).  The parent
-// record sits at byte 21*r of the tile (any alignment: the slices of nq_rounds.cuh start at any byte).
-// -> the value of the queen the child places on row `depth` (board[k] of the parent)
-__device__ __forceinline__ uint32_t nq_build_child(const uint8_t* in_tile, int item, uint8_t* image, int B) {
+// record sits at byte 21*r of the tile (read at any alignment).
+__device__ __forceinline__ void nq_build_child(const uint8_t* in_tile, int item, uint8_t* image, int B) {
   const int r = item >> 5, k = item & 31;
   const uint8_t* src = in_tile + r * NQ_REC;
   const uint32_t mis = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(src)) & 3u, a8 = mis * 8u;  // (= r & 3 for an aligned tile)
@@ -264,28 +237,17 @@ __device__ __forceinline__ uint32_t nq_build_child(const uint8_t* in_tile, int i
     if (b >= 1) d0[21] = static_cast<uint8_t>(W5 >> 8);
     if (b >= 2) d0[22] = static_cast<uint8_t>(W5 >> 16);
   }
-  return placed;
-}
-
-// side word of a child from its parent's: the diagonals through the queen just placed (value v on row depth) join
-// the parent's and move one column per row
-template <int N>
-__device__ __forceinline__ unsigned long long nq_child_ldrd(unsigned long long parent_word, uint32_t v) {
-  const uint32_t ld = static_cast<uint32_t>(parent_word) & 0xFFFFFu, rd = static_cast<uint32_t>(parent_word >> 20) & 0xFFFFFu;
-  const uint32_t bit = 1u << (v & 31u);
-  const uint32_t ld2 = ((ld | bit) << 1) & ((1u << N) - 1u), rd2 = (rd | bit) >> 1;
-  return static_cast<unsigned long long>(ld2) | static_cast<unsigned long long>(rd2) << 20;
 }
 
 // The same for a full warp of 32 consecutive children whose first one starts a word of the image (B = 4x for
 // lane 0, hence B & 3 == lane & 3): every word is stored whole — the word a child shares with its right-hand
 // neighbour is completed with the neighbour's first bytes by a warp shuffle, lane 31 ends on a word boundary
 // (32 * 21 bytes = 168 words).  `active` = the child exists; all 32 lanes must call.
-__device__ __forceinline__ uint32_t nq_build_child_warp(const uint8_t* in_tile, int item, uint8_t* image, int B,
-                                                        bool active) {
+__device__ __forceinline__ void nq_build_child_warp(const uint8_t* in_tile, int item, uint8_t* image, int B,
+                                                    bool active) {
   const int b = threadIdx.x & 3;
   const uint32_t b8 = b * 8;
-  uint32_t W0 = 0, W1 = 0, W2 = 0, W3 = 0, W4 = 0, W5 = 0, placed = 0;
+  uint32_t W0 = 0, W1 = 0, W2 = 0, W3 = 0, W4 = 0, W5 = 0;
   if (active) {
     const int r = item >> 5, k = item & 31;
     const uint8_t* src = in_tile + r * NQ_REC;
@@ -296,7 +258,7 @@ __device__ __forceinline__ uint32_t nq_build_child_warp(const uint8_t* in_tile, 
                      shf_r_wrap(s3, s4, a8), shf_r_wrap(s4, s5, a8), shf_r_wrap(s5, 0u, a8) & 0xFFu};
     const uint32_t depth = P[0] & 0xFFu;
     const uint32_t p1 = 1u + depth, p2 = 1u + static_cast<uint32_t>(k);
-    placed = src[p2];
+    const uint32_t placed = src[p2];
     const uint32_t D = static_cast<uint32_t>(src[p1]) ^ placed;
     const uint32_t x1 = D << ((p1 & 3u) * 8u), x2 = D << ((p2 & 3u) * 8u);
     const uint32_t w1 = p1 >> 2, w2 = p2 >> 2;
@@ -320,30 +282,25 @@ __device__ __forceinline__ uint32_t nq_build_child_warp(const uint8_t* in_tile, 
     dw[4] = W4;
     dw[5] = b == 3 ? W5 : (W5 | nb);  // (a last child writes up to 3 zero bytes past the image's end)
   }
-  return placed;
 }
 
-template <int N, bool AUX>
+template <int N>
 __global__ void __launch_bounds__(NQ_THREADS) nq_expand_build_kernel(const uint8_t* __restrict__ arena,
-                                                                    const unsigned long long* __restrict__ aux,
                                                                     const __grid_constant__ ExpandParams prm,
                                                                     const uint16_t* __restrict__ items,
                                                                     const int* __restrict__ tile_sums,
                                                                     uint8_t* __restrict__ children,
-                                                                    unsigned long long* __restrict__ children_aux,
                                                                     ExpandState* __restrict__ st,
                                                                     ExpandResult* __restrict__ res) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  using Smem = NqBuildSmem<AUX>;
-  constexpr int CAP = Smem::CAP;
-  Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
+  NqBuildSmem& sm = *reinterpret_cast<NqBuildSmem*>(smem_raw);
   const int t = threadIdx.x;
   constexpr uint32_t IN_BYTES = NQ_TILE * NQ_REC;
   constexpr long long IST = static_cast<long long>(NQ_TILE) * N;  // items per tile slot
   const int first = blockIdx.x, stride = gridDim.x;
   if (t == 0) {
-    mbar_init(&sm.full[0], AUX ? 3 : 2);
-    mbar_init(&sm.full[1], AUX ? 3 : 2);
+    mbar_init(&sm.full[0], 2);
+    mbar_init(&sm.full[1], 2);
     mbar_init(&sm.wbar, 1);
     mbar_fence_init();
   }
@@ -356,14 +313,9 @@ __global__ void __launch_bounds__(NQ_THREADS) nq_expand_build_kernel(const uint8
     const uint32_t nb = tile_load_bytes(at, hi, NQ_TILE, NQ_REC);
     mbar_arrive_expect_tx(&sm.full[s], nb);
     if (nb) bulk_g2s_stream(sm.in[s], arena + at * IN_BYTES, nb, &sm.full[s], pol);
-    if constexpr (AUX) {
-      const uint32_t na = tile_load_bytes(at, hi, NQ_TILE, 8);
-      mbar_arrive_expect_tx(&sm.full[s], na);
-      if (na) bulk_g2s_stream(sm.aux[s], aux + at * NQ_TILE, na, &sm.full[s], pol);
-    }
   };
   auto issue_items = [&](int lin, int s, int cnt) {  // thread 0: the first window of the tile's items
-    const uint32_t nb = (static_cast<uint32_t>(min(cnt, CAP)) * 2u + 15u) & ~15u;
+    const uint32_t nb = (static_cast<uint32_t>(min(cnt, EXP_CAP)) * 2u + 15u) & ~15u;
     mbar_arrive_expect_tx(&sm.full[s], nb);
     if (nb) bulk_g2s_stream(sm.item[s], items + lin * IST, nb, &sm.full[s], pol);
   };
@@ -383,9 +335,8 @@ __global__ void __launch_bounds__(NQ_THREADS) nq_expand_build_kernel(const uint8
     const int total = sm.scan.cnt[it];
     uint8_t* const gtile = children + static_cast<long long>(sm.scan.own[it]) * NQ_REC;
     mbar_wait(&sm.full[s], (it >> 1) & 1u);
-    unsigned long long* const gaux = AUX ? children_aux + sm.scan.own[it] : nullptr;
-    for (int c0 = 0; c0 < total; c0 += CAP) {  // windows of CAP children (one, except for dense tiles)
-      const int cnt = min(CAP, total - c0);
+    for (int c0 = 0; c0 < total; c0 += EXP_CAP) {  // windows of EXP_CAP children (one, except for dense tiles)
+      const int cnt = min(EXP_CAP, total - c0);
       if (c0 > 0) {  // dense tile: fetch the next window of items (everyone passed (B) of the previous window)
         if (t == 0) {
           const uint32_t nb = (static_cast<uint32_t>(cnt) * 2u + 15u) & ~15u;
@@ -402,19 +353,11 @@ __global__ void __launch_bounds__(NQ_THREADS) nq_expand_build_kernel(const uint8
       uint8_t* sdst = sm.stage + phase;
       // the first (-phase) & 3 children byte-wise, so that the warps' runs of 32 children start on a word
       const int c_head = min(cnt, (4 - (phase & 3)) & 3);
-      if (t < c_head) {
-        const int item = sm.item[s][t];
-        const uint32_t v = nq_build_child(sm.in[s], item, sm.stage, phase + t * NQ_REC);
-        if constexpr (AUX) gaux[c0 + t] = nq_child_ldrd<N>(sm.aux[s][item >> 5], v);
-      }
+      if (t < c_head) nq_build_child(sm.in[s], sm.item[s][t], sm.stage, phase + t * NQ_REC);
       for (int cb = c_head; cb < cnt; cb += NQ_THREADS) {
         const int c = cb + t;
         const bool active = c < cnt;
-        const int item = active ? sm.item[s][c] : 0;
-        const uint32_t v = nq_build_child_warp(sm.in[s], item, sm.stage, phase + c * NQ_REC, active);
-        if constexpr (AUX) {
-          if (active) gaux[c0 + c] = nq_child_ldrd<N>(sm.aux[s][item >> 5], v);
-        }
+        nq_build_child_warp(sm.in[s], active ? sm.item[s][c] : 0, sm.stage, phase + c * NQ_REC, active);
       }
       fence_async_smem();
       __syncthreads();  // (B) image complete; in[s] / item[s] free after the last window

@@ -42,10 +42,8 @@ constexpr int NQ_TILE = NQ_THREADS * NQ_QUAD;    // 512 parents per tile
 constexpr int NQ_REC = 21;                       // sizeof(tsb_nq_node)
 constexpr int NQ_STAGES = 2;
 
-// (T = threads per CTA, 4 parents each: 128 for bandwidth-bound batches; 64 / 32 give small chunks — the
-// reference's default --M 50000 is 97 tiles of 512 — enough CTAs to cover all SMs)
-template <int N, int T = NQ_THREADS>
-using NqSmem = TileSmem<NQ_STAGES, T * NQ_QUAD * NQ_REC, T * NQ_QUAD * N>;
+template <int N>
+using NqSmem = TileSmem<NQ_STAGES, NQ_TILE * NQ_REC, NQ_TILE * N>;
 
 // Integer multiplies that must stay multiplies: they run on the FMA pipe (IMAD), which this
 // kernel leaves idle, instead of the ALU pipe (SHF/LOP3), which is its bottleneck.
@@ -54,20 +52,12 @@ __device__ __forceinline__ uint32_t mul_lo_fma(uint32_t x, uint32_t c) {
   asm("mul.lo.u32 %0, %1, %2;" : "=r"(r) : "r"(x), "r"(c));
   return r;
 }
-__device__ __forceinline__ uint32_t mul_hi_fma(uint32_t x, uint32_t c) {
-  uint32_t r;
-  asm("mul.hi.u32 %0, %1, %2;" : "=r"(r) : "r"(x), "r"(c));
-  return r;
-}
 
 // a register whose LOW BYTE is byte B (compile-time) of the little-endian word array w
-// (VAR 1: the right shift is done as a high multiply on the FMA pipe)
-template <int B, int VAR>
+template <int B>
 __device__ __forceinline__ uint32_t low_byte_reg(const uint32_t* w) {
   if constexpr ((B & 3) == 0)
     return w[B >> 2];
-  else if constexpr (VAR == 1)
-    return mul_hi_fma(w[B >> 2], 1u << (32 - 8 * (B & 3)));
   else
     return w[B >> 2] >> (8 * (B & 3));
 }
@@ -90,32 +80,22 @@ __device__ __forceinline__ void nq_rows(uint32_t ph, uint32_t rb, const uint32_t
   U |= nq_row_term<N, I0 + 2>(ph, rb, amt) | nq_row_term<N, I0 + 3>(ph, rb, amt);
 }
 
-template <int N, int Q, int VAR>
+template <int N, int Q>
 struct NqParent {
   uint32_t depth, ph, rb, U;
   uint32_t amt[N];
 
   __device__ __forceinline__ void init(const uint32_t* w) {
-    depth = low_byte_reg<21 * Q, VAR>(w) & 0xFFu;
+    depth = low_byte_reg<21 * Q>(w) & 0xFFu;
     ph = shl_clamp(1u, depth - 1u);   // 1 << (depth-1); 0 for depth == 0 (amount wraps to >= 32)
     rb = shl_clamp(1u, 32u - depth);  // 1 << (32-depth); 0 for depth == 0
     U = 0;
     fill_amt<0>(w);
   }
-  // VAR 2: every byte by its own LDS.U8 (thread stride 84 B = 21 words: conflict free) instead of word loads +
-  // shifts — the shifts run on the ALU pipe, which is this kernel's limiter; the LSU pipe is idle
-  __device__ __forceinline__ void init_bytes(const uint8_t* pb) {
-    depth = pb[21 * Q];
-    ph = shl_clamp(1u, depth - 1u);
-    rb = shl_clamp(1u, 32u - depth);
-    U = 0;
-#pragma unroll
-    for (int i = 0; i < N; i++) amt[i] = pb[21 * Q + 1 + i];
-  }
   template <int I>
   __device__ __forceinline__ void fill_amt(const uint32_t* w) {
     if constexpr (I < N) {
-      amt[I] = low_byte_reg<21 * Q + 1 + I, VAR>(w);
+      amt[I] = low_byte_reg<21 * Q + 1 + I>(w);
       fill_amt<I + 1>(w);
     }
   }
@@ -152,7 +132,7 @@ struct NqParent {
   }
 };
 
-template <int N, int VAR>
+template <int N>
 __device__ __forceinline__ void nq_compute_tile(const uint8_t* in_tile, uint8_t* out_tile, int /*records*/) {
   const uint32_t* in_w = reinterpret_cast<const uint32_t*>(in_tile) + 21 * threadIdx.x;
   uint32_t* out_w = reinterpret_cast<uint32_t*>(out_tile) + N * threadIdx.x;
@@ -160,25 +140,17 @@ __device__ __forceinline__ void nq_compute_tile(const uint8_t* in_tile, uint8_t*
 #pragma unroll
   for (int i = 0; i < N; i++) o[i] = 0;
 
-  NqParent<N, 0, VAR> p0;
-  NqParent<N, 1, VAR> p1;
-  NqParent<N, 2, VAR> p2;
-  NqParent<N, 3, VAR> p3;
-  if constexpr (VAR == 2) {
-    const uint8_t* pb = in_tile + 84 * threadIdx.x;
-    p0.init_bytes(pb);
-    p1.init_bytes(pb);
-    p2.init_bytes(pb);
-    p3.init_bytes(pb);
-  } else {
-    uint32_t w[21];
+  NqParent<N, 0> p0;
+  NqParent<N, 1> p1;
+  NqParent<N, 2> p2;
+  NqParent<N, 3> p3;
+  uint32_t w[21];
 #pragma unroll
-    for (int i = 0; i < 21; i++) w[i] = in_w[i];
-    p0.init(w);
-    p1.init(w);
-    p2.init(w);
-    p3.init(w);
-  }
+  for (int i = 0; i < 21; i++) w[i] = in_w[i];
+  p0.init(w);
+  p1.init(w);
+  p2.init(w);
+  p3.init(w);
   const uint32_t dmax = max(max(p0.depth, p1.depth), max(p2.depth, p3.depth));
   const uint32_t dmin = min(min(p0.depth, p1.depth), min(p2.depth, p3.depth));
 
@@ -226,14 +198,14 @@ __device__ __forceinline__ void nq_compute_tile(const uint8_t* in_tile, uint8_t*
   for (int i = 0; i < N; i++) out_w[i] = o[i];
 }
 
-template <int N, int VAR, int T = NQ_THREADS>
-__global__ void __launch_bounds__(T) nq_evaluate_kernel(const uint8_t* __restrict__ parents,
-                                                       uint8_t* __restrict__ labels, long long count) {
+template <int N>
+__global__ void __launch_bounds__(NQ_THREADS) nq_evaluate_kernel(const uint8_t* __restrict__ parents,
+                                                                uint8_t* __restrict__ labels, long long count) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  NqSmem<N, T>& sm = *reinterpret_cast<NqSmem<N, T>*>(smem_raw);
-  run_tile_pipeline<NQ_STAGES, T * NQ_QUAD, NQ_REC, N>(
+  NqSmem<N>& sm = *reinterpret_cast<NqSmem<N>*>(smem_raw);
+  run_tile_pipeline<NQ_STAGES, NQ_TILE, NQ_REC, N>(
       sm, parents, labels, count,
-      [](const uint8_t* in_tile, uint8_t* out_tile, int n, long long) { nq_compute_tile<N, VAR>(in_tile, out_tile, n); });
+      [](const uint8_t* in_tile, uint8_t* out_tile, int n, long long) { nq_compute_tile<N>(in_tile, out_tile, n); });
 }
 
 // ---- small chunks (the reference's default --M 50000 is 97 tiles of 512 parents: two thirds of the SMs, each thread
@@ -269,7 +241,7 @@ __global__ void __launch_bounds__(NQ_SMALL) nq_evaluate_small_kernel(const uint8
   if (t < np) {
     uint32_t P[6];
     nq_parent_words(in + t * NQ_REC, P);
-    NqParent<N, 0, 0> p;
+    NqParent<N, 0> p;
     p.init(P);
     if (p.depth > 0u) p.template rows<0, 4>();
     if (p.depth > 4u) p.template rows<4, 8>();

@@ -1,8 +1,16 @@
 // nq_rounds_ll.cuh — the persistent multi-round N-Queens kernel without fences on its critical path.
 //
-// nq_rounds.cuh (v2) orders round r+1 after round r with a release fence (MEMBAR.ALL.GPU, thousands of cycles
-// under load) and a "done" flag exchange among all CTAs, on top of the exchange that gathers the child counts:
-// most of a round is spent waiting on them.  Here the pool lives, while the kernel runs, in a SELF-VALIDATING format
+// One round of the reference's step 2 (nqueens_gpu_chpl.chpl:197-215) is: popBackBulk(m, M) = the newest
+// n = min(size, M) nodes of the pool (nothing if size < m, lib/commons/Pool.chpl:50-59), evaluate_gpu on them,
+// generate_children pushing the surviving children back, in order.  Round i+1 pops what round i pushed, so the rounds
+// are a latency chain; at the reference's default --M 50000 two launches and a host poll per round would be the cost.
+// This kernel runs the whole loop in one cooperative launch: every CTA tracks the (tiny) pool state redundantly — a
+// deterministic function of the per-round totals, which every CTA learns anyway — so nothing is broadcast.
+//
+// An earlier version ordered round r+1 after round r with a release fence (MEMBAR.ALL.GPU, thousands of cycles under
+// load) and a "done" flag exchange among all CTAs, on top of the exchange that gathers the child counts: most of its
+// round was spent waiting on them (rounds_sync_bench_kernel at the end of this file measures that floor).  It was
+// removed in favour of this kernel.  Here the pool lives, while the kernel runs, in a SELF-VALIDATING format
 // (the "LL" idea of NCCL's low-latency protocol):
 //
 //   fat node = 4 x 8-byte words; word i = data32[i] | epoch << 32     (32 B per node = one sector, 32-byte aligned)
@@ -13,7 +21,9 @@
 //     label for slot k, nqueens_gpu_chpl.chpl:97-123), bit 30: leaf (depth == N)
 //   The diagonal masks of a parent (what its next row attacks) are not stored: a round recomputes them from the placed
 //   prefix, O(depth), for the parents that have children, while the child counts are on their way; a child's masks
-//   follow from its parent's in O(1) as in nq_rounds.cuh, and its child mask is evaluated when it is built.
+//   follow from its parent's in O(1) (ll_build_child), and its child mask is evaluated when it is built.  (The earlier
+//   version stored the masks in a side word next to each 21-byte node: 64 bytes per node, twice the poll loads and
+//   store pieces of a round.)
 //
 // Every 8-byte word is written by one store (an element of a st.v2.u64) and is therefore seen whole or not at all;
 // a reader that expects the children of round r polls the words of its slice until all four carry r's epoch.  No
@@ -42,9 +52,12 @@
 // a chain of L2 round trips with little work in between, and nothing inside one pool can fill the waits — another
 // pool's CTA on the same SM can: on the N = 17 search at M = 50000 three or four pools per launch (two CTAs per SM in
 // all, 768 parents per CTA) take little more than half the time of one pool.
+//
+// A spin loop that waits longer than ~2 s raises a global abort flag and every CTA leaves (exit code ABORT): a logic
+// error must never hang the GPU.
 #pragma once
 #include "ll_tiers.h"
-#include "nq_rounds.cuh"
+#include "nq_kernel.cuh"
 
 namespace tsb {
 
@@ -53,7 +66,39 @@ constexpr int LL_T = 256;                    // threads per CTA
 // (SMs / 2 CTAs per pool: a round's count exchange among half the CTAs costs about half, tools/flag_exchange.py, and
 // every CTA brings 1.5x the work to hide it behind)
 __host__ __device__ constexpr int ll_slice(int ppt) { return LL_T * ppt; }          // parents per CTA per round
-static_assert(ll_slice(2) == LL_SLICE2 && ll_slice(3) == LL_SLICE3 && RND_MAX_CTAS == LL_MAX_SMS, "ll_tiers.h");
+static_assert(ll_slice(2) == LL_SLICE2 && ll_slice(3) == LL_SLICE3, "ll_tiers.h");
+
+enum { RND_EXIT_DONE = 0, RND_EXIT_PAUSE = 1, RND_EXIT_SPACE = 2, RND_EXIT_ABORT = 3, RND_EXIT_RELAUNCH = 4 };
+// in / out record of a launch (pinned + mapped host memory)
+struct RoundsState {
+  long long size;                 // nodes in the pool: positions [0, size)
+  unsigned epoch;                 // last epoch used
+  int exit_code;
+  unsigned long long rounds, parents, children, solutions;  // of this launch
+  long long prof[8];  // (prm.prof) cycles CTA 0 spent per phase (the TSB_PROF indices of nq_rounds_ll_kernel)
+};
+
+__device__ __forceinline__ void st_relaxed_u64(unsigned long long* p, unsigned long long v) {
+  asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+// Every CTA needs every other CTA's flag, so the polling is done by ONE warp per CTA with coalesced 16-byte loads: one
+// thread per slot spinning on its own flag put ~22 000 loads per sweep on a handful of L2 lines and made rounds
+// several times slower.
+struct SpinGuard {  // watchdog of a spin loop: ~2 s, or another CTA's abort
+  unsigned spins = 0;
+  long long t0 = 0;
+  __device__ __forceinline__ bool expired(unsigned* abort_flag) {
+    if ((++spins & 0xFFu) != 0) return false;
+    if (*reinterpret_cast<volatile unsigned*>(abort_flag)) return true;
+    const long long now = clock64();
+    if (t0 == 0) t0 = now;
+    if (now - t0 > 4000000000LL) {
+      *reinterpret_cast<volatile unsigned*>(abort_flag) = 1u;
+      return true;
+    }
+    return false;
+  }
+};
 // children per window of the staging buffer (a CTA's share of a round averages ~0.8 children per parent; a dense
 // share takes several windows)
 constexpr int LL_CAP = 2048;
@@ -79,7 +124,7 @@ __device__ __forceinline__ void ll_set_depth(uint32_t (&d)[4], uint32_t depth) {
   d[2] = (d[2] & 0x3FFFFFFFu) | (depth >> 4) << 30;
 }
 struct LlSync {
-  unsigned long long slot[2][2 * RND_MAX_CTAS];  // by round parity, one per SUB-slice: epoch << 32 | leaves << 20 | children
+  unsigned long long slot[2][2 * LL_MAX_SMS];  // by round parity, one per SUB-slice: epoch << 32 | leaves << 20 | children
   unsigned abort;
 };
 constexpr int LL_MAX_POOLS = 4;  // independent pools one launch can serve (blockIdx.y)
@@ -126,6 +171,34 @@ __device__ __forceinline__ void st_fat2(unsigned long long* p, unsigned long lon
 // ---- plain arena <-> fat arena (one thread per node; not performance critical: the whole pool, once per hand-over).
 // Byte for byte for every node tsb_nq_pool_push admits (depth <= N, board[0..N) < N, bytes past N zero), which
 // are the only nodes a pool holds.
+
+// a node's word of the earlier 64-byte format, from its board by the reference predicate, row by row:
+//   bits  0..19  ld: values attacked on the node's next row along the rising diagonals  {board[i] + (depth - i)}
+//   bits 20..39  rd: ... along the falling diagonals                                     {board[i] - (depth - i)}
+//   bits 40..59  the node's child mask: slot k set <=> k >= depth and board[k] is not attacked (evaluate_gpu's
+//                label for slot k, nqueens_gpu_chpl.chpl:97-123)
+//   bit  60      leaf (depth == N)
+// The import keeps only the child mask and the leaf flag.  A helper that returns just those compiles the import to
+// different (not faster) code, so the whole word is kept.
+__device__ __forceinline__ unsigned long long nq_aux_pack(uint32_t ld, uint32_t rd, uint32_t cm, bool leaf) {
+  return static_cast<unsigned long long>(ld) | static_cast<unsigned long long>(rd) << 20 |
+         static_cast<unsigned long long>(cm) << 40 | static_cast<unsigned long long>(leaf ? 1u : 0u) << 60;
+}
+template <int N>
+__device__ __forceinline__ unsigned long long nq_aux_of_node(const uint8_t* node) {
+  const int d = node[0];
+  uint32_t ld = 0, rd = 0;
+  for (int i = 0; i < d && i < N; i++) {
+    const int b = node[1 + i], s = d - i;
+    if (b + s < N) ld |= 1u << (b + s);
+    if (b - s >= 0) rd |= 1u << (b - s);
+  }
+  const uint32_t U = ld | rd;
+  uint32_t cm = 0;
+  for (int k = d; k < N; k++)
+    if (!((U >> (node[1 + k] & 31)) & 1u)) cm |= 1u << k;
+  return nq_aux_pack(ld, rd, cm, d == N);
+}
 template <int N>
 __global__ void nq_fat_import_kernel(const uint8_t* __restrict__ arena, FatNode* __restrict__ fat, long long size,
                                      unsigned epoch) {
@@ -517,6 +590,97 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
       for (int i = 0; i < 8; i++) st->prof[i] = sm.prof[i];
   }
 #undef TSB_PROF
+}
+
+// ---- diagnostics (tsb_debug_flag_exchange, tools/flag_exchange.py): cycles per round of bare all-to-all flag exchanges
+// among co-resident CTAs, with no evaluation and no children — the floor that ordering the rounds puts under a round,
+// and how it scales with the number of CTAs (nq_ll_grid's CTA counts rest on it).  By default a round is two
+// exchanges: every CTA publishes a slot and polls all G slots, then releases a "done" flag (st.release) and polls all
+// G done flags followed by an acquire fence.  variant bits: 1 = no release fence (plain store of the done flag); 2 = no
+// acquire fence; 4 = every thread stores 16 bytes to global before the release (a round's children); 8 = polls are
+// weak L2 loads (ld.global.cg) instead of ld.relaxed.gpu; 16 = only ONE exchange per round (the slots); 32 = one
+// exchange through per-reader inboxes (every writer stores its flag into every reader's own row)
+struct RoundsSync {  // zeroed before the launch
+  unsigned long long slot[LL_MAX_SMS];  // 32-bit slots by round parity
+  unsigned done[LL_MAX_SMS];            // epoch of the last round this CTA has finished
+  unsigned abort;
+};
+__device__ __forceinline__ void st_release_u32(unsigned* p, unsigned v) {
+  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+template <bool CG>
+__device__ __forceinline__ void bench_ld4(const unsigned* p, unsigned& v0, unsigned& v1, unsigned& v2, unsigned& v3) {
+  if constexpr (CG)
+    asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v0), "=r"(v1), "=r"(v2), "=r"(v3) : "l"(p) : "memory");
+  else
+    asm volatile("ld.relaxed.gpu.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v0), "=r"(v1), "=r"(v2), "=r"(v3) : "l"(p) : "memory");
+}
+// warp 0: all G 32-bit flags equal `want`
+template <bool CG>
+__device__ __forceinline__ bool bench_wait32(const unsigned* f, int G, unsigned want, unsigned* abort_flag) {
+  const int lane = threadIdx.x & 31;
+  SpinGuard guard;
+  for (;;) {
+    bool ok = true;
+    for (int i = 4 * lane; i < G; i += 128) {
+      unsigned v0, v1, v2, v3;
+      bench_ld4<CG>(f + i, v0, v1, v2, v3);
+      ok &= v0 == want && (i + 1 >= G || v1 == want) && (i + 2 >= G || v2 == want) && (i + 3 >= G || v3 == want);
+    }
+    if (__all_sync(0xFFFFFFFFu, ok)) return true;
+    if (__any_sync(0xFFFFFFFFu, guard.expired(abort_flag))) return false;
+  }
+}
+template <bool CG>
+__device__ __forceinline__ void rounds_sync_bench_body(RoundsSync* sy, unsigned epoch0, int rounds, int variant,
+                                                       uint4* scratch, long long* out_cycles) {
+  const int t = threadIdx.x, wid = t >> 5, k = blockIdx.x, G = gridDim.x;
+  unsigned* const slot32 = reinterpret_cast<unsigned*>(sy->slot);  // 32-bit slots: 592 B = 5 lines per sweep
+  unsigned epoch = epoch0;
+  const long long c0 = clock64();
+  for (int r = 0; r < rounds; r++) {
+    ++epoch;
+    bool ok = true;
+    if (!(variant & 16)) {
+      if (r > 0 && wid == 0) {
+        ok = bench_wait32<CG>(sy->done, G, epoch - 1u, &sy->abort);
+        if (!(variant & 2)) __threadfence();
+      }
+      if (__syncthreads_or(!ok)) break;
+    }
+    if (variant & 32) {  // per-reader inboxes: writer k stores its flag into row j of every reader j; a reader polls
+                         // only its own row (no line is polled by more than one CTA)
+      unsigned* const inbox = reinterpret_cast<unsigned*>(scratch) + (r & 1) * 256 * 256;
+      for (int j = t; j < G; j += LL_T)
+        asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(&inbox[j * 256 + k]), "r"(epoch) : "memory");
+      if (wid == 0) ok = bench_wait32<CG>(inbox + k * 256, G, epoch, &sy->abort);
+      if (__syncthreads_or(!ok)) break;
+      continue;
+    }
+    unsigned* const sl = slot32 + 256 * (r & 1);  // (two slot arrays, by round parity: a single exchange per round
+                                                  // lets a fast CTA publish round r+1 before a slow one has read r)
+    if (t == 0) asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(&sl[k]), "r"(epoch) : "memory");
+    if (wid == 0) ok = bench_wait32<CG>(sl, G, epoch, &sy->abort);
+    if (__syncthreads_or(!ok)) break;
+    if (variant & 4) __stcg(scratch + (static_cast<long long>(k) * LL_T + t), make_uint4(epoch, t, k, r));
+    if (!(variant & 16)) {
+      __syncthreads();
+      if (t == 0) {
+        if (variant & 1)
+          asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(&sy->done[k]), "r"(epoch) : "memory");
+        else
+          st_release_u32(&sy->done[k], epoch);
+      }
+    }
+  }
+  if (k == 0 && t == 0) *out_cycles = clock64() - c0;
+}
+__global__ void __launch_bounds__(LL_T, 1) rounds_sync_bench_kernel(RoundsSync* sy, unsigned epoch0, int rounds,
+                                                                    int variant, uint4* scratch, long long* out_cycles) {
+  if (variant & 8)
+    rounds_sync_bench_body<true>(sy, epoch0, rounds, variant, scratch, out_cycles);
+  else
+    rounds_sync_bench_body<false>(sy, epoch0, rounds, variant, scratch, out_cycles);
 }
 
 }  // namespace tsb

@@ -17,8 +17,6 @@
 #include <vector>
 
 #include "nq_expand.cuh"
-#include "nq_expand2.cuh"
-#include "nq_rounds.cuh"
 #include "nq_rounds_ll.cuh"
 #include "pfsp_expand.cuh"
 #include "nq_kernel.cuh"
@@ -325,8 +323,8 @@ struct ExpandCtx {
   tsb::ExpandResult* h_res = nullptr;  // pinned + mapped: written by the scan kernel of a round
   tsb::ExpandResult* d_res = nullptr;  // device alias of h_res
   unsigned epoch = 0;
-  int occ_count = 0, occ_build = 0, occ_count2 = 0, occ_build2 = 0;
-  bool attr_set = false, attr_set2 = false;
+  int occ_count = 0, occ_build = 0;
+  bool attr_set = false;
   // (clears are ordered on the stream the kernels run on: the handle's streams do not synchronise with the
   // legacy default stream)
   int reserve(long long tiles, long long side_bytes_per_tile, cudaStream_t s, int best_init = 0x7FFFFFFF) {
@@ -398,9 +396,6 @@ struct ExpandCtx {
 // copied; the holes left behind are reclaimed by compacting into the second arena when the top reaches the end.
 struct DevicePool {
   uint8_t* arena[2] = {nullptr, nullptr};
-  // optional side array: `side_rec` bytes per arena position, moved with the nodes (N-Queens: nq_expand2.cuh)
-  uint8_t* side[2] = {nullptr, nullptr};
-  size_t side_rec = 0, side_slack = 0;
   long long cap = 0;  // nodes per arena
   int cur = 0;
   size_t rec = 0, slack = 0;
@@ -409,44 +404,35 @@ struct DevicePool {
   uint64_t compactions = 0;
   long long top() const { return ext.empty() ? 0 : ext.back().e; }
   size_t bytes(long long nodes) const { return static_cast<size_t>(nodes) * rec + slack + 64; }
-  size_t side_bytes(long long nodes) const { return static_cast<size_t>(nodes) * side_rec + side_slack + 64; }
   int ensure_arena(int which, long long nodes) {
     (void)nodes;
     if (!arena[which]) TSB_CUDA(cudaMalloc(&arena[which], bytes(cap)));
-    if (side_rec && !side[which]) TSB_CUDA(cudaMalloc(&side[which], side_bytes(cap)));
     return TSB_OK;
   }
   // all extents -> [0, size) of the other arena (or of fresh, larger arenas when `new_cap` > cap)
   int compact(cudaStream_t s, long long new_cap) {
-    uint8_t *dst = nullptr, *sdst = nullptr;
+    uint8_t* dst = nullptr;
     const bool grow = new_cap > cap;
     if (grow) {
       TSB_CUDA(cudaMalloc(&dst, static_cast<size_t>(new_cap) * rec + slack + 64));
-      if (side_rec) TSB_CUDA(cudaMalloc(&sdst, side_bytes(new_cap)));
     } else {
       int rc = ensure_arena(cur ^ 1, cap);
       if (rc != TSB_OK) return rc;
       dst = arena[cur ^ 1];
-      sdst = side[cur ^ 1];
     }
     long long at = 0;
     for (const PoolExtent& x : ext) {
       TSB_CUDA(cudaMemcpyAsync(dst + at * rec, arena[cur] + x.b * rec, static_cast<size_t>(x.e - x.b) * rec,
                                cudaMemcpyDeviceToDevice, s));
-      if (side_rec && side[cur])
-        TSB_CUDA(cudaMemcpyAsync(sdst + at * side_rec, side[cur] + x.b * side_rec,
-                                 static_cast<size_t>(x.e - x.b) * side_rec, cudaMemcpyDeviceToDevice, s));
       at += x.e - x.b;
     }
     TSB_CUDA(cudaStreamSynchronize(s));
     if (grow) {
       for (int i = 0; i < 2; i++) {
         if (arena[i]) cudaFree(arena[i]);
-        if (side[i]) cudaFree(side[i]);
-        arena[i] = side[i] = nullptr;
+        arena[i] = nullptr;
       }
       arena[0] = dst;
-      side[0] = sdst;
       cur = 0;
       cap = new_cap;
     } else {
@@ -471,8 +457,7 @@ struct DevicePool {
   void release() {
     for (int i = 0; i < 2; i++) {
       if (arena[i]) cudaFree(arena[i]);
-      if (side[i]) cudaFree(side[i]);
-      arena[i] = side[i] = nullptr;
+      arena[i] = nullptr;
     }
     ext.clear();
     size = 0;
@@ -480,19 +465,11 @@ struct DevicePool {
   }
 };
 
-// state of the persistent multi-round kernel of one handle (nq_rounds.cuh)
+// state of the persistent multi-round kernel of one handle (nq_rounds_ll.cuh)
 struct RoundsCtx {
-  tsb::RoundsSync* d_sync = nullptr;
   tsb::RoundsState* h_state = nullptr;  // pinned + mapped: written by the kernel when it leaves
   tsb::RoundsState* d_state = nullptr;  // device alias of h_state
   unsigned epoch = 0;
-  bool attr_set = false;
-  int threads = 256;  // CTA size (env TSB200_ROUNDS_THREADS = 256 | 512)
-  int ctas = 0;       // CTAs per pool (env TSB200_ROUNDS_CTAS; 0 = nq_ll_grid's measured defaults: an all-to-all flag
-                      // exchange among all SMs' CTAs costs 2-3x one among half of them (tools/flag_exchange.py), the per-CTA work
-                      // grows the other way)
-  int ppt = 0;        // env TSB200_ROUNDS_PPT=3: the 768-parent slices also where 512 would do (experiments)
-  int version = 3;    // 3 = the fence-free kernel on the fat arena (nq_rounds_ll.cuh); 2 = nq_rounds.cuh (env TSB200_ROUNDS_V)
   tsb::FatNode* d_fat = nullptr;  // the pool in the self-validating 32-byte format, while the LL kernel owns it
   long long fat_cap = 0;
   bool in_fat = false;            // the pool currently lives in d_fat (the plain arena is stale)
@@ -511,31 +488,7 @@ struct RoundsCtx {
     fat_cap = cap;
     return TSB_OK;
   }
-  unsigned long long* d_aux = nullptr;  // side word per arena position (nq_rounds.cuh)
-  long long aux_cap = 0, aux_valid = 0;
-  int ensure_aux(long long cap) {
-    if (cap <= aux_cap) return TSB_OK;
-    if (d_aux) cudaFree(d_aux);
-    d_aux = nullptr;
-    aux_cap = aux_valid = 0;
-    TSB_CUDA(cudaMalloc(&d_aux, static_cast<size_t>(cap) * sizeof(unsigned long long) + 256));
-    aux_cap = cap;
-    return TSB_OK;
-  }
-  RoundsCtx() {
-    if (const char* v = std::getenv("TSB200_ROUNDS_THREADS")) {
-      const int x = std::atoi(v);
-      if (x == 256 || x == 512) threads = x;
-    }
-    if (const char* v = std::getenv("TSB200_ROUNDS_CTAS")) ctas = std::max(1, std::atoi(v));
-    if (const char* v = std::getenv("TSB200_ROUNDS_PPT")) ppt = std::atoi(v) == 3 ? 3 : 0;
-    if (const char* v = std::getenv("TSB200_ROUNDS_V")) version = std::atoi(v) == 2 ? 2 : 3;
-  }
-  int ensure(cudaStream_t s) {
-    if (!d_sync) {
-      TSB_CUDA(cudaMalloc(&d_sync, sizeof(tsb::RoundsSync)));
-      TSB_CUDA(cudaMemsetAsync(d_sync, 0, sizeof(tsb::RoundsSync), s));
-    }
+  int ensure() {
     if (!h_state) {
       TSB_CUDA(cudaHostAlloc(&h_state, sizeof(tsb::RoundsState), cudaHostAllocPortable | cudaHostAllocMapped));
       std::memset(h_state, 0, sizeof(tsb::RoundsState));
@@ -544,30 +497,24 @@ struct RoundsCtx {
     return TSB_OK;
   }
   void release() {
-    if (d_sync) cudaFree(d_sync);
     if (h_state) cudaFreeHost(h_state);
-    if (d_aux) cudaFree(d_aux);
     if (d_fat) cudaFree(d_fat);
     if (d_ll) cudaFree(d_ll);
-    d_sync = nullptr;
     h_state = d_state = nullptr;
-    d_aux = nullptr;
     d_fat = nullptr;
     d_ll = nullptr;
-    aux_cap = aux_valid = fat_cap = 0;
+    fat_cap = 0;
     in_fat = false;
   }
 };
 
 struct tsb_nq : Base {
   tsb_nq* sibling[3] = {nullptr, nullptr, nullptr};  // further pools on the same device, owned by this handle (tsb_nq_sibling)
-  bool aux_ok = false;  // every node of the pool has its side word (nq_expand2.cuh)
   int N = 0, g = 1;
   RoundsCtx rounds;
-  int variant = 0;  // env TSB200_NQ_VARIANT (kernel A/B experiments)
-  int tile_threads = 0;  // env TSB200_NQ_TILE_THREADS = 128: always the TMA-pipelined kernel (A/B experiments)
-  int occ[3] = {0, 0, 0};  // cached CTAs per SM, per tile size (128 / 64 / 32 threads)
-  bool attr_set[3] = {false, false, false};
+  int tile_threads = 0;  // env TSB200_NQ_TILE_THREADS = 128: always the TMA-pipelined kernel (tests force it on small chunks)
+  int occ = 0;  // cached CTAs per SM of the TMA-pipelined evaluator
+  bool attr_set = false;
   // fused expand (evaluate + generate_children on the device) and the device-resident pool
   ExpandCtx ex;
   uint8_t* d_children = nullptr;  // host-buffer expand: device image of the children
@@ -579,45 +526,37 @@ namespace {
 
 int nq_materialize(tsb_nq* h);  // (defined with the LL kernel's launch helpers below)
 
-template <int N, int VAR, int T>
-int launch_nq_nt(tsb_nq* h, int slot, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
-  auto kernel = tsb::nq_evaluate_kernel<N, VAR, T>;
-  const size_t smem = sizeof(tsb::NqSmem<N, T>) + 128;
-  if (!h->attr_set[slot]) {
+// small chunks (fewer than two 512-parent tiles per SM — the reference's default --M 50000 is 97 tiles) take the
+// one-parent-per-thread kernel, everything else the TMA-pipelined one
+template <int N>
+int launch_nq_n(tsb_nq* h, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
+  if (count < 2LL * h->di.sms * tsb::NQ_TILE && h->tile_threads != 128) {
+    const int grid = static_cast<int>((count + tsb::NQ_SMALL - 1) / tsb::NQ_SMALL);
+    tsb::nq_evaluate_small_kernel<N><<<grid, tsb::NQ_SMALL, 0, s>>>(in, out, static_cast<int>(count));
+    TSB_CUDA(cudaGetLastError());
+    h->launches++;
+    return TSB_OK;
+  }
+  auto kernel = tsb::nq_evaluate_kernel<N>;
+  const size_t smem = sizeof(tsb::NqSmem<N>) + 128;
+  if (!h->attr_set) {
     TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    h->attr_set[slot] = true;
+    h->attr_set = true;
   }
   int grid = 1;
-  int rc = grid_for(kernel, T, smem, count, T * tsb::NQ_QUAD, h->di.sms, &grid, &h->occ[slot]);
+  int rc = grid_for(kernel, tsb::NQ_THREADS, smem, count, tsb::NQ_TILE, h->di.sms, &grid, &h->occ);
   if (rc != TSB_OK) return rc;
-  kernel<<<grid, T, smem, s>>>(in, out, count);
+  kernel<<<grid, tsb::NQ_THREADS, smem, s>>>(in, out, count);
   TSB_CUDA(cudaGetLastError());
   h->launches++;
   return TSB_OK;
 }
-// small chunks (fewer than two 512-parent tiles per SM — the reference's default --M 50000 is 97 tiles) take the
-// one-parent-per-thread kernel, everything else the TMA-pipelined one
-template <int N, int VAR>
-int launch_nq_n(tsb_nq* h, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
-  if constexpr (VAR == 0) {
-    if (count < 2LL * h->di.sms * tsb::NQ_TILE && h->tile_threads != 128) {
-      const int grid = static_cast<int>((count + tsb::NQ_SMALL - 1) / tsb::NQ_SMALL);
-      tsb::nq_evaluate_small_kernel<N><<<grid, tsb::NQ_SMALL, 0, s>>>(in, out, static_cast<int>(count));
-      TSB_CUDA(cudaGetLastError());
-      h->launches++;
-      return TSB_OK;
-    }
-  }
-  return launch_nq_nt<N, VAR, 128>(h, 0, in, out, count, s);
-}
 
 int launch_nq(tsb_nq* h, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
-  if (h->N == 17 && h->variant == 1) return launch_nq_n<17, 1>(h, in, out, count, s);  // A/B experiment: byte alignment as IMAD.HI
-  if (h->N == 17 && h->variant == 2) return launch_nq_n<17, 2>(h, in, out, count, s);  // A/B experiment: bytes by LDS.U8
   switch (h->N) {
 #define TSB_NQ_CASE(n) \
   case n:              \
-    return launch_nq_n<n, 0>(h, in, out, count, s);
+    return launch_nq_n<n>(h, in, out, count, s);
     TSB_NQ_CASE(1) TSB_NQ_CASE(2) TSB_NQ_CASE(3) TSB_NQ_CASE(4) TSB_NQ_CASE(5) TSB_NQ_CASE(6) TSB_NQ_CASE(7)
     TSB_NQ_CASE(8) TSB_NQ_CASE(9) TSB_NQ_CASE(10) TSB_NQ_CASE(11) TSB_NQ_CASE(12) TSB_NQ_CASE(13)
     TSB_NQ_CASE(14) TSB_NQ_CASE(15) TSB_NQ_CASE(16) TSB_NQ_CASE(17) TSB_NQ_CASE(18) TSB_NQ_CASE(19)
@@ -653,11 +592,9 @@ int make_params(const std::vector<PoolExtent>& pieces, int tile_records, tsb::Ex
 
 // one evaluate + generate_children round over `pieces` of `arena` (count, build); children packed at
 // `children_d`.  Synchronous: the counts come back through the host-mapped result record.
-// AUX: `aux` / `children_aux` are the side arrays of `arena` / `children_d` (nq_expand2.cuh)
-template <int N, bool AUX>
-int nq_expand_n(tsb_nq* h, const uint8_t* arena, const unsigned long long* aux, const std::vector<PoolExtent>& pieces,
-                uint8_t* children_d, unsigned long long* children_aux, cudaStream_t s, unsigned long long* n_children,
-                unsigned long long* n_solutions, bool early) {
+template <int N>
+int nq_expand_n(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& pieces, uint8_t* children_d,
+                cudaStream_t s, unsigned long long* n_children, unsigned long long* n_solutions, bool early) {
   tsb::ExpandParams prm;
   int rc = make_params(pieces, tsb::NQ_TILE, &prm);
   if (rc != TSB_OK) return rc;
@@ -669,27 +606,26 @@ int nq_expand_n(tsb_nq* h, const uint8_t* arena, const unsigned long long* aux, 
   rc = ex.reserve(std::max<long long>(prm.n_tiles, h->M_max / tsb::NQ_TILE + 2 * tsb::EXP_MAX_PIECES),
                   static_cast<long long>(tsb::NQ_TILE) * N * 2, s);
   if (rc != TSB_OK) return rc;
-  auto k1 = tsb::nq_expand_count_kernel<N, AUX>;
-  auto k3 = tsb::nq_expand_build_kernel<N, AUX>;
-  const size_t smem1 = sizeof(tsb::NqCountSmem<AUX>) + 128, smem3 = sizeof(tsb::NqBuildSmem<AUX>) + 128;
-  bool& attr_set = AUX ? ex.attr_set2 : ex.attr_set;
-  if (!attr_set) {
+  auto k1 = tsb::nq_expand_count_kernel<N>;
+  auto k3 = tsb::nq_expand_build_kernel<N>;
+  const size_t smem1 = sizeof(tsb::NqCountSmem) + 128, smem3 = sizeof(tsb::NqBuildSmem) + 128;
+  if (!ex.attr_set) {
     TSB_CUDA(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem1)));
     TSB_CUDA(cudaFuncSetAttribute(k3, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem3)));
-    attr_set = true;
+    ex.attr_set = true;
   }
   const long long recs = static_cast<long long>(prm.n_tiles) * tsb::NQ_TILE;
   int g1 = 1, g3 = 1;
-  rc = grid_for(k1, tsb::NQ_THREADS, smem1, recs, tsb::NQ_TILE, h->di.sms, &g1, AUX ? &ex.occ_count2 : &ex.occ_count);
+  rc = grid_for(k1, tsb::NQ_THREADS, smem1, recs, tsb::NQ_TILE, h->di.sms, &g1, &ex.occ_count);
   if (rc != TSB_OK) return rc;
-  rc = grid_for(k3, tsb::NQ_THREADS, smem3, recs, tsb::NQ_TILE, h->di.sms, &g3, AUX ? &ex.occ_build2 : &ex.occ_build);
+  rc = grid_for(k3, tsb::NQ_THREADS, smem3, recs, tsb::NQ_TILE, h->di.sms, &g3, &ex.occ_build);
   if (rc != TSB_OK) return rc;
   prm.epoch = ++ex.epoch;
   if ((prm.n_tiles + g3 - 1) / g3 > tsb::EXP_MAX_OWN) return TSB_EINVAL;  // (M_max * N < 2^31 keeps this far away)
   uint16_t* d_items = reinterpret_cast<uint16_t*>(ex.d_cmask);
   const double tr1 = trace ? tnow() : 0;
-  k1<<<g1, tsb::NQ_THREADS, smem1, s>>>(arena, aux, prm, d_items, ex.d_tile, ex.d_st);
-  k3<<<g3, tsb::NQ_THREADS, smem3, s>>>(arena, aux, prm, d_items, ex.d_tile, children_d, children_aux, ex.d_st, ex.d_res);
+  k1<<<g1, tsb::NQ_THREADS, smem1, s>>>(arena, prm, d_items, ex.d_tile, ex.d_st);
+  k3<<<g3, tsb::NQ_THREADS, smem3, s>>>(arena, prm, d_items, ex.d_tile, children_d, ex.d_st, ex.d_res);
   TSB_CUDA(cudaGetLastError());
   h->launches += 2;
   const double tr2 = trace ? tnow() : 0;
@@ -707,13 +643,11 @@ int nq_expand_n(tsb_nq* h, const uint8_t* arena, const unsigned long long* aux, 
 }
 
 int nq_expand_dispatch(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& pieces, uint8_t* children_d,
-                       cudaStream_t s, unsigned long long* nc, unsigned long long* ns, bool early = false,
-                       const unsigned long long* aux = nullptr, unsigned long long* children_aux = nullptr) {
+                       cudaStream_t s, unsigned long long* nc, unsigned long long* ns, bool early = false) {
   switch (h->N) {
-#define TSB_NQ_CASE(n)                                                                                   \
-  case n:                                                                                                \
-    return aux ? nq_expand_n<n, true>(h, arena, aux, pieces, children_d, children_aux, s, nc, ns, early) \
-               : nq_expand_n<n, false>(h, arena, nullptr, pieces, children_d, nullptr, s, nc, ns, early);
+#define TSB_NQ_CASE(n) \
+  case n:              \
+    return nq_expand_n<n>(h, arena, pieces, children_d, s, nc, ns, early);
     TSB_NQ_CASE(1) TSB_NQ_CASE(2) TSB_NQ_CASE(3) TSB_NQ_CASE(4) TSB_NQ_CASE(5) TSB_NQ_CASE(6) TSB_NQ_CASE(7)
     TSB_NQ_CASE(8) TSB_NQ_CASE(9) TSB_NQ_CASE(10) TSB_NQ_CASE(11) TSB_NQ_CASE(12) TSB_NQ_CASE(13)
     TSB_NQ_CASE(14) TSB_NQ_CASE(15) TSB_NQ_CASE(16) TSB_NQ_CASE(17) TSB_NQ_CASE(18) TSB_NQ_CASE(19)
@@ -1184,7 +1118,7 @@ int tsb_init_devices(int n) {
     // the library's kernels are loaded lazily, as one module, at the first launch (~15 ms): do it here, where
     // the Chapel runtime loads its own GPU code — at program start, outside the drivers' timers
     cudaFuncAttributes fa;
-    TSB_CUDA(cudaFuncGetAttributes(&fa, tsb::nq_evaluate_kernel<1, 0>));
+    TSB_CUDA(cudaFuncGetAttributes(&fa, tsb::nq_evaluate_kernel<1>));
   }
   // peer access between the devices of a multi-GPU search, once and before any timer (the first
   // cudaDeviceEnablePeerAccess of a pair takes milliseconds): steals between device pools then go GPU to GPU
@@ -1209,7 +1143,6 @@ int tsb_nq_create(tsb_nq** out, int device, int N, int g, int M_max) {
   if (!h) return TSB_ENOMEM;
   h->N = N;
   h->g = g;
-  if (const char* v = std::getenv("TSB200_NQ_VARIANT")) h->variant = std::atoi(v);
   if (const char* v = std::getenv("TSB200_NQ_TILE_THREADS")) h->tile_threads = std::atoi(v);
   int rc = h->init(device, M_max, sizeof(tsb_nq_node), static_cast<size_t>(N));
   if (rc != TSB_OK) {
@@ -1289,54 +1222,9 @@ long long nq_pool_min_cap(const tsb_nq* h) {
   if (const long long c = env_pool_cap(); c > 0) return c;
   return std::max<long long>(1LL << 22, 4LL * h->M_max * h->N);
 }
-// A/B experiment, off by default (TSB200_AUX=1 turns it on): one side word per node (nq_expand2.cuh).  The
-// instructions it saves in the count kernel are paid back as more bytes per node (see nq_expand2.cuh).
-bool env_aux() {
-  static const bool v = [] {
-    const char* e = std::getenv("TSB200_AUX");
-    return e && *e && *e != '0';
-  }();
-  return v;
-}
 void nq_pool_setup(tsb_nq* h) {
   h->pool.rec = sizeof(tsb_nq_node);
   h->pool.slack = static_cast<size_t>(tsb::NQ_TILE) * sizeof(tsb_nq_node);  // full-tile loads may run past the top
-  if (env_aux()) {
-    h->pool.side_rec = sizeof(unsigned long long);
-    h->pool.side_slack = static_cast<size_t>(tsb::NQ_TILE) * sizeof(unsigned long long);
-  }
-}
-template <int N>
-int nq_aux_fill_n(tsb_nq* h, long long lo, long long hi) {
-  if (hi <= lo) return TSB_OK;
-  const long long blocks = std::min<long long>((hi - lo + 255) / 256, 64LL * h->di.sms);
-  tsb::nq_aux_fill_kernel<N><<<static_cast<unsigned>(blocks), 256, 0, h->stream>>>(
-      h->pool.arena[h->pool.cur], reinterpret_cast<unsigned long long*>(h->pool.side[h->pool.cur]), lo, hi);
-  TSB_CUDA(cudaGetLastError());
-  h->launches++;
-  return TSB_OK;
-}
-int nq_aux_fill(tsb_nq* h, long long lo, long long hi) {
-  switch (h->N) {
-#define TSB_NQ_CASE(n) \
-  case n:              \
-    return nq_aux_fill_n<n>(h, lo, hi);
-    TSB_NQ_CASE(1) TSB_NQ_CASE(2) TSB_NQ_CASE(3) TSB_NQ_CASE(4) TSB_NQ_CASE(5) TSB_NQ_CASE(6) TSB_NQ_CASE(7)
-    TSB_NQ_CASE(8) TSB_NQ_CASE(9) TSB_NQ_CASE(10) TSB_NQ_CASE(11) TSB_NQ_CASE(12) TSB_NQ_CASE(13)
-    TSB_NQ_CASE(14) TSB_NQ_CASE(15) TSB_NQ_CASE(16) TSB_NQ_CASE(17) TSB_NQ_CASE(18) TSB_NQ_CASE(19)
-    TSB_NQ_CASE(20)
-#undef TSB_NQ_CASE
-  }
-  return TSB_EINVAL;
-}
-// side words for every node of the pool (after host pushes into a pool whose words were stale, a steal, the
-// persistent kernel's export)
-int nq_aux_ensure(tsb_nq* h) {
-  if (h->aux_ok || !h->pool.side_rec) return TSB_OK;
-  for (const PoolExtent& x : h->pool.ext)
-    if (int rc = nq_aux_fill(h, x.b, x.e); rc != TSB_OK) return rc;
-  h->aux_ok = true;
-  return TSB_OK;
 }
 // what a pool may hold: depth <= N, board[0..N) < N, the bytes past N zero (every node the reference or this library
 // creates; the persistent kernel packs a node into 125 bits on these terms, nq_rounds_ll.cuh)
@@ -1359,7 +1247,6 @@ int tsb_nq_pool_push(tsb_nq* h, const void* nodes, int64_t n) {
   nq_pool_setup(h);
   int rc = nq_materialize(h);
   if (rc != TSB_OK) return rc;
-  h->rounds.aux_valid = 0;  // (the side words of the persistent kernel describe the pool it left behind)
   rc = h->pool.reserve(h->stream, n, nq_pool_min_cap(h));
   if (rc != TSB_OK) return rc;
   if (n == 0) return TSB_OK;
@@ -1368,13 +1255,11 @@ int tsb_nq_pool_push(tsb_nq* h, const void* nodes, int64_t n) {
   rc = h->copy_h2d(h->pool.arena[h->pool.cur] + at * sizeof(tsb_nq_node), nodes,
                    static_cast<size_t>(n) * sizeof(tsb_nq_node), h->stream);
   if (rc != TSB_OK) return rc;
-  if (h->pool.size == 0) h->aux_ok = true;  // (nothing else to describe)
   if (h->pool.ext.empty())
     h->pool.ext.push_back({at, at + n});
   else
     h->pool.ext.back().e += n;
   h->pool.size += n;
-  if (h->aux_ok && h->pool.side_rec) return nq_aux_fill(h, at, at + n);  // (ordered after the copy on the handle's stream)
   return TSB_OK;
 }
 
@@ -1389,7 +1274,6 @@ int tsb_nq_pool_step(tsb_nq* h, int m, int M, int64_t* n_parents, uint64_t* n_ch
   TSB_CUDA(cudaSetDevice(h->device));
   int rc = nq_materialize(h);
   if (rc != TSB_OK) return rc;
-  h->rounds.aux_valid = 0;
   const long long n = std::min<long long>(p.size, M);
   // room above the top for the worst case (every slot of every parent survives); the chunk itself is read
   // in place, as the newest pieces of the extent stack
@@ -1403,15 +1287,7 @@ int tsb_nq_pool_step(tsb_nq* h, int m, int M, int64_t* n_parents, uint64_t* n_ch
   const long long top = p.top();
   unsigned long long nc = 0, ns = 0;
   uint8_t* arena = p.arena[p.cur];
-  if (p.side_rec) {  // every node evaluated once, when it is built (nq_expand2.cuh)
-    rc = nq_aux_ensure(h);
-    if (rc != TSB_OK) return rc;
-    unsigned long long* side = reinterpret_cast<unsigned long long*>(p.side[p.cur]);
-    rc = nq_expand_dispatch(h, arena, pieces, arena + top * sizeof(tsb_nq_node), h->stream, &nc, &ns, /*early=*/true, side,
-                            side + top);
-  } else {
-    rc = nq_expand_dispatch(h, arena, pieces, arena + top * sizeof(tsb_nq_node), h->stream, &nc, &ns, /*early=*/true);
-  }
+  rc = nq_expand_dispatch(h, arena, pieces, arena + top * sizeof(tsb_nq_node), h->stream, &nc, &ns, /*early=*/true);
   if (rc != TSB_OK) return rc;
   pool_pop(p, n);
   if (nc) {
@@ -1426,38 +1302,6 @@ int tsb_nq_pool_step(tsb_nq* h, int m, int M, int64_t* n_parents, uint64_t* n_ch
 
 }  // extern "C"
 namespace {
-template <int N, int T>
-int nq_rounds_launch_nt(tsb_nq* h, const tsb::RoundsParams& prm, int grid, cudaStream_t s) {
-  auto kernel = tsb::nq_rounds_kernel<N, T>;
-  const size_t smem = sizeof(tsb::RoundsSmem<T>) + 128;
-  if (!h->rounds.attr_set) {
-    TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    h->rounds.attr_set = true;
-  }
-  void* args[] = {const_cast<tsb::RoundsParams*>(&prm)};
-  // cooperative: all CTAs co-resident (they exchange flags through L2), or the launch fails
-  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid), dim3(T), args, smem, s));
-  h->launches++;
-  return TSB_OK;
-}
-template <int N>
-int nq_rounds_launch_n(tsb_nq* h, const tsb::RoundsParams& prm, int grid, cudaStream_t s) {
-  if (h->rounds.threads == 256) return nq_rounds_launch_nt<N, 256>(h, prm, grid, s);
-  return nq_rounds_launch_nt<N, 512>(h, prm, grid, s);
-}
-int nq_rounds_launch(tsb_nq* h, const tsb::RoundsParams& prm, int grid, cudaStream_t s) {
-  switch (h->N) {
-#define TSB_NQ_CASE(n) \
-  case n:              \
-    return nq_rounds_launch_n<n>(h, prm, grid, s);
-    TSB_NQ_CASE(1) TSB_NQ_CASE(2) TSB_NQ_CASE(3) TSB_NQ_CASE(4) TSB_NQ_CASE(5) TSB_NQ_CASE(6) TSB_NQ_CASE(7)
-    TSB_NQ_CASE(8) TSB_NQ_CASE(9) TSB_NQ_CASE(10) TSB_NQ_CASE(11) TSB_NQ_CASE(12) TSB_NQ_CASE(13)
-    TSB_NQ_CASE(14) TSB_NQ_CASE(15) TSB_NQ_CASE(16) TSB_NQ_CASE(17) TSB_NQ_CASE(18) TSB_NQ_CASE(19)
-    TSB_NQ_CASE(20)
-#undef TSB_NQ_CASE
-  }
-  return TSB_EINVAL;
-}
 template <int N>
 int nq_ll_launch_n(tsb_nq* h, const tsb::LlMultiParams& prm, int grid, int pools, int ppt, cudaStream_t s) {
   // (one pool: the 160-register build, one CTA per SM; several: capped at 128 registers for two CTAs per SM; three
@@ -1527,7 +1371,6 @@ int nq_materialize(tsb_nq* h) {
     TSB_CUDA(cudaStreamSynchronize(h->stream));
   }
   h->rounds.in_fat = false;
-  h->aux_ok = false;  // (the exported nodes carry no side words)
   return TSB_OK;
 }
 bool env_no_rounds() {
@@ -1536,17 +1379,17 @@ bool env_no_rounds() {
 }
 // grid (CTAs per pool) of the persistent kernel for chunks of up to M parents when one launch serves `pools` pools;
 // 0: M is too large for it.  Chosen on the N = 17 search at M = 50000: one pool: 7/8 of the SMs
-// (one CTA per SM); two pools: one CTA per SM each (two per SM in all); four pools: SMs / 2 CTAs each.
+// (one CTA per SM); two pools: one CTA per SM each (two per SM in all); four pools: SMs / 2 CTAs each.  An all-to-all
+// flag exchange among all SMs' CTAs costs 2-3x one among half of them (tools/flag_exchange.py); the per-CTA work grows
+// the other way.
 // *ppt: parents per thread of the kernel variant to launch (2, or 3 when the pool's CTAs would not cover M with 2).
 int nq_ll_grid(const tsb_nq* h, int M, int pools, int* ppt = nullptr) {
   if (!h->di.coop || env_no_rounds() || pools < 1 || pools > tsb::LL_MAX_POOLS) return 0;
-  const int sms = std::min(h->di.sms, static_cast<int>(tsb::RND_MAX_CTAS));
-  int most = tsb::ll_ctas_per_pool(sms, pools);  // (ll_tiers.h: the drivers size their warm-up by the same tiers)
-  int per = static_cast<long long>(most) * tsb::ll_slice(2) >= M ? 2 : 3;
-  if (pools > 1 && h->rounds.ppt == 3) per = 3;
+  const int sms = std::min(h->di.sms, tsb::LL_MAX_SMS);
+  const int most = tsb::ll_ctas_per_pool(sms, pools);  // (ll_tiers.h: the drivers size their warm-up by the same tiers)
+  const int per = static_cast<long long>(most) * tsb::ll_slice(2) >= M ? 2 : 3;
   const int slice = tsb::ll_slice(per);
   int grid = pools == 1 ? std::max(1, (sms * 7 / 8) & ~1) : most;
-  if (h->rounds.ctas > 0) grid = std::min(most, h->rounds.ctas);
   while (static_cast<long long>(grid) * slice < M && grid < most) ++grid;  // (M decides)
   if (ppt) *ppt = per;
   return static_cast<long long>(M) <= static_cast<long long>(grid) * slice && (pools > 1 || per == 2) ? grid : 0;
@@ -1562,7 +1405,7 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
     left[i] = max_rounds;
     active[i] = true;
     nq_pool_setup(hs[i]);
-    int rc = hs[i]->rounds.ensure(hs[i]->stream);
+    int rc = hs[i]->rounds.ensure();
     if (rc != TSB_OK) return rc;
   }
   const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
@@ -1663,98 +1506,28 @@ int tsb_nq_pool_run(tsb_nq* h, int m, int M, int64_t max_rounds, uint64_t* n_rou
   if (!h || m < 1 || M < 1 || M > h->M_max || max_rounds < 0 || !n_rounds || !n_parents || !n_children || !n_solutions)
     return TSB_EINVAL;
   *n_rounds = *n_parents = *n_children = *n_solutions = 0;
-  DevicePool& p = h->pool;
   TSB_CUDA(cudaSetDevice(h->device));
-  int rc = h->rounds.ensure(h->stream);
-  if (rc != TSB_OK) return rc;
-  int grid = std::min(h->di.sms, static_cast<int>(tsb::RND_MAX_CTAS));
-  if (h->rounds.version == 3)  // 7/8 of the SMs: a smaller count exchange
-    grid = h->rounds.ctas > 0 ? std::min(grid, h->rounds.ctas) : std::max(1, (grid * 7 / 8) & ~1);
-  else
-    grid = h->rounds.ctas > 0 ? std::min(grid, h->rounds.ctas) : std::max(1, 2 * grid / 3);
-  while (static_cast<long long>(grid) * h->rounds.threads * tsb::RND_PPT < M && grid < h->di.sms) ++grid;  // (M decides)
-  const bool persistent = static_cast<long long>(M) <= static_cast<long long>(grid) * h->rounds.threads * tsb::RND_PPT &&
-                          h->di.coop && !env_no_rounds();
-  if (!persistent) {  // large chunks: one round = two bandwidth-bound kernels (tsb_nq_pool_step)
-    while (static_cast<int64_t>(*n_rounds) < max_rounds) {
-      int64_t np = 0;
-      uint64_t nc = 0, ns = 0;
-      int rc = tsb_nq_pool_step(h, m, M, &np, &nc, &ns);
-      if (rc != TSB_OK) return rc;
-      if (np == 0) break;
-      ++*n_rounds;
-      *n_parents += static_cast<uint64_t>(np);
-      *n_children += nc;
-      *n_solutions += ns;
-    }
-    return TSB_OK;
-  }
-  nq_pool_setup(h);
-  if (h->rounds.version == 3 && nq_ll_grid(h, M, 1) > 0) {
-    // ---- the fence-free kernel on the fat arena (nq_rounds_ll.cuh)
+  if (nq_ll_grid(h, M, 1) > 0) {  // the whole loop in launches of the persistent kernel (nq_rounds_ll.cuh)
     uint64_t out[4] = {0, 0, 0, 0};
     tsb_nq* one[1] = {h};
-    rc = nq_ll_run_multi(one, 1, m, M, max_rounds, out);
+    const int rc = nq_ll_run_multi(one, 1, m, M, max_rounds, out);
     *n_rounds = out[0];
     *n_parents = out[1];
     *n_children = out[2];
     *n_solutions = out[3];
     return rc;
   }
-  nq_pool_setup(h);
-  while (p.size >= m && static_cast<int64_t>(*n_rounds) < max_rounds) {
-    // the kernel works on ONE contiguous stack [0, size) with room for the worst case of the next round
-    const long long n = std::min<long long>(p.size, M);
-    const long long need = p.size - n + n * h->N;
-    if (need > p.cap) {
-      rc = p.compact(h->stream, std::max<long long>(2 * p.cap, need + need / 2));
-      h->rounds.aux_valid = 0;
-    } else if (p.ext.size() != 1 || p.ext[0].b != 0) {
-      rc = p.compact(h->stream, p.cap);
-      h->rounds.aux_valid = 0;
-    }
-    if (rc == TSB_OK) rc = h->rounds.ensure_aux(p.cap);
+  // large chunks: one round = two bandwidth-bound kernels (tsb_nq_pool_step)
+  while (static_cast<int64_t>(*n_rounds) < max_rounds) {
+    int64_t np = 0;
+    uint64_t nc = 0, ns = 0;
+    int rc = tsb_nq_pool_step(h, m, M, &np, &nc, &ns);
     if (rc != TSB_OK) return rc;
-    tsb::RoundsParams prm;
-    prm.aux = h->rounds.d_aux;
-    prm.aux_valid = std::min(h->rounds.aux_valid, p.size);
-    prm.arena = p.arena[p.cur];
-    prm.cap = p.cap;
-    prm.size0 = p.size;
-    prm.epoch0 = h->rounds.epoch;
-    prm.m = m;
-    prm.M = M;
-    prm.max_rounds = max_rounds - static_cast<int64_t>(*n_rounds);
-    prm.prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
-    prm.sync = h->rounds.d_sync;
-    prm.state = h->rounds.d_state;
-    h->rounds.h_state->exit_code = -1;
-    rc = nq_rounds_launch(h, prm, grid, h->stream);
-    if (rc != TSB_OK) return rc;
-    TSB_CUDA(cudaStreamSynchronize(h->stream));
-    const tsb::RoundsState st = *h->rounds.h_state;
-    if (st.exit_code < 0 || st.exit_code == tsb::RND_EXIT_ABORT) {
-      g_last_cuda_error = "nq_rounds_kernel: watchdog abort (a flag exchange did not complete)";
-      return TSB_ECUDA;
-    }
-    if (prm.prof)
-      std::fprintf(stderr, "[tsb200] rounds kernel: %llu rounds; CTA 0 cycles per round: wait-done %.0f load %.0f eval+scan %.0f "
-                   "gather %.0f build+store %.0f release %.0f\n", static_cast<unsigned long long>(st.rounds),
-                   1.0 * st.prof[0] / std::max<unsigned long long>(1, st.rounds), 1.0 * st.prof[1] / std::max<unsigned long long>(1, st.rounds),
-                   1.0 * st.prof[2] / std::max<unsigned long long>(1, st.rounds), 1.0 * st.prof[3] / std::max<unsigned long long>(1, st.rounds),
-                   1.0 * st.prof[4] / std::max<unsigned long long>(1, st.rounds), 1.0 * st.prof[5] / std::max<unsigned long long>(1, st.rounds));
-    h->rounds.epoch = st.epoch;
-    h->aux_ok = false;
-    h->rounds.aux_valid = st.size;
-    p.size = st.size;
-    p.ext.clear();
-    if (p.size) p.ext.push_back({0, p.size});
-    *n_rounds += st.rounds;
-    *n_parents += st.parents;
-    *n_children += st.children;
-    *n_solutions += st.solutions;
-    if (st.exit_code == tsb::RND_EXIT_SPACE && st.rounds == 0 && need <= p.cap) return TSB_ENOMEM;  // (cannot happen)
-    if (st.exit_code != tsb::RND_EXIT_SPACE) break;  // DONE or PAUSE
+    if (np == 0) break;
+    ++*n_rounds;
+    *n_parents += static_cast<uint64_t>(np);
+    *n_children += nc;
+    *n_solutions += ns;
   }
   return TSB_OK;
 }
@@ -1770,7 +1543,7 @@ int tsb_nq_sibling(tsb_nq* h, int index, tsb_nq** sibling) {
 }
 
 int tsb_nq_pools_per_launch(const tsb_nq* h, int M) {
-  if (!h || M < 1 || M > h->M_max || h->rounds.version != 3) return 1;
+  if (!h || M < 1 || M > h->M_max) return 1;
   for (int pools = tsb::LL_MAX_POOLS; pools > 1; pools--)
     if (nq_ll_grid(h, M, pools) > 0) return pools;
   return 1;
@@ -1786,8 +1559,7 @@ int tsb_nq_pool_run_multi(tsb_nq* const* handles, int n_pools, int m, int M, int
   }
   std::memset(out, 0, sizeof(uint64_t) * 4 * n_pools);
   TSB_CUDA(cudaSetDevice(handles[0]->device));
-  const int grid = handles[0]->rounds.version == 3 ? nq_ll_grid(handles[0], M, n_pools) : 0;
-  if (grid == 0) {  // chunks too large for the persistent kernel with this many pools: one pool after the other
+  if (nq_ll_grid(handles[0], M, n_pools) == 0) {  // chunks too large for the persistent kernel with this many pools: one pool after the other
     for (int i = 0; i < n_pools; i++) {
       int rc = tsb_nq_pool_run(handles[i], m, M, max_rounds, &out[4 * i], &out[4 * i + 1], &out[4 * i + 2], &out[4 * i + 3]);
       if (rc != TSB_OK) return rc;
@@ -1809,16 +1581,13 @@ int tsb_nq_pool_steal(tsb_nq* victim, tsb_nq* thief, int m, int64_t* n_stolen) {
   int rc = nq_materialize(victim);
   if (rc == TSB_OK) rc = nq_materialize(thief);
   if (rc != TSB_OK) return rc;
-  victim->rounds.aux_valid = 0;
-  thief->rounds.aux_valid = 0;
   rc = pool_steal_front(victim->pool, victim->device, victim->stream, thief->pool, thief->device, thief->stream, m,
                             nq_pool_min_cap(thief), &n);
   *n_stolen = n;
-  if (n) thief->aux_ok = false;  // (the stolen nodes arrive without side words: filled before the thief's next round)
   return rc;
 }
 
-// diagnostics: cycles per round of the bare flag-exchange skeleton of the persistent kernel (nq_rounds.cuh)
+// diagnostics: cycles per round of bare flag exchanges among co-resident CTAs (rounds_sync_bench_kernel, nq_rounds_ll.cuh)
 int tsb_debug_flag_exchange(int device, int rounds, int variant, int ctas, double* cycles_per_round) {
   if (!cycles_per_round || rounds < 1) return TSB_EINVAL;
   DeviceInfo di;
@@ -1828,10 +1597,10 @@ int tsb_debug_flag_exchange(int device, int rounds, int variant, int ctas, doubl
   tsb::RoundsSync* sy = nullptr;
   uint4* scratch = nullptr;
   long long* d_out = nullptr;
-  int grid = std::min(di.sms, static_cast<int>(tsb::RND_MAX_CTAS));
+  int grid = std::min(di.sms, tsb::LL_MAX_SMS);
   if (ctas > 0 && ctas < grid) grid = ctas;
   TSB_CUDA(cudaMalloc(&sy, sizeof(*sy)));
-  const size_t scratch_bytes = std::max<size_t>((static_cast<size_t>(grid) * tsb::RND_THREADS + 2) * sizeof(uint4), 2 * 256 * 256 * 4);
+  const size_t scratch_bytes = std::max<size_t>((static_cast<size_t>(grid) * tsb::LL_T + 2) * sizeof(uint4), 2 * 256 * 256 * 4);
   TSB_CUDA(cudaMalloc(&scratch, scratch_bytes));
   TSB_CUDA(cudaMemset(scratch, 0, scratch_bytes));
   TSB_CUDA(cudaMalloc(&d_out, sizeof(long long)));
@@ -1839,7 +1608,7 @@ int tsb_debug_flag_exchange(int device, int rounds, int variant, int ctas, doubl
   unsigned epoch0 = 0;
   void* args[] = {&sy, &epoch0, &rounds, &variant, &scratch, &d_out};
   cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(tsb::rounds_sync_bench_kernel), dim3(grid),
-                                              dim3(tsb::RND_THREADS), args, 0, nullptr);
+                                              dim3(tsb::LL_T), args, 0, nullptr);
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   long long cyc = 0;
   if (e == cudaSuccess) e = cudaMemcpy(&cyc, d_out, sizeof(cyc), cudaMemcpyDeviceToHost);

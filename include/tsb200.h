@@ -144,8 +144,9 @@ int tsb_nq_pool_drain(tsb_nq* h, void* nodes, int64_t capacity_nodes, int64_t* n
 /* rounds until the pool holds fewer than m nodes (or max_rounds are done): exactly the sequence of
  * tsb_nq_pool_step rounds — the same chunks, the same pool after every round — but for chunk sizes up to
  * 512 x #SMs (the reference's default --M 50000) the whole loop of nqueens_gpu_chpl.chpl:197-215 runs inside ONE
- * persistent cooperative kernel (two flag exchanges through L2 per round instead of two launches and a host
- * round trip); larger M falls back to one tsb_nq_pool_step per round.  Totals over the rounds come back. */
+ * persistent cooperative kernel (per round one exchange of the child counts among its CTAs plus one store -> L2 ->
+ * poll hop of the self-validating nodes, instead of two launches and a host round trip); larger M falls back to one
+ * tsb_nq_pool_step per round.  Totals over the rounds come back. */
 /* work stealing between two device pools (the reference steals between its per-GPU host pools,
  * nqueens_multigpu_chpl.chpl:255-312): if the victim holds >= 2 m nodes, the oldest size / 2 of them
  * (popFrontBulkFree, lib/commons/Pool_par.chpl:178-191) move to the top of the thief's pool, device to device
@@ -183,9 +184,11 @@ uint64_t tsb_nq_kernel_launches(const tsb_nq* h); /* kernels launched through th
 void* tsb_nq_stream(const tsb_nq* h); /* the handle's cudaStream_t: the pool / expand / host-buffer entry points launch
                                         * on it (to bracket them with CUDA events) */
 
-/* diagnostics: SM cycles per round of the bare two-flag-exchange skeleton of the persistent multi-round kernel
- * (no evaluation, no children) — the floor under a round of tsb_nq_pool_run; variant bits: 1 = no release fence,
- * 2 = no acquire fence, 4 = 16 bytes per thread stored before the release, 8 = weak L2 polls, 16 = one exchange */
+/* diagnostics: SM cycles per round of bare all-to-all flag exchanges among `ctas` co-resident CTAs (no evaluation,
+ * no children): by default two exchanges per round, the second ordered by a release store and an acquire fence —
+ * what ordering rounds with fences would cost — and what one exchange among fewer CTAs costs (the measurement behind
+ * the persistent kernel's CTA counts).  variant bits: 1 = no release fence, 2 = no acquire fence, 4 = 16 bytes per
+ * thread stored before the release, 8 = weak L2 polls, 16 = one exchange, 32 = one exchange through per-reader rows */
 int tsb_debug_flag_exchange(int device, int rounds, int variant, int ctas /* 0 = one per SM */, double* cycles_per_round);
 
 /* ------------------------------------------------------------------ PFSP ----------------- */

@@ -164,25 +164,6 @@ def test_pool_run_multi_equals_separate_pool_runs(N, m, M, K):
             ev.close()
 
 
-def test_side_word_variant_of_the_round_kernels_counts():
-    """TSB200_AUX=1 (A/B experiment, nq_expand2.cuh: each node's diagonals kept in a side array, the count kernel reads
-    them instead of walking the board): same counts and chunk sequence; read once per process, hence the subprocess"""
-    import subprocess
-    import sys
-    code = ("import sys; sys.path[:0] = [%r, %r]; import tsb200; "
-            "st = tsb200.nqueens_search_device(14, 1, 25, 1 << 17, 1); "
-            "print(st.explored_tree, st.explored_sol, st.offloads, st.kernel_launches)") % (
-                os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
-                os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpu-accelerated-tree-search-chapel_b200"))
-    env = dict(os.environ, TSB200_AUX="1", TSB200_NO_STEAL="1", TSB200_POOLS="1")
-    out = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0, out.stderr[-2000:]
-    tree, sol, offloads, launches = map(int, out.stdout.split())
-    ref = po.nq_search_offload(14, 1, 25, 1 << 17, 1)
-    assert (tree, sol) == (27358552, 365596) and offloads == ref.offloads
-    assert launches == 2 * offloads + 1  # count, build per round + the side words of the root
-
-
 @pytest.mark.parametrize("N,m,M,D", [(13, 25, 2000, 3), (14, 25, 50000, 4), (15, 25, 50000, 8), (15, 25, 1 << 18, 4),
                                      (12, 5, 300, 2)])
 def test_device_resident_search_with_work_stealing(golden_dir, N, m, M, D):

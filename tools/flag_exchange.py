@@ -1,4 +1,6 @@
-"""cycles per round of the bare flag-exchange skeleton of the persistent multi-round kernel (nq_rounds.cuh):
+"""cycles per round of bare all-to-all flag exchanges among co-resident CTAs (tsb_debug_flag_exchange): what ordering
+rounds with release / acquire fences costs, and how one exchange scales with the number of CTAs (the persistent
+N-Queens kernel's CTA counts rest on it):
 python tools/flag_exchange.py [variant[:ctas] ...]"""
 import ctypes as C, sys
 sys.path.insert(0, "gpu-accelerated-tree-search-chapel_b200")

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Wall time of whole device-pool searches: python tools/search_time.py N M [reps [D]]   (env knobs apply, e.g. TSB200_AUX=1)"""
+"""Wall time of whole device-pool searches: python tools/search_time.py N M [reps [D]]   (env knobs apply, e.g. TSB200_POOLS=1)"""
 import os
 import sys
 import time
