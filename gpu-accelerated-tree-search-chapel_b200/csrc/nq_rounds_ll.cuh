@@ -42,7 +42,9 @@
 // CTA that scans the counts and writes every worker its own result line (two contention-free hops, no gain),
 // per-reader rows that only their owner polls (no gain), CTAs of 512 threads (slower scan), fewer CTAs (cheaper
 // exchange, more work per CTA: the default uses 7/8 of the SMs), a sentinel poll (one lane per warp watches one piece
-// and the full sweeps start when it has arrived: the extra hop costs more than the poll traffic it saves).
+// and the full sweeps start when it has arrived: the extra hop costs more than the poll traffic it saves).  Taking the
+// exchange out of the round altogether, with the next round's counts published next to the children, measured 1.65x
+// slower (DESIGN §5): the in-place stores then need their own "every slice read" wait, and the build is no longer hidden.
 //
 // The plain 21-byte arena is converted
 // to and from the fat arena by nq_fat_import / nq_fat_export (whole pool, only when the host needs the plain form:
@@ -229,22 +231,34 @@ __device__ __forceinline__ bool warp_gather_slots2(const unsigned long long* slo
                                                    unsigned* abort_flag, unsigned long long& before0,
                                                    unsigned long long& before1, unsigned long long& all) {
   const int lane = threadIdx.x & 31;
+  // slot pairs per lane in flight: a sweep of up to 64 B slots (2 G on GPUs of up to 160 SMs) is ONE L2 round trip.
+  // (A loop that sums each pair before it loads the next one issued them one after the other: two or three dependent
+  // round trips per sweep at 2 G = 132, all of the last sweep exposed in the round.)
+  constexpr int B = 5;
   SpinGuard guard;
   for (;;) {
     bool ok = true;
     before0 = before1 = all = 0;
-    for (int i = 2 * lane; i < n; i += 64) {
-      unsigned long long v0, v1;
-      asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(v0), "=l"(v1) : "l"(slot + i) : "memory");
-      const bool has1 = i + 1 < n;
-      ok &= static_cast<unsigned>(v0 >> 32) == epoch && (!has1 || static_cast<unsigned>(v1 >> 32) == epoch);
-      const unsigned long long p0 = (v0 & 0xFFFFFull) | ((v0 >> 20) & 0xFFFull) << 32;
-      const unsigned long long p1 = has1 ? (v1 & 0xFFFFFull) | ((v1 >> 20) & 0xFFFull) << 32 : 0ull;
-      all += p0 + p1;
-      if (i < k0) before0 += p0;
-      if (i + 1 < k0) before0 += p1;
-      if (i < k1) before1 += p0;
-      if (i + 1 < k1) before1 += p1;
+    for (int i0 = 2 * lane; i0 < n; i0 += 64 * B) {
+      unsigned long long v0[B], v1[B];
+#pragma unroll
+      for (int u = 0; u < B; u++)
+        if (i0 + 64 * u < n)
+          asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(v0[u]), "=l"(v1[u]) : "l"(slot + i0 + 64 * u) : "memory");
+#pragma unroll
+      for (int u = 0; u < B; u++) {
+        const int i = i0 + 64 * u;
+        if (i >= n) break;
+        const bool has1 = i + 1 < n;
+        ok &= static_cast<unsigned>(v0[u] >> 32) == epoch && (!has1 || static_cast<unsigned>(v1[u] >> 32) == epoch);
+        const unsigned long long p0 = (v0[u] & 0xFFFFFull) | ((v0[u] >> 20) & 0xFFFull) << 32;
+        const unsigned long long p1 = has1 ? (v1[u] & 0xFFFFFull) | ((v1[u] >> 20) & 0xFFFull) << 32 : 0ull;
+        all += p0 + p1;
+        if (i < k0) before0 += p0;
+        if (i + 1 < k0) before0 += p1;
+        if (i < k1) before1 += p0;
+        if (i + 1 < k1) before1 += p1;
+      }
     }
     if (__all_sync(0xFFFFFFFFu, ok)) break;
     if (__any_sync(0xFFFFFFFFu, guard.expired(abort_flag))) return false;
