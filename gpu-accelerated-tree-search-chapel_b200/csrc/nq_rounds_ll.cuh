@@ -20,7 +20,7 @@
 //     data32[3] bits 10..29: the node's child mask (slot k set <=> k >= depth and board[k] is not attacked: evaluate_gpu's
 //     label for slot k, nqueens_gpu_chpl.chpl:97-123), bit 30: leaf (depth == N)
 //   The diagonal masks of a parent (what its next row attacks) are not stored: a round recomputes them from the placed
-//   prefix, O(depth), for the parents that have children, while the child counts are on their way; a child's masks
+//   prefix, O(depth) independent terms (ll_parent_diag), while the child counts are on their way; a child's masks
 //   follow from its parent's in O(1) (ll_build_child), and its child mask is evaluated when it is built.  (The earlier
 //   version stored the masks in a side word next to each 21-byte node: 64 bytes per node, twice the poll loads and
 //   store pieces of a round.)
@@ -276,7 +276,7 @@ template <int T, int PPT>
 struct LlSmem {
   alignas(16) uint4 parent[T * PPT];   // the slice: data32[0..3] of every parent
   alignas(16) uint4 stage[LL_CAP];     // the window's children: data32[0..3]
-  alignas(8) uint2 diag[T * PPT];      // {ld, rd} of every parent that has children (ll_parent_diag)
+  alignas(8) uint2 diag[T * PPT];      // {ld, rd} of every parent (ll_parent_diag; read for those with children)
   alignas(16) uint16_t item[T * PPT * 20];  // (record << 5) | slot, in child order
   unsigned long long warp_tot64[T / 32];
   unsigned long long red[3];
@@ -286,20 +286,26 @@ struct LlSmem {
 };
 
 // the values a parent's next row (row `depth`) attacks along the rising (ld) and falling (rd) diagonals of its placed
-// rows 0 .. depth-1: every row's queen moves one value further per row, as ll_build_child moves its parent's masks
+// rows 0 .. depth-1: the queen of row i attacks board[i] + (depth - i) and board[i] - (depth - i) there.  Each row's
+// term is computed on its own and the terms are ORed, with ld masked to N bits once: bits that leave [0, N) never
+// come back, so this equals moving the masks row by row as ll_build_child does (ld = ((ld | bit) << 1) mod 2^N,
+// rd = (rd | bit) >> 1), without that chain of ~3 dependent operations per row.  The variable shifts are products
+// with 2^(depth-1-i) (ld) and the high word of one with 2^(32-depth+i) (rd): multiplies run on the FMA pipe, beside
+// the shifts and ORs on the integer pipe, and the factors, shifted by the constant i, are 0 for the rows i >= depth
+// (no predicate).
 template <int N>
 __device__ __forceinline__ uint2 ll_parent_diag(const uint4 p) {
   const uint32_t P[4] = {p.x, p.y, p.z, p.w};
   const uint32_t depth = ll_depth(p.x, p.y, p.z);
+  const uint32_t pl = shl_clamp(1u, depth - 1u), pr = shl_clamp(1u, 32u - depth);  // (both 0 for depth 0)
   uint32_t ld = 0, rd = 0;
 #pragma unroll
-  for (int i = 0; i < N; i++)
-    if (i < depth) {
-      const uint32_t bit = 1u << (P[ll_fw(i)] >> ll_fs(i) & 31u);
-      ld = ((ld | bit) << 1) & ((1u << N) - 1u);
-      rd = (rd | bit) >> 1;
-    }
-  return make_uint2(ld, rd);
+  for (int i = 0; i < N; i++) {
+    const uint32_t x2 = shf_l_wrap(0u, 2u, P[ll_fw(i)] >> ll_fs(i));  // 2 << board[i] (the shift wraps mod 32)
+    ld |= x2 * (pl >> i);         // (1 << board[i]) << (depth - i); 0 for i >= depth
+    rd |= __umulhi(x2, pr << i);  // (2 << board[i]) >> (depth - i); 0 for i >= depth
+  }
+  return make_uint2(ld & ((1u << N) - 1u), rd >> 1);
 }
 
 // child `item` of the slice -> its four data words: board[depth] and board[k] swapped, depth + 1, its masks from the
@@ -505,10 +511,16 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
         }
       }
     }
-    // ---- (5) the diagonals of my parents that have children (the counts are on their way meanwhile)
+    // ---- (5) the diagonals of my parents (the counts are on their way meanwhile).  Computed for all of them, side by
+    // side: only those of parents with children are read, and skipping the others would run a thread's parents one
+    // after the other (so would storing each before loading the next: the compiler cannot tell the arrays apart).
+    {
+      uint4 p[LL_PPT];
 #pragma unroll
-    for (int q = 0; q < LL_PPT; q++)
-      if (cm[q]) sm.diag[LL_PPT * t + q] = ll_parent_diag<N>(sm.parent[LL_PPT * t + q]);
+      for (int q = 0; q < LL_PPT; q++) p[q] = sm.parent[LL_PPT * t + q];
+#pragma unroll
+      for (int q = 0; q < LL_PPT; q++) sm.diag[LL_PPT * t + q] = ll_parent_diag<N>(p[q]);
+    }
     ll_bar(T);  // items and diagonals complete
     TSB_PROF(2)
     // ---- (5b) my children (first window), built and evaluated while the other CTAs' counts are on their way
