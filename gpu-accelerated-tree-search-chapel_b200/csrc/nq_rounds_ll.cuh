@@ -5,7 +5,9 @@
 // generate_children pushing the surviving children back, in order.  Round i+1 pops what round i pushed, so the rounds
 // are a latency chain; at the reference's default --M 50000 two launches and a host poll per round would be the cost.
 // This kernel runs the whole loop in one cooperative launch: every CTA tracks the (tiny) pool state redundantly — a
-// deterministic function of the per-round totals, which every CTA learns anyway — so nothing is broadcast.
+// deterministic function of the per-round totals, which every CTA learns anyway — so nothing is broadcast.  Inside a
+// CTA, eight worker warps move and build the nodes and a ninth, the EXCHANGE warp, owns the count exchange and the
+// pool state (the round is described above nq_rounds_ll_kernel).
 //
 // An earlier version ordered round r+1 after round r with a release fence (MEMBAR.ALL.GPU, thousands of cycles under
 // load) and a "done" flag exchange among all CTAs, on top of the exchange that gathers the child counts: most of its
@@ -45,6 +47,10 @@
 // and the full sweeps start when it has arrived: the extra hop costs more than the poll traffic it saves).  Taking the
 // exchange out of the round altogether, with the next round's counts published next to the children, measured 1.65x
 // slower (DESIGN §5): the in-place stores then need their own "every slice read" wait, and the build is no longer hidden.
+// What did pay: the same 256 worker threads plus one exchange warp per CTA.  Warp 0 used to start the gather only after
+// its share of the build, and all eight warps ran the round's bookkeeping and the next round's set-up after their
+// stores, behind two CTA barriers; the exchange warp gathers while the workers build and does the bookkeeping before
+// the handoff, so the workers go from their stores straight into the next poll (6 % faster, DESIGN §5).
 //
 // The plain 21-byte arena is converted
 // to and from the fat arena by nq_fat_import / nq_fat_export (whole pool, only when the host needs the plain form:
@@ -63,7 +69,7 @@
 
 namespace tsb {
 
-constexpr int LL_T = 256;                    // threads per CTA
+constexpr int LL_T = 256;                    // worker threads per CTA (plus the exchange warp)
 // parents per worker thread (PPT): 2 with one or two pools per launch (7/8 of the SMs / all SMs per pool), 3 with three or four
 // (SMs / 2 CTAs per pool: a round's count exchange among half the CTAs costs about half, tools/flag_exchange.py, and
 // every CTA brings 1.5x the work to hide it behind)
@@ -77,7 +83,7 @@ struct RoundsState {
   unsigned epoch;                 // last epoch used
   int exit_code;
   unsigned long long rounds, parents, children, solutions;  // of this launch
-  long long prof[8];  // (prm.prof) cycles CTA 0 spent per phase (the TSB_PROF indices of nq_rounds_ll_kernel)
+  long long prof[12];  // (prm.prof) cycles CTA 0 spent per phase (the LL_PROF_* indices of nq_rounds_ll_kernel)
 };
 
 __device__ __forceinline__ void st_relaxed_u64(unsigned long long* p, unsigned long long v) {
@@ -148,17 +154,21 @@ struct LlMultiParams {
   LlParams pool[LL_MAX_POOLS];
 };
 
-// ---- CTA barriers on a named barrier (kept from the version that had a side warp outside them)
-__device__ __forceinline__ void ll_bar(int threads) { asm volatile("bar.sync 1, %0;" ::"r"(threads) : "memory"); }
-__device__ __forceinline__ bool ll_bar_or(int threads, bool pred) {
+// ---- named barriers of the persistent kernel: LL_BAR_W among the worker warps only, LL_BAR_SCAN workers -> exchange
+// warp (bar.arrive / bar.sync: the counts are scanned), LL_BAR_HAND exchange warp <-> workers (the handoff)
+constexpr int LL_BAR_W = 1, LL_BAR_SCAN = 2, LL_BAR_HAND = 3;
+__device__ __forceinline__ void ll_bar(int threads) { asm volatile("bar.sync %0, %1;" ::"n"(LL_BAR_W), "r"(threads) : "memory"); }
+__device__ __forceinline__ void ll_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ void ll_wait(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ bool ll_bar_or(int id, int threads, bool pred) {
   uint32_t r;
   asm volatile(
       "{\n\t.reg .pred p, q;\n\t"
       "setp.ne.u32 p, %1, 0;\n\t"
-      "bar.red.or.pred q, 1, %2, p;\n\t"
+      "bar.red.or.pred q, %2, %3, p;\n\t"
       "selp.u32 %0, 1, 0, q;\n\t}"
       : "=r"(r)
-      : "r"(static_cast<uint32_t>(pred)), "r"(threads)
+      : "r"(static_cast<uint32_t>(pred)), "r"(id), "r"(threads)
       : "memory");
   return r != 0;
 }
@@ -225,7 +235,7 @@ __global__ void nq_fat_export_kernel(const FatNode* __restrict__ fat, uint8_t* _
   for (int i = 0; i < NQ_REC - 1; i++) node[1 + i] = static_cast<uint8_t>(d[ll_fw(i)] >> ll_fs(i) & 31u);
 }
 
-// warp 0: until all n slots carry `epoch`; sums of {leaves << 32 | children} over all slots and over the slots
+// the exchange warp: until all n slots carry `epoch`; sums of {leaves << 32 | children} over all slots and over the slots
 // before k0 / before k1 (valid in every lane); false = abort
 __device__ __forceinline__ bool warp_gather_slots2(const unsigned long long* slot, int n, int k0, int k1, unsigned epoch,
                                                    unsigned* abort_flag, unsigned long long& before0,
@@ -272,6 +282,24 @@ __device__ __forceinline__ bool warp_gather_slots2(const unsigned long long* slo
   return true;
 }
 
+// what the exchange warp hands the workers at the end of a round's gather (one record: the workers copy the offsets
+// right after the handoff and the geometry before their next poll; the exchange warp writes the next record only
+// after the next scan, i.e. after both)
+struct LlPlan {
+  long long s0;             // next round: position of the chunk's first parent (= of the round's first child)
+  int a0, len0, a1, len1;   // next round: this CTA's two sub-slices of the chunk (first parent, parents)
+  unsigned epoch;           // next round's epoch
+  int top;                  // next round: top layer of the layer stack
+  int exit;                 // -1: run the next round; else the RND_EXIT_* code all threads leave with
+  int off0, off1;           // this round: first child of each of this CTA's sub-slices among the round's children
+};
+// TSB200_ROUNDS_PROF phases (CTA 0 cycles; workers: thread 0, exchange warp: its lane 0)
+enum {
+  LL_PROF_SETUP = 0, LL_PROF_POLL, LL_PROF_SCAN, LL_PROF_BUILD, LL_PROF_HAND, LL_PROF_STORE,  // workers
+  LL_PROF_X_SCAN, LL_PROF_X_GATHER, LL_PROF_X_BOOK, LL_PROF_X_HAND,                         // exchange warp
+  LL_PROF_N
+};
+static_assert(LL_PROF_N <= 12, "RoundsState::prof");
 template <int T, int PPT>
 struct LlSmem {
   alignas(16) uint4 parent[T * PPT];   // the slice: data32[0..3] of every parent
@@ -279,8 +307,10 @@ struct LlSmem {
   alignas(8) uint2 diag[T * PPT];      // {ld, rd} of every parent (ll_parent_diag; read for those with children)
   alignas(16) uint16_t item[T * PPT * 20];  // (record << 5) | slot, in child order
   unsigned long long warp_tot64[T / 32];
-  unsigned long long red[3];
-  long long prof[8], prof_t;       // (prm.prof, CTA 0) cycles per phase, clock at the end of the last one
+  LlPlan plan;
+  int poll_abort;                  // a worker's poll gave up: the exchange warp leaves after the scan barrier
+  long long prof[LL_PROF_N], prof_t[2];  // (prm.prof, CTA 0) cycles per phase; clock at the end of the last one
+                                         // (workers, exchange warp)
   long long lay_start[LL_LAYERS];  // the pool's layers, bottom to top: first position ...
   unsigned lay_epoch[LL_LAYERS];   // ... and the epoch its nodes were stored with (LL_TRUSTED: before the launch)
 };
@@ -339,271 +369,325 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
   return make_uint4(P[0], P[1], P[2], P[3]);
 }
 
+// One CTA = LL_T worker threads (warps 0-7) + one EXCHANGE warp (warp 8).  A round:
+//   workers:   poll the slice -> child masks, block scan -> (LL_BAR_SCAN arrive) -> items, parent diagonals -> build
+//              the first window -> HANDOFF -> store the windows -> the next round's poll
+//   exchange:  (LL_BAR_SCAN wait) -> publish the CTA's two count slots -> gather all 2G slots -> offsets, layer stack,
+//              pool size, counters, exit tests and the next round's geometry -> HANDOFF
+// so the gather runs while the workers build, and the bookkeeping of a round and the set-up of the next are off the
+// workers' chain: after their stores they go straight into the next poll.  The pool state (size, epoch, layers,
+// counters) is the exchange warp's alone; the workers get what they need through sm.plan.
 template <int N, int T, int MINB, int PPT>
-__global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_constant__ LlMultiParams mprm) {
+__global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid_constant__ LlMultiParams mprm) {
   const LlParams& prm = mprm.pool[blockIdx.y];
   constexpr int LL_PPT = PPT;
+  constexpr int TX = T + 32;  // the whole CTA: workers + exchange warp
   extern __shared__ __align__(128) uint8_t smem_raw[];
   LlSmem<T, PPT>& sm = *reinterpret_cast<LlSmem<T, PPT>*>(smem_raw);
   const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
-  const int k = blockIdx.x, G = gridDim.x;
+  const int k = blockIdx.x, G = gridDim.x, G2 = 2 * G;
   LlSync* const sy = prm.sync;
   FatNode* const fat = prm.fat;
-  // the profile lives in shared memory, touched by CTA 0's thread 0 only: no per-thread state, nothing when it is off
-  const bool prof_on = prm.prof != 0 && k == 0 && t == 0;
-
-  if (t == 0) {
-    sm.lay_start[0] = 0;
-    sm.lay_epoch[0] = LL_TRUSTED;
-    if (prof_on)
-      for (int i = 0; i < 8; i++) sm.prof[i] = 0;
+  // the profile lives in shared memory, touched by CTA 0's thread 0 (workers) and thread T (exchange warp) only: no
+  // per-thread state, nothing when it is off
+  const bool prof_w = prm.prof != 0 && k == 0 && t == 0;
+  const bool prof_x = prm.prof != 0 && k == 0 && t == T;
+#define TSB_PROF(on, who, i)          \
+  if (on) {                           \
+    const long long now = clock64();  \
+    sm.prof[i] += now - sm.prof_t[who]; \
+    sm.prof_t[who] = now;             \
   }
-  __syncthreads();
-  int n_lay = prm.size0 > 0 ? 1 : 0;
 
-  // ------------------------------------------------------------------------------------------ the workers
-  long long size = prm.size0;
+  // ---- the exchange warp's pool state (every lane holds the same values; lane 0 writes shared memory)
+  long long size = prm.size0, chunk_s0 = 0, chunk_n = 0;  // (the chunk of the current round)
   unsigned epoch = prm.epoch0;
+  int n_lay = prm.size0 > 0 ? 1 : 0;
   unsigned long long rounds = 0, tot_parents = 0, tot_children = 0, tot_solutions = 0;
   int exit_code = RND_EXIT_PAUSE;
-#define TSB_PROF(i)                  \
-  if (prof_on) {                     \
-    const long long now = clock64(); \
-    sm.prof[i] += now - sm.prof_t;   \
-    sm.prof_t = now;                 \
+  // (0) the next round's chunk: popBackBulk(m, M) -> sm.plan; -1 or the exit code (uniform decisions: every CTA
+  // holds the same state)
+  const auto plan = [&]() {
+    int ex = -1;
+    if (size < prm.m)
+      ex = RND_EXIT_DONE;
+    else if (static_cast<long long>(rounds) >= prm.max_rounds)
+      ex = RND_EXIT_PAUSE;
+    else {
+      chunk_n = size < prm.M ? size : prm.M;
+      chunk_s0 = size - chunk_n;
+      if (chunk_s0 + chunk_n * N > prm.cap)  // worst case: every slot of every parent survives
+        ex = RND_EXIT_SPACE;
+      else if (n_lay >= LL_LAYERS)  // (no room to record this round's children: start over with one trusted layer)
+        ex = RND_EXIT_RELAUNCH;
+    }
+    if (ex < 0) {
+      ++epoch;
+      // this CTA's share of the chunk: TWO sub-slices of n / 2G parents — number k from the bottom and number k from
+      // the top.  The bottom of a chunk holds the shallow nodes (many children), the top the deep ones (few): a
+      // single slice per CTA left the bottom CTA with 3x the average children, and its build + node stores were the
+      // round's critical path; pairing k with 2G-1-k evens the load without knowing it in advance.
+      // (n <= 768 G and k < G <= 256: the products fit 32 bits — 64-bit divisions are slow emulated sequences)
+      const unsigned n32 = static_cast<unsigned>(chunk_n), uG2 = static_cast<unsigned>(G2), uk = static_cast<unsigned>(k);
+      const int a0 = static_cast<int>(n32 * uk / uG2), a1 = static_cast<int>(n32 * (uG2 - 1u - uk) / uG2);
+      if (lane == 0) {
+        sm.plan.s0 = chunk_s0;
+        sm.plan.a0 = a0;
+        sm.plan.len0 = static_cast<int>(n32 * (uk + 1u) / uG2) - a0;
+        sm.plan.a1 = a1;
+        sm.plan.len1 = static_cast<int>(n32 * (uG2 - uk) / uG2) - a1;
+        sm.plan.epoch = epoch;
+        sm.plan.top = n_lay - 1;
+      }
+    }
+    if (lane == 0) sm.plan.exit = ex;
+    return ex;
+  };
+
+  if (wid == T / 32) {
+    if (lane == 0) {
+      sm.lay_start[0] = 0;
+      sm.lay_epoch[0] = LL_TRUSTED;
+      sm.poll_abort = 0;
+      if (prof_x)
+        for (int i = 0; i < LL_PROF_N; i++) sm.prof[i] = 0;
+    }
+    exit_code = plan();
   }
+  __syncthreads();
+  if (prm.prof != 0 && k == 0 && (t == 0 || t == T)) sm.prof_t[t == T] = clock64();
 
-  for (long long r = 0;; r++) {
-    // ---- (0) the round's chunk: popBackBulk(m, M) (uniform decisions: every CTA holds the same state)
-    if (size < prm.m) {
-      exit_code = RND_EXIT_DONE;
-      break;
-    }
-    if (r >= prm.max_rounds) {
-      exit_code = RND_EXIT_PAUSE;
-      break;
-    }
-    const long long n = size < prm.M ? size : prm.M;
-    const long long s0 = size - n;  // position of the chunk's first parent = of the round's first child
-    if (s0 + n * N > prm.cap) {     // worst case: every slot of every parent survives
-      exit_code = RND_EXIT_SPACE;
-      break;
-    }
-    if (n_lay >= LL_LAYERS) {  // (no room to record this round's children: start over with one trusted layer)
-      exit_code = RND_EXIT_RELAUNCH;
-      break;
-    }
-    ++epoch;
-    if (prof_on) sm.prof_t = clock64();
-    // my share of the chunk: TWO sub-slices of n / 2G parents — number k from the bottom and number k from the top.
-    // The bottom of a chunk holds the shallow nodes (many children), the top the deep ones (few): a single slice per
-    // CTA left the bottom CTA with 3x the average children, and its build + node stores were the round's
-    // critical path; pairing k with 2G-1-k evens the load without knowing it in advance.
-    const int G2 = 2 * G;
-    const unsigned n32 = static_cast<unsigned>(n), uG2 = static_cast<unsigned>(G2), uk = static_cast<unsigned>(k);
-    // (n <= 768 G and k < G <= 256: the products fit 32 bits — 64-bit divisions are slow emulated sequences)
-    const int a0 = static_cast<int>(n32 * uk / uG2), len0 = static_cast<int>(n32 * (uk + 1u) / uG2) - a0;
-    const int a1 = static_cast<int>(n32 * (uG2 - 1u - uk) / uG2), len1 = static_cast<int>(n32 * (uG2 - uk) / uG2) - a1;
-    const int len = len0 + len1;
-
-    bool ok = true;
-    TSB_PROF(0)
-
-    // ---- (2) my slice -> shared memory, 16-byte piece by piece (2 pieces per node, consecutive lanes on consecutive
-    // pieces: every warp load is 512 contiguous bytes); a piece is polled until both of its words carry the epoch of
-    // the layer its node lies in
-    {
-      SpinGuard guard;
-      const unsigned long long* src0 = fat[s0 + a0].w;
-      const unsigned long long* src1 = fat[s0 + a1].w - LL_WORDS * len0;  // (indexed by the concatenated piece number)
-      const int top = n_lay - 1;
-      constexpr int PCS = 2 * LL_PPT;  // pieces per thread
-      unsigned long long w0[PCS], w1[PCS];
-      unsigned pending = 0;
+  if (wid == T / 32) {
+    // ------------------------------------------------------------------------------------------ the exchange warp
+    while (exit_code < 0) {
+      ll_wait(LL_BAR_SCAN, TX);  // the workers' warp totals are in sm.warp_tot64 (they have read their slices)
+      TSB_PROF(prof_x, 1, LL_PROF_X_SCAN)
+      if (sm.poll_abort) {
+        exit_code = RND_EXIT_ABORT;
+        break;
+      }
+      // ---- (4) publish {epoch, leaves, children} of my two sub-slices (slot s = sub-slice s, bottom to top)
+      unsigned long long tot = 0;
 #pragma unroll
-      for (int j = 0; j < PCS; j++)
-        if (t + j * T < 2 * len) pending |= 1u << j;
-      // the epoch node i of my slice was stored with: that of the layer its position lies in (mostly the top one)
-      const auto want_of = [&](int i) {
-        const long long pos = s0 + (i < len0 ? a0 + i : a1 + (i - len0));
-        int L = top;
-        while (L > 0 && sm.lay_start[L] > pos) --L;
-        return sm.lay_epoch[L];
-      };
-      while (pending) {
-        // all loads of a sweep are issued back to back (a dependent re-poll per piece would serialise 8 L2 round trips)
-#pragma unroll
-        for (int j = 0; j < PCS; j++)
-          if (pending & (1u << j)) {
-            const int pc = t + j * T;
-            ld_fat2((pc < 2 * len0 ? src0 : src1) + 2 * pc, w0[j], w1[j]);
+      for (int i = 0; i < T / 32; i++) tot += sm.warp_tot64[i];
+      const unsigned my_children = static_cast<unsigned>(tot & 0xFFFFF), my_leaves = static_cast<unsigned>(tot >> 20) & 0xFFFu;
+      const unsigned cnt0 = static_cast<unsigned>(tot >> 32);
+      unsigned long long* const slots = sy->slot[epoch & 1u];
+      const unsigned long long e = static_cast<unsigned long long>(epoch) << 32;
+      if (lane < 2)
+        st_relaxed_u64(&slots[lane == 0 ? k : G2 - 1 - k],
+                       lane == 0 ? e | static_cast<unsigned long long>(my_leaves) << 20 | cnt0 : e | (my_children - cnt0));
+      // ---- (6) all-to-all: everybody's {leaves, children}; my child offsets and the round's totals (the workers
+      // build their first window meanwhile)
+      unsigned long long before0 = 0, before1 = 0, all = 0;
+      const bool ok = warp_gather_slots2(slots, G2, k, G2 - 1 - k, epoch, &sy->abort, before0, before1, all);
+      TSB_PROF(prof_x, 1, LL_PROF_X_GATHER)
+      if (ok) {
+        if (lane == 0) {
+          sm.plan.off0 = static_cast<int>(before0 & 0xFFFFFFFFull);
+          sm.plan.off1 = static_cast<int>(before1 & 0xFFFFFFFFull);
+        }
+        const long long round_children = static_cast<long long>(all & 0xFFFFFFFFull);
+        // ---- (8) the pool's layers after the round: every layer that starts inside the chunk is consumed, the
+        // round's children form the new top layer (same computation in every CTA).  The workers read the stack only
+        // in their poll, and all of them have finished this round's poll (they arrived at LL_BAR_SCAN) and start
+        // the next one after the handoff: nobody reads an entry while it changes.
+        int nl = n_lay;
+        while (nl > 0 && sm.lay_start[nl - 1] >= chunk_s0) --nl;
+        __syncwarp();  // (every lane has read the entry lane 0 may overwrite)
+        if (round_children > 0) {
+          if (lane == 0) {
+            sm.lay_start[nl] = chunk_s0;
+            sm.lay_epoch[nl] = epoch;
           }
+          ++nl;
+        }
+        n_lay = nl;
+        // ---- (9) the pool after the round, and the next round's chunk
+        size = chunk_s0 + round_children;
+        ++rounds;
+        tot_parents += static_cast<unsigned long long>(chunk_n);
+        tot_children += static_cast<unsigned long long>(round_children);
+        tot_solutions += all >> 32;
+        exit_code = plan();
+      }
+      TSB_PROF(prof_x, 1, LL_PROF_X_BOOK)
+      if (ll_bar_or(LL_BAR_HAND, TX, !ok)) {  // the handoff (an abort reaches the workers here)
+        exit_code = RND_EXIT_ABORT;
+        break;
+      }
+      TSB_PROF(prof_x, 1, LL_PROF_X_HAND)
+    }
+  } else {
+    // ------------------------------------------------------------------------------------------ the workers
+    for (;;) {
+      if (sm.plan.exit >= 0) break;
+      const long long s0 = sm.plan.s0;
+      const int a0 = sm.plan.a0, len0 = sm.plan.len0, a1 = sm.plan.a1, len1 = sm.plan.len1;
+      const unsigned round_epoch = sm.plan.epoch;
+      const int top = sm.plan.top;
+      const int len = len0 + len1;
+      bool ok = true;
+      TSB_PROF(prof_w, 0, LL_PROF_SETUP)
+
+      // ---- (2) my slice -> shared memory, 16-byte piece by piece (2 pieces per node, consecutive lanes on
+      // consecutive pieces: every warp load is 512 contiguous bytes); a piece is polled until both of its words
+      // carry the epoch of the layer its node lies in
+      {
+        SpinGuard guard;
+        const unsigned long long* src0 = fat[s0 + a0].w;
+        const unsigned long long* src1 = fat[s0 + a1].w - LL_WORDS * len0;  // (indexed by the concatenated piece number)
+        constexpr int PCS = 2 * LL_PPT;  // pieces per thread
+        unsigned long long w0[PCS], w1[PCS];
+        unsigned pending = 0;
 #pragma unroll
         for (int j = 0; j < PCS; j++)
-          if (pending & (1u << j)) {
-            const int pc = t + j * T, i = pc >> 1;
-            const unsigned want = want_of(i);
-            if (want == LL_TRUSTED || (static_cast<unsigned>(w0[j] >> 32) == want && static_cast<unsigned>(w1[j] >> 32) == want)) {
-              reinterpret_cast<uint2*>(&sm.parent[i])[pc & 1] =
-                  make_uint2(static_cast<uint32_t>(w0[j]), static_cast<uint32_t>(w1[j]));
-              pending &= ~(1u << j);
+          if (t + j * T < 2 * len) pending |= 1u << j;
+        // the epoch node i of my slice was stored with: that of the layer its position lies in (mostly the top one)
+        const auto want_of = [&](int i) {
+          const long long pos = s0 + (i < len0 ? a0 + i : a1 + (i - len0));
+          int L = top;
+          while (L > 0 && sm.lay_start[L] > pos) --L;
+          return sm.lay_epoch[L];
+        };
+        while (pending) {
+          // all loads of a sweep are issued back to back (a dependent re-poll per piece would serialise 8 L2 round
+          // trips)
+#pragma unroll
+          for (int j = 0; j < PCS; j++)
+            if (pending & (1u << j)) {
+              const int pc = t + j * T;
+              ld_fat2((pc < 2 * len0 ? src0 : src1) + 2 * pc, w0[j], w1[j]);
             }
+#pragma unroll
+          for (int j = 0; j < PCS; j++)
+            if (pending & (1u << j)) {
+              const int pc = t + j * T, i = pc >> 1;
+              const unsigned want = want_of(i);
+              if (want == LL_TRUSTED ||
+                  (static_cast<unsigned>(w0[j] >> 32) == want && static_cast<unsigned>(w1[j] >> 32) == want)) {
+                reinterpret_cast<uint2*>(&sm.parent[i])[pc & 1] =
+                    make_uint2(static_cast<uint32_t>(w0[j]), static_cast<uint32_t>(w1[j]));
+                pending &= ~(1u << j);
+              }
+            }
+          if (pending && guard.expired(&sy->abort)) {
+            ok = false;
+            break;
           }
-        if (pending && guard.expired(&sy->abort)) {
-          ok = false;
-          break;
         }
       }
-    }
-    if (ll_bar_or(T, !ok)) {  // the slice is in shared memory
-      exit_code = RND_EXIT_ABORT;
-      break;
-    }
-    uint32_t cm[LL_PPT];
-    int leaves = 0, mine = 0, mine0 = 0;
-#pragma unroll
-    for (int q = 0; q < LL_PPT; q++) {
-      const int i = LL_PPT * t + q;
-      cm[q] = 0;
-      if (i < len) {
-        const uint32_t w3 = sm.parent[i].w;
-        cm[q] = w3 >> LL_CM_SHIFT & 0xFFFFFu;
-        leaves += (w3 & LL_LEAF) ? 1 : 0;
-        mine += __popc(cm[q]);
-        if (i < len0) mine0 += __popc(cm[q]);
+      if (ll_bar_or(LL_BAR_W, T, !ok)) {  // the slice is in shared memory
+        if (t == 0) sm.poll_abort = 1;
+        ll_arrive(LL_BAR_SCAN, TX);  // (the exchange warp waits there, sees the flag and leaves too)
+        break;
       }
-    }
-    TSB_PROF(1)
-    // ---- (3) block scan: children | leaves << 20 | children of the bottom sub-slice << 32
-    unsigned long long incl = static_cast<unsigned long long>(mine) | static_cast<unsigned long long>(leaves) << 20 |
-                              static_cast<unsigned long long>(mine0) << 32;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-      if (lane >= o) incl += y;
-    }
-    if (lane == 31) sm.warp_tot64[wid] = incl;
-    ll_bar(T);
-    unsigned long long woff = 0, tot = 0;
-#pragma unroll
-    for (int i = 0; i < T / 32; i++) {
-      if (i < wid) woff += sm.warp_tot64[i];
-      tot += sm.warp_tot64[i];
-    }
-    const int my_children = static_cast<int>(tot & 0xFFFFF), my_leaves = static_cast<int>(tot >> 20) & 0xFFF;
-    const int cnt0 = static_cast<int>(tot >> 32), cnt1 = my_children - cnt0;
-    // ---- (4) publish {epoch, leaves, children} of my two sub-slices (slot s = sub-slice s, bottom to top)
-    unsigned long long* const slots = sy->slot[epoch & 1u];
-    if (t == 0) {
-      st_relaxed_u64(&slots[k], static_cast<unsigned long long>(epoch) << 32 | static_cast<unsigned long long>(my_leaves) << 20 |
-                                    static_cast<unsigned long long>(cnt0));
-      st_relaxed_u64(&slots[G2 - 1 - k], static_cast<unsigned long long>(epoch) << 32 | static_cast<unsigned long long>(cnt1));
-    }
-    {
-      uint16_t* it = sm.item + (static_cast<int>((woff + incl) & 0xFFFFF) - mine);
+      uint32_t cm[LL_PPT];
+      int leaves = 0, mine = 0, mine0 = 0;
 #pragma unroll
       for (int q = 0; q < LL_PPT; q++) {
-        uint32_t m = cm[q];
-        while (m) {
-          const int s = __ffs(m) - 1;
-          m &= m - 1;
-          *it++ = static_cast<uint16_t>(((LL_PPT * t + q) << 5) | s);
+        const int i = LL_PPT * t + q;
+        cm[q] = 0;
+        if (i < len) {
+          const uint32_t w3 = sm.parent[i].w;
+          cm[q] = w3 >> LL_CM_SHIFT & 0xFFFFFu;
+          leaves += (w3 & LL_LEAF) ? 1 : 0;
+          mine += __popc(cm[q]);
+          if (i < len0) mine0 += __popc(cm[q]);
         }
       }
-    }
-    // ---- (5) the diagonals of my parents (the counts are on their way meanwhile).  Computed for all of them, side by
-    // side: only those of parents with children are read, and skipping the others would run a thread's parents one
-    // after the other (so would storing each before loading the next: the compiler cannot tell the arrays apart).
-    {
-      uint4 p[LL_PPT];
+      TSB_PROF(prof_w, 0, LL_PROF_POLL)
+      // ---- (3) block scan: children | leaves << 20 | children of the bottom sub-slice << 32
+      unsigned long long incl = static_cast<unsigned long long>(mine) | static_cast<unsigned long long>(leaves) << 20 |
+                                static_cast<unsigned long long>(mine0) << 32;
 #pragma unroll
-      for (int q = 0; q < LL_PPT; q++) p[q] = sm.parent[LL_PPT * t + q];
-#pragma unroll
-      for (int q = 0; q < LL_PPT; q++) sm.diag[LL_PPT * t + q] = ll_parent_diag<N>(p[q]);
-    }
-    ll_bar(T);  // items and diagonals complete
-    TSB_PROF(2)
-    // ---- (5b) my children (first window), built and evaluated while the other CTAs' counts are on their way
-    auto build_window = [&](int c0, int cnt) {
-      for (int c = t; c < cnt; c += T) sm.stage[c] = ll_build_child<N>(sm.parent, sm.diag, sm.item[c0 + c]);
-    };
-    build_window(0, min(LL_CAP, my_children));
-    TSB_PROF(6)
-    // ---- (6) all-to-all: everybody's {leaves, children}; my child offset and the round's totals
-    unsigned long long before0 = 0, before1 = 0, all = 0;
-    if (wid == 0) {
-      ok = warp_gather_slots2(slots, G2, k, G2 - 1 - k, epoch, &sy->abort, before0, before1, all);
-      if (lane == 0) {
-        sm.red[0] = before0;
-        sm.red[1] = before1;
-        sm.red[2] = all;
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+        if (lane >= o) incl += y;
       }
-    }
-    if (ll_bar_or(T, !ok)) {  // (also: the window is complete, red[] visible)
-      exit_code = RND_EXIT_ABORT;
-      break;
-    }
-    TSB_PROF(3)
-    const long long off0 = static_cast<long long>(sm.red[0] & 0xFFFFFFFFull);
-    const long long off1 = static_cast<long long>(sm.red[1] & 0xFFFFFFFFull);
-    all = sm.red[2];
-    const long long round_children = static_cast<long long>(all & 0xFFFFFFFFull);
-    const long long round_leaves = static_cast<long long>(all >> 32);
-
-    // ---- (7) my children, in place, tagged with this round's epoch (every slice of the chunk has been read: all
-    // G slots carried this epoch)
-    const unsigned long long tag = static_cast<unsigned long long>(epoch) << 32;
-    for (int c0 = 0; c0 < my_children; c0 += LL_CAP) {
-      const int cnt = min(LL_CAP, my_children - c0);
-      if (c0 > 0) {
-        ll_bar(T);  // the previous window has been copied out
-        build_window(c0, cnt);
-        ll_bar(T);
-      }
-      // child c of my share goes to position s0 + off0 + c (bottom sub-slice) or s0 + off1 + (c - cnt0) (top one)
-      unsigned long long* const dst0 = fat[s0 + off0 + c0].w;
-      unsigned long long* const dst1 = fat[s0 + off1 + c0 - cnt0].w;
-      const int npc = 2 * cnt;  // 16-byte pieces, consecutive lanes on consecutive pieces, four in flight per thread
-      for (int pc = t; pc < npc; pc += 4 * T) {
-        uint2 d[4];
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-          const int x = min(pc + u * T, npc - 1);
-          d[u] = reinterpret_cast<const uint2*>(&sm.stage[x >> 1])[x & 1];
-        }
-#pragma unroll
-        for (int u = 0; u < 4; u++) {
-          const int x = pc + u * T;
-          if (x < npc) st_fat2((c0 + (x >> 1) < cnt0 ? dst0 : dst1) + 2 * x, d[u].x | tag, d[u].y | tag);
-        }
-      }
-    }
-    TSB_PROF(4)
-    // ---- (8) the pool's layers after the round: every layer that starts inside the chunk is consumed, the round's
-    // children form the new top layer (same computation in every CTA)
-    {
-      int nl = n_lay;
-      while (nl > 0 && sm.lay_start[nl - 1] >= s0) --nl;
-      ll_bar(T);  // (everybody has read the old entries, the window buffers and sm.red)
-      if (round_children > 0) {
-        if (t == 0) {
-          sm.lay_start[nl] = s0;
-          sm.lay_epoch[nl] = epoch;
-        }
-        ++nl;
-      }
-      n_lay = nl;
+      if (lane == 31) sm.warp_tot64[wid] = incl;
+      ll_arrive(LL_BAR_SCAN, TX);  // the exchange warp publishes the totals and gathers everybody's
       ll_bar(T);
+      unsigned long long woff = 0, tot = 0;
+#pragma unroll
+      for (int i = 0; i < T / 32; i++) {
+        if (i < wid) woff += sm.warp_tot64[i];
+        tot += sm.warp_tot64[i];
+      }
+      const int my_children = static_cast<int>(tot & 0xFFFFF);
+      const int cnt0 = static_cast<int>(tot >> 32);
+      {
+        uint16_t* it = sm.item + (static_cast<int>((woff + incl) & 0xFFFFF) - mine);
+#pragma unroll
+        for (int q = 0; q < LL_PPT; q++) {
+          uint32_t m = cm[q];
+          while (m) {
+            const int s = __ffs(m) - 1;
+            m &= m - 1;
+            *it++ = static_cast<uint16_t>(((LL_PPT * t + q) << 5) | s);
+          }
+        }
+      }
+      // ---- (5) the diagonals of my parents (the counts are on their way meanwhile).  Computed for all of them,
+      // side by side: only those of parents with children are read, and skipping the others would run a thread's
+      // parents one after the other (so would storing each before loading the next: the compiler cannot tell the
+      // arrays apart).
+      {
+        uint4 p[LL_PPT];
+#pragma unroll
+        for (int q = 0; q < LL_PPT; q++) p[q] = sm.parent[LL_PPT * t + q];
+#pragma unroll
+        for (int q = 0; q < LL_PPT; q++) sm.diag[LL_PPT * t + q] = ll_parent_diag<N>(p[q]);
+      }
+      ll_bar(T);  // items and diagonals complete
+      TSB_PROF(prof_w, 0, LL_PROF_SCAN)
+      // ---- (5b) my children (first window), built and evaluated while the other CTAs' counts are on their way
+      auto build_window = [&](int c0, int cnt) {
+        for (int c = t; c < cnt; c += T) sm.stage[c] = ll_build_child<N>(sm.parent, sm.diag, sm.item[c0 + c]);
+      };
+      build_window(0, min(LL_CAP, my_children));
+      TSB_PROF(prof_w, 0, LL_PROF_BUILD)
+      // ---- the handoff: my offsets from the exchange warp (also: the first window is complete)
+      if (ll_bar_or(LL_BAR_HAND, TX, false)) break;  // (an abort of the gather)
+      TSB_PROF(prof_w, 0, LL_PROF_HAND)
+      const int off0 = sm.plan.off0, off1 = sm.plan.off1;
+
+      // ---- (7) my children, in place, tagged with this round's epoch (every slice of the chunk has been read: all
+      // 2G slots carried this epoch)
+      const unsigned long long tag = static_cast<unsigned long long>(round_epoch) << 32;
+      for (int c0 = 0; c0 < my_children; c0 += LL_CAP) {
+        const int cnt = min(LL_CAP, my_children - c0);
+        if (c0 > 0) {
+          ll_bar(T);  // the previous window has been copied out
+          build_window(c0, cnt);
+          ll_bar(T);
+        }
+        // child c of my share goes to position s0 + off0 + c (bottom sub-slice) or s0 + off1 + (c - cnt0) (top one)
+        unsigned long long* const dst0 = fat[s0 + off0 + c0].w;
+        unsigned long long* const dst1 = fat[s0 + off1 + c0 - cnt0].w;
+        const int npc = 2 * cnt;  // 16-byte pieces, consecutive lanes on consecutive pieces, four in flight per thread
+        for (int pc = t; pc < npc; pc += 4 * T) {
+          uint2 d[4];
+#pragma unroll
+          for (int u = 0; u < 4; u++) {
+            const int x = min(pc + u * T, npc - 1);
+            d[u] = reinterpret_cast<const uint2*>(&sm.stage[x >> 1])[x & 1];
+          }
+#pragma unroll
+          for (int u = 0; u < 4; u++) {
+            const int x = pc + u * T;
+            if (x < npc) st_fat2((c0 + (x >> 1) < cnt0 ? dst0 : dst1) + 2 * x, d[u].x | tag, d[u].y | tag);
+          }
+        }
+      }
+      TSB_PROF(prof_w, 0, LL_PROF_STORE)
+      // (straight into the next round: sm.plan holds its geometry since the handoff.  No worker barrier is needed
+      // before the next poll overwrites sm.parent: every build of this round ended before a barrier all workers
+      // passed, and sm.stage is next written after the next poll's barrier, when every store has read it.)
     }
-    TSB_PROF(5)
-    // ---- (9) the pool after the round
-    size = s0 + round_children;
-    ++rounds;
-    tot_parents += static_cast<unsigned long long>(n);
-    tot_children += static_cast<unsigned long long>(round_children);
-    tot_solutions += static_cast<unsigned long long>(round_leaves);
   }
-  if (k == 0 && t == 0) {
+  __syncthreads();  // (all CTA threads leave the loop at the same round; the profile is complete)
+  if (k == 0 && t == T) {
     RoundsState* st = prm.state;
     st->size = size;
     st->epoch = epoch;
@@ -612,8 +696,8 @@ __global__ void __launch_bounds__(T, MINB) nq_rounds_ll_kernel(const __grid_cons
     st->children = tot_children;
     st->solutions = tot_solutions;
     st->exit_code = exit_code;
-    if (prof_on)
-      for (int i = 0; i < 8; i++) st->prof[i] = sm.prof[i];
+    if (prof_x)
+      for (int i = 0; i < LL_PROF_N; i++) st->prof[i] = sm.prof[i];
   }
 #undef TSB_PROF
 }

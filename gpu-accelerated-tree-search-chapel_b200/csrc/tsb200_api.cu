@@ -1304,8 +1304,8 @@ int tsb_nq_pool_step(tsb_nq* h, int m, int M, int64_t* n_parents, uint64_t* n_ch
 namespace {
 template <int N>
 int nq_ll_launch_n(tsb_nq* h, const tsb::LlMultiParams& prm, int grid, int pools, int ppt, cudaStream_t s) {
-  // (one pool: the 160-register build, one CTA per SM; several: capped at 128 registers for two CTAs per SM; three
-  // or four pools: 66 CTAs per pool with 768 parents each on 132 SMs, see ll_slice)
+  // (one pool: one CTA per SM; several: two CTAs of LL_T workers + the exchange warp per SM, capped at 112
+  // registers; three or four pools: 66 CTAs per pool with 768 parents each on 132 SMs, see ll_slice)
   const int var = pools == 1 ? 0 : ppt == 2 ? 1 : 2;
   auto kernel = var == 0   ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 2>
                 : var == 1 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 2>
@@ -1318,7 +1318,7 @@ int nq_ll_launch_n(tsb_nq* h, const tsb::LlMultiParams& prm, int grid, int pools
   }
   void* args[] = {const_cast<tsb::LlMultiParams*>(&prm)};
   // cooperative: all CTAs of all pools co-resident (two per SM when there are two pools), or the launch fails
-  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid, pools), dim3(tsb::LL_T), args, smem, s));
+  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid, pools), dim3(tsb::LL_T + 32), args, smem, s));
   h->launches++;
   return TSB_OK;
 }
@@ -1471,13 +1471,16 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
         g_last_cuda_error = "nq_rounds_ll_kernel: watchdog abort (a flag exchange or a node poll did not complete)";
         return TSB_ECUDA;
       }
-      if (prof)
-        std::fprintf(stderr, "[tsb200] LL rounds kernel (pool %d of %d): %llu rounds; CTA 0 cycles per round: build %.0f | fence-check %.0f "
-                     "poll-nodes %.0f scan+items+diag %.0f gather-wait %.0f store %.0f signal %.0f\n", a, n_act,
-                     static_cast<unsigned long long>(st.rounds), 1.0 * st.prof[6] / std::max<unsigned long long>(1, st.rounds),
-                     1.0 * st.prof[0] / std::max<unsigned long long>(1, st.rounds), 1.0 * st.prof[1] / std::max<unsigned long long>(1, st.rounds),
-                     1.0 * st.prof[2] / std::max<unsigned long long>(1, st.rounds), 1.0 * st.prof[3] / std::max<unsigned long long>(1, st.rounds),
-                     1.0 * st.prof[4] / std::max<unsigned long long>(1, st.rounds), 1.0 * st.prof[5] / std::max<unsigned long long>(1, st.rounds));
+      if (prof) {
+        const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
+        std::fprintf(stderr, "[tsb200] LL rounds kernel (pool %d of %d): %llu rounds; CTA 0 cycles per round: workers: set-up %.0f "
+                     "poll-nodes %.0f scan+items+diag %.0f build %.0f handoff-wait %.0f store %.0f | exchange warp: "
+                     "scan-wait %.0f publish+gather %.0f bookkeeping %.0f handoff-wait %.0f\n", a, n_act,
+                     static_cast<unsigned long long>(st.rounds), st.prof[tsb::LL_PROF_SETUP] / r, st.prof[tsb::LL_PROF_POLL] / r,
+                     st.prof[tsb::LL_PROF_SCAN] / r, st.prof[tsb::LL_PROF_BUILD] / r, st.prof[tsb::LL_PROF_HAND] / r,
+                     st.prof[tsb::LL_PROF_STORE] / r, st.prof[tsb::LL_PROF_X_SCAN] / r, st.prof[tsb::LL_PROF_X_GATHER] / r,
+                     st.prof[tsb::LL_PROF_X_BOOK] / r, st.prof[tsb::LL_PROF_X_HAND] / r);
+      }
       h->rounds.epoch = st.epoch;
       p.size = st.size;
       p.ext.clear();
