@@ -19,6 +19,7 @@
 #include "nq_expand.cuh"
 #include "nq_rounds_ll.cuh"
 #include "pfsp_expand.cuh"
+#include "pfsp_rounds.cuh"
 #include "nq_kernel.cuh"
 #include "pfsp_kernels.cuh"
 #include "pfsp_wide.cuh"
@@ -767,6 +768,12 @@ struct tsb_pfsp : Base {
   uint64_t slow_rounds = 0;
   std::vector<tsb_pfsp_node> h_chunk, h_kids;  // slow path scratch
   std::vector<int32_t> h_bounds;
+  // the persistent multi-round kernel (pfsp_rounds.cuh)
+  tsb::RoundsState* rnd_h = nullptr;  // pinned + mapped: written by the kernel when it leaves
+  tsb::RoundsState* rnd_d = nullptr;  // device alias of rnd_h
+  tsb::PfRoundsSync* rnd_sync = nullptr;
+  unsigned rnd_epoch = 0;
+  bool rnd_attr[2] = {false, false};  // lb1_d, lb1
 };
 
 namespace {
@@ -1908,6 +1915,8 @@ void tsb_pfsp_destroy(tsb_pfsp* h) {
   if (h->d_tabu) cudaFree(h->d_tabu);
   h->ex.release();
   if (h->d_children) cudaFree(h->d_children);
+  if (h->rnd_h) cudaFreeHost(h->rnd_h);
+  if (h->rnd_sync) cudaFree(h->rnd_sync);
   h->pool.release();
   h->fini();
   delete h;
@@ -2100,6 +2109,162 @@ int tsb_pfsp_pool_drain(tsb_pfsp* h, void* nodes, int64_t capacity, int64_t* n) 
   }
   p.ext.clear();
   p.size = 0;
+  return TSB_OK;
+}
+
+}  // extern "C"
+
+// ---- PFSP: the whole offload loop in launches of the persistent kernel (pfsp_rounds.cuh)
+namespace {
+// CTAs of the persistent PFSP kernel for chunks of up to M parents (one per SM at most, each with up to PFR_SLICE
+// parents; fewer CTAs for smaller M, so that the two exchanges of a round involve only the CTAs that have parents to
+// evaluate); 0: the loop of tsb_pfsp_pool_step runs instead (lb2, M above PFR_MAX_M where the step loop is faster, M
+// beyond pf_rounds_capacity, no cooperative launch, env TSB200_NO_ROUNDS=1)
+int pfsp_rounds_grid(const tsb_pfsp* h, int lb_kind, int M) {
+  if (lb_kind == TSB_LB2 || !h->di.coop || env_no_rounds()) return 0;
+  if (M > tsb::PFR_MAX_M || M > tsb::pf_rounds_capacity(h->di.sms)) return 0;
+  const int sms = std::min(h->di.sms, tsb::PFR_MAX_CTAS);
+  return static_cast<int>(std::min<long long>(sms, (static_cast<long long>(M) + tsb::PF_TILE - 1) / tsb::PF_TILE));
+}
+template <int KIND, int M>
+int pfsp_rounds_launch_km(tsb_pfsp* h, const tsb::PfRoundsParams& prm, int grid, cudaStream_t s) {
+  auto kernel = h->simd16 ? tsb::pfsp_rounds_kernel<KIND, M, true> : tsb::pfsp_rounds_kernel<KIND, M, false>;
+  const size_t smem = sizeof(tsb::PfRoundsSmem) + 128;
+  if (!h->rnd_attr[KIND]) {
+    TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    h->rnd_attr[KIND] = true;
+  }
+  void* args[] = {const_cast<tsb::PfRoundsParams*>(&prm)};
+  // cooperative: every CTA co-resident (the exchanges wait for all of them), or the launch fails
+  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid), dim3(tsb::PF_THREADS), args, smem, s));
+  h->launches++;
+  return TSB_OK;
+}
+template <int KIND>
+int pfsp_rounds_launch_k(tsb_pfsp* h, const tsb::PfRoundsParams& prm, int grid, cudaStream_t s) {
+  if (h->mt == 5) return pfsp_rounds_launch_km<KIND, 5>(h, prm, grid, s);
+  if (h->mt == 10) return pfsp_rounds_launch_km<KIND, 10>(h, prm, grid, s);
+  return pfsp_rounds_launch_km<KIND, 20>(h, prm, grid, s);
+}
+// Up to max_rounds rounds in launches of the persistent kernel; out[] += {rounds, parents, children, solutions}.  A
+// launch leaves when the pool holds fewer than m nodes, after its round budget, when the next round's worst case
+// does not fit the arena (it grows and the loop relaunches) or when a leaf of the chunk improves *best (that round
+// goes through tsb_pfsp_pool_step and its sequential rule, then the loop relaunches with the new incumbent).
+int pfsp_rounds_run(tsb_pfsp* h, int lb_kind, int m, int M, int grid, int64_t max_rounds, int64_t* best, uint64_t* out) {
+  DevicePool& p = h->pool;
+  pfsp_pool_setup(h);
+  if (!h->rnd_h) {
+    TSB_CUDA(cudaHostAlloc(&h->rnd_h, sizeof(tsb::RoundsState), cudaHostAllocPortable | cudaHostAllocMapped));
+    std::memset(h->rnd_h, 0, sizeof(tsb::RoundsState));
+    TSB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&h->rnd_d), h->rnd_h, 0));
+  }
+  if (!h->rnd_sync) {
+    TSB_CUDA(cudaMalloc(&h->rnd_sync, sizeof(tsb::PfRoundsSync)));
+    TSB_CUDA(cudaMemsetAsync(h->rnd_sync, 0, sizeof(tsb::PfRoundsSync), h->stream));
+  }
+  const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
+  int64_t left = max_rounds;
+  while (left > 0 && p.size >= m) {
+    // the pool as ONE contiguous stack [0, size) with room for the worst case of the next round
+    const long long n = std::min<long long>(p.size, M);
+    const long long need = p.size - n + n * h->jobs;
+    int rc = TSB_OK;
+    if (need > p.cap)
+      rc = p.compact(h->stream, std::max<long long>(2 * p.cap, need + need / 2));
+    else if (p.ext.size() != 1 || p.ext[0].b != 0)
+      rc = p.compact(h->stream, p.cap);
+    if (rc != TSB_OK) return rc;
+    tsb::PfRoundsParams prm;
+    std::memset(&prm, 0, sizeof(prm));
+    prm.arena = p.arena[p.cur];
+    prm.tables = h->d_tab1;
+    prm.cap = p.cap;
+    prm.size0 = p.size;
+    prm.max_rounds = left;
+    prm.epoch0 = h->rnd_epoch;
+    prm.m = m;
+    prm.M = M;
+    prm.best = clamp_best(*best);
+    prm.prof = prof;
+    prm.sync = h->rnd_sync;
+    prm.state = h->rnd_d;
+    h->rnd_h->exit_code = -1;
+    rc = lb_kind == TSB_LB1 ? pfsp_rounds_launch_k<1>(h, prm, grid, h->stream) : pfsp_rounds_launch_k<0>(h, prm, grid, h->stream);
+    if (rc != TSB_OK) return rc;
+    TSB_CUDA(cudaStreamSynchronize(h->stream));
+    const tsb::RoundsState st = *h->rnd_h;
+    if (st.exit_code < 0 || st.exit_code == tsb::RND_EXIT_ABORT) {
+      g_last_cuda_error = "pfsp_rounds_kernel: watchdog abort (a count or store exchange did not complete)";
+      return TSB_ECUDA;
+    }
+    if (prof) {
+      const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
+      std::fprintf(stderr, "[tsb200] PFSP rounds kernel: %llu rounds (exit %d); CTA 0 cycles per round: load %.0f bounds %.0f "
+                   "publish+items %.0f gather %.0f store %.0f store-exchange %.0f\n",
+                   static_cast<unsigned long long>(st.rounds), st.exit_code, st.prof[tsb::PFR_PROF_LOAD] / r,
+                   st.prof[tsb::PFR_PROF_BOUND] / r, st.prof[tsb::PFR_PROF_PUBLISH] / r, st.prof[tsb::PFR_PROF_GATHER] / r,
+                   st.prof[tsb::PFR_PROF_STORE] / r, st.prof[tsb::PFR_PROF_BARRIER] / r);
+    }
+    h->rnd_epoch = st.epoch;
+    p.size = st.size;
+    p.ext.clear();
+    if (p.size) p.ext.push_back({0, p.size});
+    out[0] += st.rounds;
+    out[1] += st.parents;
+    out[2] += st.children;
+    out[3] += st.solutions;
+    left -= static_cast<int64_t>(st.rounds);
+    if (st.exit_code == tsb::RND_EXIT_SPACE) {
+      if (st.rounds == 0 && need <= p.cap) return TSB_ENOMEM;  // (cannot happen: the arena was grown for `need`)
+    } else if (st.exit_code == tsb::PFR_EXIT_IMPROVED) {
+      int64_t np = 0;
+      uint64_t nc = 0, ns = 0;
+      rc = tsb_pfsp_pool_step(h, lb_kind, m, M, best, &np, &nc, &ns);
+      if (rc != TSB_OK) return rc;
+      out[0] += 1;
+      out[1] += static_cast<uint64_t>(np);
+      out[2] += nc;
+      out[3] += ns;
+      --left;
+    } else {
+      break;  // DONE or PAUSE
+    }
+  }
+  return TSB_OK;
+}
+}  // namespace
+extern "C" {
+
+int tsb_pfsp_pool_run(tsb_pfsp* h, int lb_kind, int m, int M, int64_t max_rounds, int64_t* best, uint64_t* n_rounds,
+                      uint64_t* n_parents, uint64_t* n_children, uint64_t* n_solutions) {
+  if (h && h->wide) return TSB_EUNSUPPORTED;  // (the fused expand / device pool exist for MAX_JOBS = 20 only)
+  if (!h || lb_kind < 0 || lb_kind > 2 || m < 1 || M < 1 || M > h->M_max || max_rounds < 0 || !best || !n_rounds ||
+      !n_parents || !n_children || !n_solutions)
+    return TSB_EINVAL;
+  if (lb_kind == TSB_LB2 && h->pairs == 0) return TSB_EINVAL;
+  *n_rounds = *n_parents = *n_children = *n_solutions = 0;
+  TSB_CUDA(cudaSetDevice(h->device));
+  if (const int grid = pfsp_rounds_grid(h, lb_kind, M); grid > 0) {
+    uint64_t out[4] = {0, 0, 0, 0};
+    const int rc = pfsp_rounds_run(h, lb_kind, m, M, grid, max_rounds, best, out);
+    *n_rounds = out[0];
+    *n_parents = out[1];
+    *n_children = out[2];
+    *n_solutions = out[3];
+    return rc;
+  }
+  // lb2, large chunks: one round = two kernels (tsb_pfsp_pool_step)
+  while (static_cast<int64_t>(*n_rounds) < max_rounds) {
+    int64_t np = 0;
+    uint64_t nc = 0, ns = 0;
+    const int rc = tsb_pfsp_pool_step(h, lb_kind, m, M, best, &np, &nc, &ns);
+    if (rc != TSB_OK) return rc;
+    if (np == 0) break;
+    ++*n_rounds;
+    *n_parents += static_cast<uint64_t>(np);
+    *n_children += nc;
+    *n_solutions += ns;
+  }
   return TSB_OK;
 }
 

@@ -691,24 +691,22 @@ void pfsp_devpool_on(tsb_pfsp* h, int lb_kind, int m, int M, Pool<tsb_pfsp_node>
   const auto steal = [m](void* v, void* t, int64_t* got) {
     return tsb_pfsp_pool_steal(static_cast<tsb_pfsp*>(v), static_cast<tsb_pfsp*>(t), m, got);
   };
-  int since_service = 0;
+  // all rounds of step 2 inside the library (one persistent kernel for lb1 / lb1_d and small M, two kernels per
+  // round otherwise); thieves are served between calls
   while (r.rc == TSB_OK) {
-    int64_t np = 0;
-    uint64_t nc = 0, ns = 0;
-    r.rc = tsb_pfsp_pool_step(h, lb_kind, m, M, &r.best, &np, &nc, &ns);
+    uint64_t nr = 0, np = 0, nc = 0, ns = 0;
+    r.rc = tsb_pfsp_pool_run(h, lb_kind, m, M, rounds_per_call(sb, M), &r.best, &nr, &np, &nc, &ns);
     if (r.rc != TSB_OK) break;
-    if (np == 0) {
-      if (!board_acquire(sb, me, tsb_pfsp_pool_size(h), steal_floor(m, M))) break;
-      continue;
-    }
     r.tree += nc;
     r.sol += ns;
-    ++r.offloads;
-    r.parents += static_cast<uint64_t>(np);
-    if (sb && ++since_service >= 2) {  // publish the pool size / serve thieves every other round
-      since_service = 0;
-      r.rc = board_service(sb, me, tsb_pfsp_pool_size(h), steal_floor(m, M), steal);
+    r.offloads += nr;
+    r.parents += np;
+    const long long size = tsb_pfsp_pool_size(h);
+    if (size >= m) {
+      r.rc = board_service(sb, me, size, steal_floor(m, M), steal);
+      continue;
     }
+    if (!board_acquire(sb, me, size, steal_floor(m, M))) break;
   }
   if (r.rc != TSB_OK) board_abort(sb, me);
   if (r.rc == TSB_OK) {

@@ -144,6 +144,16 @@ class PfspEvaluator:
               "tsb_pfsp_pool_step")
         return int(np_.value), int(nc.value), int(ns.value), int(b.value)
 
+    def pool_run(self, lb, m: int, M: int, best: int, max_rounds: int = 2**62):
+        """(rounds, parents, children, solutions, best_after): pool_step rounds until the pool holds fewer than m
+        nodes or max_rounds are done, for lb1 / lb1_d and M up to 20 000 in one persistent kernel"""
+        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        b = C.c_int64(int(best))
+        nr, np_, nc, ns = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        check(lib().tsb_pfsp_pool_run(self._h, kind, m, M, max_rounds, C.byref(b), C.byref(nr), C.byref(np_),
+                                      C.byref(nc), C.byref(ns)), "tsb_pfsp_pool_run")
+        return int(nr.value), int(np_.value), int(nc.value), int(ns.value), int(b.value)
+
     def search(self, inst: int, lb, ub: int = 1, m: int = 25, M: int | None = None) -> SearchStats:
         """the whole 3-step search (pfsp_gpu_chpl.chpl:306-431) with the pool of step 2 on this handle's device"""
         kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)

@@ -247,6 +247,14 @@ int tsb_pfsp_pool_step(tsb_pfsp* h, int lb_kind, int m, int M, int64_t* best, in
                        uint64_t* n_children, uint64_t* n_solutions);
 int tsb_pfsp_pool_drain(tsb_pfsp* h, void* nodes, int64_t capacity_nodes, int64_t* n);
 int tsb_pfsp_pool_steal(tsb_pfsp* victim, tsb_pfsp* thief, int m, int64_t* n_stolen);
+/* rounds until the pool holds fewer than m nodes or max_rounds are done: exactly the sequence of
+ * tsb_pfsp_pool_step rounds (same chunks, same pool after every round, same *best after every round).  For lb1 and
+ * lb1_d with chunks of up to 20 000 parents (and at most 384 x #SMs) the loop runs inside one persistent cooperative
+ * kernel (csrc/pfsp_rounds.cuh), up to 1.8x faster per round on an H100; a round in which a leaf improves *best
+ * leaves it and is run through tsb_pfsp_pool_step.  lb2, larger M (including the reference's default --M 50000,
+ * where the two-kernel rounds measured faster) or env TSB200_NO_ROUNDS=1: one tsb_pfsp_pool_step per round.  Totals over the rounds come back; argument checks as tsb_pfsp_pool_step, plus max_rounds >= 0. */
+int tsb_pfsp_pool_run(tsb_pfsp* h, int lb_kind, int m, int M, int64_t max_rounds, int64_t* best,
+                      uint64_t* n_rounds, uint64_t* n_parents, uint64_t* n_children, uint64_t* n_solutions);
 int tsb_pfsp_register_host(tsb_pfsp* h, void* ptr, size_t bytes);
 int tsb_pfsp_unregister_host(tsb_pfsp* h, void* ptr);
 int tsb_pfsp_set_xfer(tsb_pfsp* h, int mode);
