@@ -304,8 +304,9 @@ template <int T, int PPT>
 struct LlSmem {
   alignas(16) uint4 parent[T * PPT];   // the slice: data32[0..3] of every parent
   alignas(16) uint4 stage[LL_CAP];     // the window's children: data32[0..3]
-  alignas(8) uint2 diag[T * PPT];      // {ld, rd} of every parent (ll_parent_diag; read for those with children)
+  alignas(8) uint2 diag[T * PPT];      // {ld, rd} of the parents with children (ll_parent_diag), at their own index
   alignas(16) uint16_t item[T * PPT * 20];  // (record << 5) | slot, in child order
+  uint16_t fertile[T * PPT];           // per warp (32 PPT entries each): the records of its parents with children
   unsigned long long warp_tot64[T / 32];
   LlPlan plan;
   int poll_abort;                  // a worker's poll gave up: the exchange warp leaves after the scan barrier
@@ -348,11 +349,15 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
   uint32_t P[4] = {p.x, p.y, p.z, p.w};
   const uint32_t depth = ll_depth(p.x, p.y, p.z);
   const auto word = [&](uint32_t w) { return w == 0 ? P[0] : w == 1 ? P[1] : w == 2 ? P[2] : P[3]; };
-  const uint32_t wd = depth / 6u, sd = 5u * (depth - 6u * wd), wk = k / 6u, sk = 5u * (k - 6u * wk);
+  // first bit of board[i] in the four data words read as one 128-bit value: 32 (i / 6) + 5 (i % 6) = 5 i + 2 (i / 6),
+  // with i / 6 = (43 i) >> 8 for every i < 20 (no division)
+  const uint32_t bd = 5u * depth + 2u * (depth * 43u >> 8), bk = 5u * k + 2u * (k * 43u >> 8);
+  const uint32_t wd = bd >> 5, sd = bd & 31u, wk = bk >> 5, sk = bk & 31u;
   const uint32_t v = word(wk) >> sk & 31u;  // the queen placed on row `depth`
   const uint32_t D = (word(wd) >> sd & 31u) ^ v;
+  // (a clamped shift by bd - 32 j is D << sd in word wd and 0 in every other word: no field straddles two words)
 #pragma unroll
-  for (uint32_t j = 0; j < 4; j++) P[j] ^= (j == wd ? D << sd : 0u) ^ (j == wk ? D << sk : 0u);
+  for (uint32_t j = 0; j < 4; j++) P[j] ^= shl_clamp(D, bd - 32u * j) ^ shl_clamp(D, bk - 32u * j);
   const uint32_t cd = depth + 1u;
   ll_set_depth(P, cd);
   const uint2 pd = diag[r];
@@ -370,8 +375,9 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
 }
 
 // One CTA = LL_T worker threads (warps 0-7) + one EXCHANGE warp (warp 8).  A round:
-//   workers:   poll the slice -> child masks, block scan -> (LL_BAR_SCAN arrive) -> items, parent diagonals -> build
-//              the first window -> HANDOFF -> store the windows -> the next round's poll
+//   workers:   poll the slice -> child masks, block scan -> (LL_BAR_SCAN arrive) -> items, each warp's list of parents
+//              with children and their diagonals -> build the first window -> HANDOFF -> store the windows -> the
+//              next round's poll
 //   exchange:  (LL_BAR_SCAN wait) -> publish the CTA's two count slots -> gather all 2G slots -> offsets, layer stack,
 //              pool size, counters, exit tests and the next round's geometry -> HANDOFF
 // so the gather runs while the workers build, and the bookkeeping of a round and the set-up of the next are off the
@@ -403,8 +409,13 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
   long long size = prm.size0, chunk_s0 = 0, chunk_n = 0;  // (the chunk of the current round)
   unsigned epoch = prm.epoch0;
   int n_lay = prm.size0 > 0 ? 1 : 0;
+  long long lay_top = 0;  // lay_start[n_lay - 1] (n_lay > 0)
   unsigned long long rounds = 0, tot_parents = 0, tot_children = 0, tot_solutions = 0;
   int exit_code = RND_EXIT_PAUSE;
+  // this CTA's sub-slices of a chunk of geo_n parents (relative to the chunk's start: they depend on n alone, and
+  // n == M in almost every round, so the four divisions run only when n changes)
+  long long geo_n = -1;
+  int geo_a0 = 0, geo_len0 = 0, geo_a1 = 0, geo_len1 = 0;
   // (0) the next round's chunk: popBackBulk(m, M) -> sm.plan; -1 or the exit code (uniform decisions: every CTA
   // holds the same state)
   const auto plan = [&]() {
@@ -428,14 +439,20 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       // single slice per CTA left the bottom CTA with 3x the average children, and its build + node stores were the
       // round's critical path; pairing k with 2G-1-k evens the load without knowing it in advance.
       // (n <= 768 G and k < G <= 256: the products fit 32 bits — 64-bit divisions are slow emulated sequences)
-      const unsigned n32 = static_cast<unsigned>(chunk_n), uG2 = static_cast<unsigned>(G2), uk = static_cast<unsigned>(k);
-      const int a0 = static_cast<int>(n32 * uk / uG2), a1 = static_cast<int>(n32 * (uG2 - 1u - uk) / uG2);
+      if (chunk_n != geo_n) {
+        geo_n = chunk_n;
+        const unsigned n32 = static_cast<unsigned>(chunk_n), uG2 = static_cast<unsigned>(G2), uk = static_cast<unsigned>(k);
+        geo_a0 = static_cast<int>(n32 * uk / uG2);
+        geo_len0 = static_cast<int>(n32 * (uk + 1u) / uG2) - geo_a0;
+        geo_a1 = static_cast<int>(n32 * (uG2 - 1u - uk) / uG2);
+        geo_len1 = static_cast<int>(n32 * (uG2 - uk) / uG2) - geo_a1;
+      }
       if (lane == 0) {
         sm.plan.s0 = chunk_s0;
-        sm.plan.a0 = a0;
-        sm.plan.len0 = static_cast<int>(n32 * (uk + 1u) / uG2) - a0;
-        sm.plan.a1 = a1;
-        sm.plan.len1 = static_cast<int>(n32 * (uG2 - uk) / uG2) - a1;
+        sm.plan.a0 = geo_a0;
+        sm.plan.len0 = geo_len0;
+        sm.plan.a1 = geo_a1;
+        sm.plan.len1 = geo_len1;
         sm.plan.epoch = epoch;
         sm.plan.top = n_lay - 1;
       }
@@ -471,7 +488,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
 #pragma unroll
       for (int i = 0; i < T / 32; i++) tot += sm.warp_tot64[i];
       const unsigned my_children = static_cast<unsigned>(tot & 0xFFFFF), my_leaves = static_cast<unsigned>(tot >> 20) & 0xFFFu;
-      const unsigned cnt0 = static_cast<unsigned>(tot >> 32);
+      const unsigned cnt0 = static_cast<unsigned>(tot >> 32) & 0xFFFFFu;
       unsigned long long* const slots = sy->slot[epoch & 1u];
       const unsigned long long e = static_cast<unsigned long long>(epoch) << 32;
       if (lane < 2)
@@ -491,9 +508,14 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         // ---- (8) the pool's layers after the round: every layer that starts inside the chunk is consumed, the
         // round's children form the new top layer (same computation in every CTA).  The workers read the stack only
         // in their poll, and all of them have finished this round's poll (they arrived at LL_BAR_SCAN) and start
-        // the next one after the handoff: nobody reads an entry while it changes.
+        // the next one after the handoff: nobody reads an entry while it changes.  (lay_top = lay_start[n_lay - 1]:
+        // the loop ends at the top layer in most rounds, without waiting for a shared-memory load.)
         int nl = n_lay;
-        while (nl > 0 && sm.lay_start[nl - 1] >= chunk_s0) --nl;
+        long long below = lay_top;
+        while (nl > 0 && below >= chunk_s0) {
+          --nl;
+          below = nl > 0 ? sm.lay_start[nl - 1] : -1;
+        }
         __syncwarp();  // (every lane has read the entry lane 0 may overwrite)
         if (round_children > 0) {
           if (lane == 0) {
@@ -501,8 +523,10 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
             sm.lay_epoch[nl] = epoch;
           }
           ++nl;
+          below = chunk_s0;
         }
         n_lay = nl;
+        lay_top = below;
         // ---- (9) the pool after the round, and the next round's chunk
         size = chunk_s0 + round_children;
         ++rounds;
@@ -583,7 +607,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         break;
       }
       uint32_t cm[LL_PPT];
-      int leaves = 0, mine = 0, mine0 = 0;
+      int leaves = 0, mine = 0, mine0 = 0, fert = 0;
 #pragma unroll
       for (int q = 0; q < LL_PPT; q++) {
         const int i = LL_PPT * t + q;
@@ -594,12 +618,15 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
           leaves += (w3 & LL_LEAF) ? 1 : 0;
           mine += __popc(cm[q]);
           if (i < len0) mine0 += __popc(cm[q]);
+          fert += cm[q] != 0u ? 1 : 0;
         }
       }
       TSB_PROF(prof_w, 0, LL_PROF_POLL)
-      // ---- (3) block scan: children | leaves << 20 | children of the bottom sub-slice << 32
+      // ---- (3) block scan: children | leaves << 20 | children of the bottom sub-slice << 32 | parents with
+      // children << 52 (at most 13 056, 768, 13 056 and 768 per CTA: no field overflows into the next)
       unsigned long long incl = static_cast<unsigned long long>(mine) | static_cast<unsigned long long>(leaves) << 20 |
-                                static_cast<unsigned long long>(mine0) << 32;
+                                static_cast<unsigned long long>(mine0) << 32 |
+                                static_cast<unsigned long long>(fert) << 52;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
         const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
@@ -615,12 +642,14 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         tot += sm.warp_tot64[i];
       }
       const int my_children = static_cast<int>(tot & 0xFFFFF);
-      const int cnt0 = static_cast<int>(tot >> 32);
+      const int cnt0 = static_cast<int>(tot >> 32 & 0xFFFFF);
       {
         uint16_t* it = sm.item + (static_cast<int>((woff + incl) & 0xFFFFF) - mine);
+        uint16_t* f = sm.fertile + 32 * LL_PPT * wid + (static_cast<int>(incl >> 52) - fert);  // (my warp's list)
 #pragma unroll
         for (int q = 0; q < LL_PPT; q++) {
           uint32_t m = cm[q];
+          if (m) *f++ = static_cast<uint16_t>(LL_PPT * t + q);
           while (m) {
             const int s = __ffs(m) - 1;
             m &= m - 1;
@@ -628,16 +657,24 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
           }
         }
       }
-      // ---- (5) the diagonals of my parents (the counts are on their way meanwhile).  Computed for all of them,
-      // side by side: only those of parents with children are read, and skipping the others would run a thread's
-      // parents one after the other (so would storing each before loading the next: the compiler cannot tell the
-      // arrays apart).
-      {
-        uint4 p[LL_PPT];
+      // ---- (5) the diagonals of the parents with children (the counts are on their way meanwhile; ll_build_child
+      // reads no others: about a third of the parents have none).  Each warp takes its own list, all loads first: a
+      // list of the whole CTA costs one more CTA barrier and measured slower (DESIGN §5).
+      __syncwarp();  // (my warp's list is complete)
+      const int n_fert = static_cast<int>(__shfl_sync(0xFFFFFFFFu, incl, 31) >> 52);
+      const uint16_t* const fl = sm.fertile + 32 * LL_PPT * wid;
+      // (DG parents side by side: three do not fit the 96 registers a thread has at two CTAs per SM at N >= 19, nor,
+      // as ptxas allocates them, at N <= 5)
+      constexpr int DG = N >= 19 || N <= 5 ? 2 : LL_PPT;
 #pragma unroll
-        for (int q = 0; q < LL_PPT; q++) p[q] = sm.parent[LL_PPT * t + q];
+      for (int q0 = 0; q0 < LL_PPT; q0 += DG) {
+        uint4 p[DG];
 #pragma unroll
-        for (int q = 0; q < LL_PPT; q++) sm.diag[LL_PPT * t + q] = ll_parent_diag<N>(p[q]);
+        for (int q = q0; q < q0 + DG && q < LL_PPT; q++)
+          if (lane + 32 * q < n_fert) p[q - q0] = sm.parent[fl[lane + 32 * q]];
+#pragma unroll
+        for (int q = q0; q < q0 + DG && q < LL_PPT; q++)
+          if (lane + 32 * q < n_fert) sm.diag[fl[lane + 32 * q]] = ll_parent_diag<N>(p[q - q0]);
       }
       ll_bar(T);  // items and diagonals complete
       TSB_PROF(prof_w, 0, LL_PROF_SCAN)
