@@ -14,6 +14,7 @@
 #include <mutex>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "nq_expand.cuh"
@@ -25,6 +26,7 @@
 #include "pfsp_wide.cuh"
 #include "tsb200.h"
 
+// Internals shared by both handle types (the handles themselves are the header's types, defined after this block)
 namespace {
 
 thread_local std::string g_last_cuda_error;
@@ -54,6 +56,10 @@ int env_xfer() {
 bool env_no_register() {
   const char* s = std::getenv("TSB200_NO_REGISTER");
   return s && *s && *s != '0';
+}
+bool env_no_rounds() {
+  const char* v = std::getenv("TSB200_NO_ROUNDS");
+  return v && *v && *v != '0';
 }
 
 // Host ranges the CALLER asked to page-lock + map (tsb_*_register_host): cudaMemcpyAsync is truly asynchronous
@@ -124,6 +130,249 @@ int query_device(int device, DeviceInfo& di) {
   return TSB_OK;
 }
 
+struct PoolExtent {
+  long long b, e;  // arena positions [b, e)
+};
+
+// Device-resident pool: a stack of extents inside one arena of `rec`-byte nodes.  A round reads the newest
+// nodes in place (possibly spanning several extents) and appends the children above the top, so nothing is
+// copied; the holes left behind are reclaimed by compacting into the second arena when the top reaches the end.
+struct DevicePool {
+  uint8_t* arena[2] = {nullptr, nullptr};
+  long long cap = 0;  // nodes per arena
+  int cur = 0;
+  std::vector<PoolExtent> ext;
+  long long size = 0;
+  // the node format (set_format)
+  size_t rec = 0, slack = 0;
+  long long align = 1;        // extents start at a multiple of `align` records
+  int fanout = 0;             // most children one node can have
+  long long default_cap = 0;  // nodes the arena starts with
+
+  // `node_bytes`-byte nodes read in tiles of `tile` records (full-tile loads may run past the top)
+  void set_format(size_t node_bytes, int tile, long long node_align, int max_children, long long start_cap) {
+    rec = node_bytes;
+    slack = static_cast<size_t>(tile) * node_bytes;
+    align = node_align;
+    fanout = max_children;
+    default_cap = start_cap;
+  }
+  // (read when the arena is first allocated: the search drivers keep handles between searches)
+  long long min_cap() const {
+    if (const long long c = env_pool_cap(); c > 0) return c;
+    return default_cap;
+  }
+  long long top() const { return ext.empty() ? 0 : ext.back().e; }
+  // where the next extent may start
+  long long aligned_top() const { return (top() + align - 1) / align * align; }
+  size_t bytes(long long nodes) const { return static_cast<size_t>(nodes) * rec + slack + 64; }
+  int ensure_arena(int which) {
+    if (!arena[which]) TSB_CUDA(cudaMalloc(&arena[which], bytes(cap)));
+    return TSB_OK;
+  }
+  // all extents -> [0, size) of the other arena (or of fresh, larger arenas when `new_cap` > cap)
+  int compact(cudaStream_t s, long long new_cap) {
+    uint8_t* dst = nullptr;
+    const bool grow = new_cap > cap;
+    if (grow) {
+      TSB_CUDA(cudaMalloc(&dst, bytes(new_cap)));
+    } else {
+      int rc = ensure_arena(cur ^ 1);
+      if (rc != TSB_OK) return rc;
+      dst = arena[cur ^ 1];
+    }
+    long long at = 0;
+    for (const PoolExtent& x : ext) {
+      TSB_CUDA(cudaMemcpyAsync(dst + at * rec, arena[cur] + x.b * rec, static_cast<size_t>(x.e - x.b) * rec,
+                               cudaMemcpyDeviceToDevice, s));
+      at += x.e - x.b;
+    }
+    TSB_CUDA(cudaStreamSynchronize(s));
+    if (grow) {
+      for (int i = 0; i < 2; i++) {
+        if (arena[i]) cudaFree(arena[i]);
+        arena[i] = nullptr;
+      }
+      arena[0] = dst;
+      cur = 0;
+      cap = new_cap;
+    } else {
+      cur ^= 1;
+    }
+    ext.clear();
+    if (at) ext.push_back({0, at});
+    return TSB_OK;
+  }
+  // room for `extra` nodes above the top
+  int reserve(cudaStream_t s, long long extra) {
+    if (cap == 0) {
+      cap = std::max<long long>(min_cap(), extra + 1024);
+      int rc = ensure_arena(cur);
+      if (rc != TSB_OK) return rc;
+    }
+    if (top() + extra <= cap) return TSB_OK;
+    const long long need = size + extra;
+    return compact(s, need > cap ? std::max<long long>(2 * cap, need + need / 2) : cap);
+  }
+  // the pool as ONE contiguous stack [0, size) in an arena of at least `need` nodes (the persistent kernels' layout)
+  int make_stack(cudaStream_t s, long long need) {
+    if (need > cap) return compact(s, std::max<long long>(2 * cap, need + need / 2));
+    if (ext.size() != 1 || ext[0].b != 0) return compact(s, cap);
+    return TSB_OK;
+  }
+  // a persistent launch left the pool as the stack [0, n)
+  void set_stack(long long n) {
+    size = n;
+    ext.clear();
+    if (n) ext.push_back({0, n});
+  }
+  // the newest n nodes, as pieces in logical order
+  void top_pieces(long long n, std::vector<PoolExtent>* pieces) const {
+    pieces->clear();
+    long long left = n;
+    for (size_t i = ext.size(); i-- > 0 && left > 0;) {
+      const long long t = std::min(left, ext[i].e - ext[i].b);
+      pieces->insert(pieces->begin(), PoolExtent{ext[i].e - t, ext[i].e});
+      left -= t;
+    }
+  }
+  // drop the newest n nodes
+  void pop(long long n) {
+    long long left = n;
+    while (left > 0 && !ext.empty()) {
+      PoolExtent& x = ext.back();
+      const long long t = std::min(left, x.e - x.b);
+      x.e -= t;
+      left -= t;
+      if (x.e == x.b) ext.pop_back();
+    }
+    size -= n;
+  }
+  // n nodes written at [at, at + n) become the newest extent
+  void push_extent(long long at, long long n) {
+    if (!n) return;
+    ext.push_back({at, at + n});
+    size += n;
+  }
+  void release() {
+    for (int i = 0; i < 2; i++) {
+      if (arena[i]) cudaFree(arena[i]);
+      arena[i] = nullptr;
+    }
+    ext.clear();
+    size = 0;
+    cap = 0;
+  }
+};
+
+// state of the fused expand kernels of one handle (expand_common.cuh)
+struct ExpandCtx {
+  uint32_t* d_cmask = nullptr;  // side array of the round, `side_bytes` per tile: PFSP: one child mask per parent;
+                                // N-Queens: the tile's items (one uint16 per child)
+  int* d_tile = nullptr;        // per-tile child counts
+  long long tile_cap = 0;       // tiles the two arrays above hold
+  long long side_bytes = 0;
+  tsb::ExpandState* d_st = nullptr;
+  tsb::ExpandResult* h_res = nullptr;  // pinned + mapped: written by the scan kernel of a round
+  tsb::ExpandResult* d_res = nullptr;  // device alias of h_res
+  unsigned epoch = 0;
+  // (clears are ordered on the stream the kernels run on: the handle's streams do not synchronise with the
+  // legacy default stream)
+  int reserve(long long tiles, long long side_bytes_per_tile, cudaStream_t s, int best_init = 0x7FFFFFFF) {
+    if (!d_st) {
+      TSB_CUDA(cudaMalloc(&d_st, sizeof(tsb::ExpandState)));
+      const tsb::ExpandState init{0ull, best_init, 0};
+      TSB_CUDA(cudaMemcpyAsync(d_st, &init, sizeof(init), cudaMemcpyHostToDevice, s));
+      TSB_CUDA(cudaStreamSynchronize(s));  // `init` lives on this stack frame
+    }
+    if (!h_res) {
+      TSB_CUDA(cudaHostAlloc(&h_res, sizeof(tsb::ExpandResult), cudaHostAllocPortable | cudaHostAllocMapped));
+      // (epochs start at 1: recycled pinned memory may hold another handle's old record, epoch included — the early
+      // wait below would take it for this handle's first round)
+      std::memset(h_res, 0, sizeof(tsb::ExpandResult));
+      TSB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&d_res), h_res, 0));
+    }
+    if (tiles > tile_cap || side_bytes_per_tile > side_bytes) {
+      side_bytes_per_tile = std::max(side_bytes_per_tile, side_bytes);
+      if (d_cmask) cudaFree(d_cmask);
+      if (d_tile) cudaFree(d_tile);
+      d_cmask = nullptr;
+      d_tile = nullptr;
+      tile_cap = 0;
+      const long long cap = std::max<long long>(tiles + tiles / 4 + 16, 1024);
+      TSB_CUDA(cudaMalloc(&d_cmask, static_cast<size_t>(cap) * side_bytes_per_tile + 64));
+      TSB_CUDA(cudaMalloc(&d_tile, static_cast<size_t>(cap) * sizeof(int)));
+      tile_cap = cap;
+      side_bytes = side_bytes_per_tile;
+    }
+    return TSB_OK;
+  }
+  // Wait for the round's result record.  `early`: return as soon as the build kernel's first CTA has published
+  // the counts (it does so in its prologue) — the children are still being written, which is fine for a caller
+  // whose next use of them is ordered on the same stream (the pool); the host then prepares and launches the next
+  // round while this one finishes, which hides the launch + synchronisation latency of small rounds.
+  int wait_result(unsigned want_epoch, cudaStream_t s, bool early) {
+    if (early) {
+      const volatile unsigned long long* ep = &h_res->epoch;
+      for (unsigned spin = 0;; spin++) {
+        if (*ep == want_epoch) return TSB_OK;
+        if ((spin & 1023u) == 1023u) {  // a faulted kernel never publishes: ask the stream now and then
+          const cudaError_t q = cudaStreamQuery(s);
+          if (q == cudaSuccess) return *ep == want_epoch ? TSB_OK : TSB_ECUDA;
+          if (q != cudaErrorNotReady) {
+            g_last_cuda_error = std::string("expand kernels: ") + cudaGetErrorString(q);
+            (void)cudaGetLastError();
+            return TSB_ECUDA;
+          }
+        }
+      }
+    }
+    TSB_CUDA(cudaStreamSynchronize(s));
+    return h_res->epoch == want_epoch ? TSB_OK : TSB_ECUDA;
+  }
+  void release() {
+    if (d_cmask) cudaFree(d_cmask);
+    if (d_tile) cudaFree(d_tile);
+    if (d_st) cudaFree(d_st);
+    if (h_res) cudaFreeHost(h_res);
+    d_cmask = nullptr;
+    d_tile = nullptr;
+    d_st = nullptr;
+    h_res = d_res = nullptr;
+  }
+};
+
+// state of the persistent multi-round kernel of one handle (nq_rounds_ll.cuh, pfsp_rounds.cuh)
+struct RoundsCtx {
+  tsb::RoundsState* h_state = nullptr;  // pinned + mapped: written by the kernel when it leaves
+  tsb::RoundsState* d_state = nullptr;  // device alias of h_state
+  void* d_sync = nullptr;               // the kernel's exchange flags: tsb::LlSync or tsb::PfRoundsSync
+  unsigned epoch = 0;                   // epoch the last launch left the flags at
+  template <class Sync>
+  int ensure(cudaStream_t s) {
+    if (!h_state) {
+      TSB_CUDA(cudaHostAlloc(&h_state, sizeof(tsb::RoundsState), cudaHostAllocPortable | cudaHostAllocMapped));
+      std::memset(h_state, 0, sizeof(tsb::RoundsState));
+      TSB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&d_state), h_state, 0));
+    }
+    if (!d_sync) {
+      TSB_CUDA(cudaMalloc(&d_sync, sizeof(Sync)));
+      TSB_CUDA(cudaMemsetAsync(d_sync, 0, sizeof(Sync), s));
+    }
+    return TSB_OK;
+  }
+  template <class Sync>
+  Sync* sync() const {
+    return static_cast<Sync*>(d_sync);
+  }
+  void release() {
+    if (h_state) cudaFreeHost(h_state);
+    if (d_sync) cudaFree(d_sync);
+    h_state = d_state = nullptr;
+    d_sync = nullptr;
+  }
+};
+
 // common part of both handle types
 struct Base {
   int device = 0, M_max = 0, xfer = TSB_XFER_AUTO;
@@ -136,6 +385,19 @@ struct Base {
   size_t in_rec = 0, out_rec = 0;
   HostRegistry reg;
   uint64_t launches = 0;
+  // fused expand (evaluate + generate_children on the device) and the device-resident pool
+  ExpandCtx ex;
+  uint8_t* d_children = nullptr;  // host-buffer expand: device image of the children
+  size_t d_children_bytes = 0;
+  DevicePool pool;
+  RoundsCtx rounds;
+  // Launch configuration of the handle's kernels, by kernel: the dynamic shared memory limit is raised on first use
+  // (an attribute of the kernel in the device's context) and the CTAs per SM are queried once (0: not yet).
+  struct KernelConfig {
+    const void* fn;
+    int per_sm;
+  };
+  std::vector<KernelConfig> kernels;
 
   int init(int dev, int M, size_t irec, size_t orec) {
     device = dev;
@@ -161,6 +423,10 @@ struct Base {
   void fini() {
     cudaSetDevice(device);
     if (stream) cudaStreamSynchronize(stream);
+    ex.release();
+    rounds.release();
+    if (d_children) cudaFree(d_children);
+    pool.release();
     reg.release();
     if (d_in) cudaFree(d_in);
     if (d_out) cudaFree(d_out);
@@ -171,6 +437,55 @@ struct Base {
     if (bounce_ev[1]) cudaEventDestroy(bounce_ev[1]);
     if (stream) cudaStreamDestroy(stream);
     if (stream2) cudaStreamDestroy(stream2);
+  }
+
+  // the kernel's launch configuration, with its dynamic shared memory limit raised to `smem`
+  template <class K>
+  int configure(K kernel, size_t smem, KernelConfig** cfg = nullptr) {
+    const void* fn = reinterpret_cast<const void*>(kernel);
+    KernelConfig* c = nullptr;
+    for (KernelConfig& x : kernels)
+      if (x.fn == fn) c = &x;
+    if (!c) {
+      TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+      kernels.push_back({fn, 0});
+      c = &kernels.back();
+    }
+    if (cfg) *cfg = c;
+    return TSB_OK;
+  }
+  // persistent grid: enough CTAs to fill the GPU, never more than there are full tiles
+  template <class K>
+  int grid_for(K kernel, int threads, size_t smem, long long count, int tile, int* grid) {
+    KernelConfig* c = nullptr;
+    int rc = configure(kernel, smem, &c);
+    if (rc != TSB_OK) return rc;
+    if (c->per_sm <= 0) {
+      int per_sm = 0;
+      TSB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+      c->per_sm = std::max(per_sm, 1);
+    }
+    const long long tiles = std::max<long long>(1, count / tile);
+    *grid = static_cast<int>(std::min<long long>(tiles, static_cast<long long>(c->per_sm) * di.sms));
+    return TSB_OK;
+  }
+
+  // What a finished launch of the persistent kernel `kernel` left in *st: TSB_ECUDA when its watchdog stopped it
+  // (`stuck`: what did not complete); otherwise the pool [0, st->size) and the epoch are committed and
+  // out[0..3] += {rounds, parents, children, solutions}.
+  int finish_launch(const char* kernel, const char* stuck, tsb::RoundsState* st, uint64_t* out) {
+    *st = *rounds.h_state;
+    if (st->exit_code < 0 || st->exit_code == tsb::RND_EXIT_ABORT) {
+      g_last_cuda_error = std::string(kernel) + ": watchdog abort (" + stuck + ")";
+      return TSB_ECUDA;
+    }
+    rounds.epoch = st->epoch;
+    pool.set_stack(st->size);
+    out[0] += st->rounds;
+    out[1] += st->parents;
+    out[2] += st->children;
+    out[3] += st->solutions;
+    return TSB_OK;
   }
 
   // Copies between a caller-owned host range and the device, ordered on stream `s` (the stream the kernels
@@ -292,284 +607,26 @@ struct Base {
   }
 };
 
-// persistent grid: enough CTAs to fill the GPU, never more than there are full tiles
-template <class K>
-int grid_for(K kernel, int threads, size_t smem, long long count, int tile, int sms, int* grid, int* cache) {
-  int per_sm = *cache;
-  if (per_sm <= 0) {
-    TSB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
-    if (per_sm < 1) per_sm = 1;
-    *cache = per_sm;
-  }
-  const long long tiles = std::max<long long>(1, count / tile);
-  *grid = static_cast<int>(std::min<long long>(tiles, static_cast<long long>(per_sm) * sms));
-  return TSB_OK;
+// f(std::integral_constant<int, N>) for the board size N = 1..TSB_MAX_QUEENS
+template <int N = 1, class F>
+int with_queens(int n, F&& f) {
+  if constexpr (N > TSB_MAX_QUEENS)
+    return TSB_EINVAL;
+  else
+    return n == N ? f(std::integral_constant<int, N>{}) : with_queens<N + 1>(n, f);
+}
+// f(std::integral_constant<int, M>) for the template machine count mt = 5, 10 or 20
+template <class F>
+int with_machines(int mt, F&& f) {
+  if (mt == 5) return f(std::integral_constant<int, 5>{});
+  if (mt == 10) return f(std::integral_constant<int, 10>{});
+  return f(std::integral_constant<int, 20>{});
 }
 
-}  // namespace
-
-// ============================================================================ N-Queens
-struct PoolExtent {
-  long long b, e;  // arena positions [b, e)
-};
-
-// state of the fused expand kernels of one handle (expand_common.cuh)
-struct ExpandCtx {
-  uint32_t* d_cmask = nullptr;  // side array of the round, `side_bytes` per tile: PFSP: one child mask per parent;
-                                // N-Queens: the tile's items (one uint16 per child)
-  int* d_tile = nullptr;        // per-tile child counts
-  long long tile_cap = 0;       // tiles the two arrays above hold
-  long long side_bytes = 0;
-  tsb::ExpandState* d_st = nullptr;
-  tsb::ExpandResult* h_res = nullptr;  // pinned + mapped: written by the scan kernel of a round
-  tsb::ExpandResult* d_res = nullptr;  // device alias of h_res
-  unsigned epoch = 0;
-  int occ_count = 0, occ_build = 0;
-  bool attr_set = false;
-  // (clears are ordered on the stream the kernels run on: the handle's streams do not synchronise with the
-  // legacy default stream)
-  int reserve(long long tiles, long long side_bytes_per_tile, cudaStream_t s, int best_init = 0x7FFFFFFF) {
-    if (!d_st) {
-      TSB_CUDA(cudaMalloc(&d_st, sizeof(tsb::ExpandState)));
-      const tsb::ExpandState init{0ull, best_init, 0};
-      TSB_CUDA(cudaMemcpyAsync(d_st, &init, sizeof(init), cudaMemcpyHostToDevice, s));
-      TSB_CUDA(cudaStreamSynchronize(s));  // `init` lives on this stack frame
-    }
-    if (!h_res) {
-      TSB_CUDA(cudaHostAlloc(&h_res, sizeof(tsb::ExpandResult), cudaHostAllocPortable | cudaHostAllocMapped));
-      // (epochs start at 1: recycled pinned memory may hold another handle's old record, epoch included — the early
-      // wait below would take it for this handle's first round)
-      std::memset(h_res, 0, sizeof(tsb::ExpandResult));
-      TSB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&d_res), h_res, 0));
-    }
-    if (tiles > tile_cap || side_bytes_per_tile > side_bytes) {
-      side_bytes_per_tile = std::max(side_bytes_per_tile, side_bytes);
-      if (d_cmask) cudaFree(d_cmask);
-      if (d_tile) cudaFree(d_tile);
-      d_cmask = nullptr;
-      d_tile = nullptr;
-      tile_cap = 0;
-      const long long cap = std::max<long long>(tiles + tiles / 4 + 16, 1024);
-      TSB_CUDA(cudaMalloc(&d_cmask, static_cast<size_t>(cap) * side_bytes_per_tile + 64));
-      TSB_CUDA(cudaMalloc(&d_tile, static_cast<size_t>(cap) * sizeof(int)));
-      tile_cap = cap;
-      side_bytes = side_bytes_per_tile;
-    }
-    return TSB_OK;
-  }
-  // Wait for the round's result record.  `early`: return as soon as the build kernel's first CTA has published
-  // the counts (it does so in its prologue) — the children are still being written, which is fine for a caller
-  // whose next use of them is ordered on the same stream (the pool); the host then prepares and launches the next
-  // round while this one finishes, which hides the launch + synchronisation latency of small rounds.
-  int wait_result(unsigned want_epoch, cudaStream_t s, bool early) {
-    if (early) {
-      const volatile unsigned long long* ep = &h_res->epoch;
-      for (unsigned spin = 0;; spin++) {
-        if (*ep == want_epoch) return TSB_OK;
-        if ((spin & 1023u) == 1023u) {  // a faulted kernel never publishes: ask the stream now and then
-          const cudaError_t q = cudaStreamQuery(s);
-          if (q == cudaSuccess) return *ep == want_epoch ? TSB_OK : TSB_ECUDA;
-          if (q != cudaErrorNotReady) {
-            g_last_cuda_error = std::string("expand kernels: ") + cudaGetErrorString(q);
-            (void)cudaGetLastError();
-            return TSB_ECUDA;
-          }
-        }
-      }
-    }
-    TSB_CUDA(cudaStreamSynchronize(s));
-    return h_res->epoch == want_epoch ? TSB_OK : TSB_ECUDA;
-  }
-  void release() {
-    if (d_cmask) cudaFree(d_cmask);
-    if (d_tile) cudaFree(d_tile);
-    if (d_st) cudaFree(d_st);
-    if (h_res) cudaFreeHost(h_res);
-    d_cmask = nullptr;
-    d_tile = nullptr;
-    d_st = nullptr;
-    h_res = d_res = nullptr;
-  }
-};
-
-// Device-resident pool: a stack of extents inside one arena of `rec`-byte nodes.  A round reads the newest
-// nodes in place (possibly spanning several extents) and appends the children above the top, so nothing is
-// copied; the holes left behind are reclaimed by compacting into the second arena when the top reaches the end.
-struct DevicePool {
-  uint8_t* arena[2] = {nullptr, nullptr};
-  long long cap = 0;  // nodes per arena
-  int cur = 0;
-  size_t rec = 0, slack = 0;
-  std::vector<PoolExtent> ext;
-  long long size = 0;
-  uint64_t compactions = 0;
-  long long top() const { return ext.empty() ? 0 : ext.back().e; }
-  size_t bytes(long long nodes) const { return static_cast<size_t>(nodes) * rec + slack + 64; }
-  int ensure_arena(int which, long long nodes) {
-    (void)nodes;
-    if (!arena[which]) TSB_CUDA(cudaMalloc(&arena[which], bytes(cap)));
-    return TSB_OK;
-  }
-  // all extents -> [0, size) of the other arena (or of fresh, larger arenas when `new_cap` > cap)
-  int compact(cudaStream_t s, long long new_cap) {
-    uint8_t* dst = nullptr;
-    const bool grow = new_cap > cap;
-    if (grow) {
-      TSB_CUDA(cudaMalloc(&dst, static_cast<size_t>(new_cap) * rec + slack + 64));
-    } else {
-      int rc = ensure_arena(cur ^ 1, cap);
-      if (rc != TSB_OK) return rc;
-      dst = arena[cur ^ 1];
-    }
-    long long at = 0;
-    for (const PoolExtent& x : ext) {
-      TSB_CUDA(cudaMemcpyAsync(dst + at * rec, arena[cur] + x.b * rec, static_cast<size_t>(x.e - x.b) * rec,
-                               cudaMemcpyDeviceToDevice, s));
-      at += x.e - x.b;
-    }
-    TSB_CUDA(cudaStreamSynchronize(s));
-    if (grow) {
-      for (int i = 0; i < 2; i++) {
-        if (arena[i]) cudaFree(arena[i]);
-        arena[i] = nullptr;
-      }
-      arena[0] = dst;
-      cur = 0;
-      cap = new_cap;
-    } else {
-      cur ^= 1;
-    }
-    ext.clear();
-    if (at) ext.push_back({0, at});
-    ++compactions;
-    return TSB_OK;
-  }
-  // room for `extra` nodes above the top
-  int reserve(cudaStream_t s, long long extra, long long min_cap) {
-    if (cap == 0) {
-      cap = std::max<long long>(min_cap, extra + 1024);
-      int rc = ensure_arena(cur, cap);
-      if (rc != TSB_OK) return rc;
-    }
-    if (top() + extra <= cap) return TSB_OK;
-    const long long need = size + extra;
-    return compact(s, need > cap ? std::max<long long>(2 * cap, need + need / 2) : cap);
-  }
-  void release() {
-    for (int i = 0; i < 2; i++) {
-      if (arena[i]) cudaFree(arena[i]);
-      arena[i] = nullptr;
-    }
-    ext.clear();
-    size = 0;
-    cap = 0;
-  }
-};
-
-// state of the persistent multi-round kernel of one handle (nq_rounds_ll.cuh)
-struct RoundsCtx {
-  tsb::RoundsState* h_state = nullptr;  // pinned + mapped: written by the kernel when it leaves
-  tsb::RoundsState* d_state = nullptr;  // device alias of h_state
-  unsigned epoch = 0;
-  tsb::FatNode* d_fat = nullptr;  // the pool in the self-validating 32-byte format, while the LL kernel owns it
-  long long fat_cap = 0;
-  bool in_fat = false;            // the pool currently lives in d_fat (the plain arena is stale)
-  bool attr_llv[3] = {false, false, false};
-  tsb::LlSync* d_ll = nullptr;
-  int ensure_fat(long long cap, cudaStream_t s) {
-    if (!d_ll) {
-      TSB_CUDA(cudaMalloc(&d_ll, sizeof(tsb::LlSync)));
-      TSB_CUDA(cudaMemsetAsync(d_ll, 0, sizeof(tsb::LlSync), s));
-    }
-    if (cap <= fat_cap) return TSB_OK;
-    if (d_fat) cudaFree(d_fat);
-    d_fat = nullptr;
-    fat_cap = 0;
-    TSB_CUDA(cudaMalloc(&d_fat, static_cast<size_t>(cap) * sizeof(tsb::FatNode)));
-    fat_cap = cap;
-    return TSB_OK;
-  }
-  int ensure() {
-    if (!h_state) {
-      TSB_CUDA(cudaHostAlloc(&h_state, sizeof(tsb::RoundsState), cudaHostAllocPortable | cudaHostAllocMapped));
-      std::memset(h_state, 0, sizeof(tsb::RoundsState));
-      TSB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&d_state), h_state, 0));
-    }
-    return TSB_OK;
-  }
-  void release() {
-    if (h_state) cudaFreeHost(h_state);
-    if (d_fat) cudaFree(d_fat);
-    if (d_ll) cudaFree(d_ll);
-    h_state = d_state = nullptr;
-    d_fat = nullptr;
-    d_ll = nullptr;
-    fat_cap = 0;
-    in_fat = false;
-  }
-};
-
-struct tsb_nq : Base {
-  tsb_nq* sibling[3] = {nullptr, nullptr, nullptr};  // further pools on the same device, owned by this handle (tsb_nq_sibling)
-  int N = 0, g = 1;
-  RoundsCtx rounds;
-  int tile_threads = 0;  // env TSB200_NQ_TILE_THREADS = 128: always the TMA-pipelined kernel (tests force it on small chunks)
-  int occ = 0;  // cached CTAs per SM of the TMA-pipelined evaluator
-  bool attr_set = false;
-  // fused expand (evaluate + generate_children on the device) and the device-resident pool
-  ExpandCtx ex;
-  uint8_t* d_children = nullptr;  // host-buffer expand: device image of the children
-  size_t d_children_bytes = 0;
-  DevicePool pool;
-};
-
-namespace {
-
-int nq_materialize(tsb_nq* h);  // (defined with the LL kernel's launch helpers below)
-
-// small chunks (fewer than two 512-parent tiles per SM — the reference's default --M 50000 is 97 tiles) take the
-// one-parent-per-thread kernel, everything else the TMA-pipelined one
-template <int N>
-int launch_nq_n(tsb_nq* h, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
-  if (count < 2LL * h->di.sms * tsb::NQ_TILE && h->tile_threads != 128) {
-    const int grid = static_cast<int>((count + tsb::NQ_SMALL - 1) / tsb::NQ_SMALL);
-    tsb::nq_evaluate_small_kernel<N><<<grid, tsb::NQ_SMALL, 0, s>>>(in, out, static_cast<int>(count));
-    TSB_CUDA(cudaGetLastError());
-    h->launches++;
-    return TSB_OK;
-  }
-  auto kernel = tsb::nq_evaluate_kernel<N>;
-  const size_t smem = sizeof(tsb::NqSmem<N>) + 128;
-  if (!h->attr_set) {
-    TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    h->attr_set = true;
-  }
-  int grid = 1;
-  int rc = grid_for(kernel, tsb::NQ_THREADS, smem, count, tsb::NQ_TILE, h->di.sms, &grid, &h->occ);
-  if (rc != TSB_OK) return rc;
-  kernel<<<grid, tsb::NQ_THREADS, smem, s>>>(in, out, count);
-  TSB_CUDA(cudaGetLastError());
-  h->launches++;
-  return TSB_OK;
+// bounds are int32 and `lb > best` can never hold for best >= INT32_MAX (Chapel's max(int) under --ub 0)
+inline int clamp_best(int64_t best64) {
+  return best64 > INT_MAX ? INT_MAX : best64 < INT_MIN ? INT_MIN : static_cast<int>(best64);
 }
-
-int launch_nq(tsb_nq* h, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
-  switch (h->N) {
-#define TSB_NQ_CASE(n) \
-  case n:              \
-    return launch_nq_n<n>(h, in, out, count, s);
-    TSB_NQ_CASE(1) TSB_NQ_CASE(2) TSB_NQ_CASE(3) TSB_NQ_CASE(4) TSB_NQ_CASE(5) TSB_NQ_CASE(6) TSB_NQ_CASE(7)
-    TSB_NQ_CASE(8) TSB_NQ_CASE(9) TSB_NQ_CASE(10) TSB_NQ_CASE(11) TSB_NQ_CASE(12) TSB_NQ_CASE(13)
-    TSB_NQ_CASE(14) TSB_NQ_CASE(15) TSB_NQ_CASE(16) TSB_NQ_CASE(17) TSB_NQ_CASE(18) TSB_NQ_CASE(19)
-    TSB_NQ_CASE(20)
-#undef TSB_NQ_CASE
-  }
-  return TSB_EINVAL;
-}
-
-}  // namespace
-
-namespace {
 
 // tile table of a round: pieces in logical order -> ExpandParams
 int make_params(const std::vector<PoolExtent>& pieces, int tile_records, tsb::ExpandParams* prm) {
@@ -591,6 +648,241 @@ int make_params(const std::vector<PoolExtent>& pieces, int tile_records, tsb::Ex
   return TSB_OK;
 }
 
+// ---- device-pool operations of both handle types.  `plain()` brings the pool into its plain arena first (the
+// N-Queens pool may live in the persistent kernel's own format); `expand(arena, pieces, children_d, &nc, &ns)` runs
+// one evaluate + generate_children round on the handle's stream.
+
+template <class Plain>
+int pool_push(Base& h, const void* nodes, int64_t n, Plain&& plain) {
+  TSB_CUDA(cudaSetDevice(h.device));
+  int rc = plain();
+  if (rc != TSB_OK) return rc;
+  DevicePool& p = h.pool;
+  rc = p.reserve(h.stream, n);
+  if (rc != TSB_OK) return rc;
+  if (n == 0) return TSB_OK;
+  const long long at = p.top();
+  // (on the handle's non-blocking stream, which the kernels of the next round are ordered after)
+  rc = h.copy_h2d(p.arena[p.cur] + at * p.rec, nodes, static_cast<size_t>(n) * p.rec, h.stream);
+  if (rc != TSB_OK) return rc;
+  if (p.ext.empty())
+    p.ext.push_back({at, at + n});
+  else
+    p.ext.back().e += n;
+  p.size += n;
+  return TSB_OK;
+}
+
+template <class Plain>
+int pool_drain(Base& h, void* nodes, int64_t capacity, int64_t* n, Plain&& plain) {
+  DevicePool& p = h.pool;
+  *n = p.size;
+  if (p.size > capacity) return TSB_ENOMEM;
+  TSB_CUDA(cudaSetDevice(h.device));
+  if (int rc = plain(); rc != TSB_OK) return rc;
+  long long at = 0;
+  for (const PoolExtent& x : p.ext) {  // extents are the pool in logical (oldest first) order
+    int rc = h.copy_d2h(static_cast<uint8_t*>(nodes) + at * p.rec, p.arena[p.cur] + x.b * p.rec,
+                        static_cast<size_t>(x.e - x.b) * p.rec, h.stream);
+    if (rc != TSB_OK) return rc;
+    at += x.e - x.b;
+  }
+  p.ext.clear();
+  p.size = 0;
+  return TSB_OK;
+}
+
+// one round: popBackBulk(m, M), expand, the children pushed
+template <class Plain, class Expand>
+int pool_step(Base& h, int m, int M, int64_t* n_parents, uint64_t* n_children, uint64_t* n_solutions, Plain&& plain,
+              Expand&& expand) {
+  *n_parents = 0;
+  *n_children = *n_solutions = 0;
+  DevicePool& p = h.pool;
+  if (p.size < m) return TSB_OK;  // popBackBulk returns 0 below m (lib/commons/Pool.chpl:50-59)
+  TSB_CUDA(cudaSetDevice(h.device));
+  int rc = plain();
+  if (rc != TSB_OK) return rc;
+  const long long n = std::min<long long>(p.size, M);
+  // room above the top for the worst case (every slot of every parent survives) and the children's alignment; the
+  // chunk itself is read in place, as the newest pieces of the extent stack
+  std::vector<PoolExtent> pieces;
+  p.top_pieces(n, &pieces);
+  if (pieces.size() > tsb::EXP_MAX_PIECES) rc = p.compact(h.stream, p.cap);
+  if (rc == TSB_OK) rc = p.reserve(h.stream, n * p.fanout + 2 * (p.align - 1));
+  if (rc != TSB_OK) return rc;
+  p.top_pieces(n, &pieces);  // (positions change when the pool was compacted)
+  const long long top = p.aligned_top();
+  unsigned long long nc = 0, ns = 0;
+  uint8_t* arena = p.arena[p.cur];
+  rc = expand(arena, pieces, arena + top * p.rec, &nc, &ns);
+  if (rc != TSB_OK) return rc;
+  p.pop(n);
+  p.push_extent(top, static_cast<long long>(nc));
+  *n_parents = n;
+  *n_children = nc;
+  *n_solutions = ns;
+  return TSB_OK;
+}
+
+// `step(&np, &nc, &ns)` until a round takes no parents or max_rounds rounds have run; out[] += {rounds, parents,
+// children, solutions}
+template <class Step>
+int step_loop(int64_t max_rounds, uint64_t* out, Step&& step) {
+  for (int64_t r = 0; r < max_rounds; r++) {
+    int64_t np = 0;
+    uint64_t nc = 0, ns = 0;
+    const int rc = step(&np, &nc, &ns);
+    if (rc != TSB_OK) return rc;
+    if (np == 0) break;
+    out[0] += 1;
+    out[1] += static_cast<uint64_t>(np);
+    out[2] += nc;
+    out[3] += ns;
+  }
+  return TSB_OK;
+}
+
+// expand of host arrays: the parents through d_in, the children through d_children (room for M_max parents' worst
+// case)
+template <class Expand>
+int expand_host(Base& h, const void* parents, int count, void* children, uint64_t capacity, uint64_t* n_children,
+                uint64_t* n_solutions, Expand&& expand) {
+  TSB_CUDA(cudaSetDevice(h.device));
+  const size_t rec = h.pool.rec, need = static_cast<size_t>(h.M_max) * h.pool.fanout * rec + 64;
+  if (h.d_children_bytes < need) {
+    if (h.d_children) cudaFree(h.d_children);
+    h.d_children = nullptr;
+    h.d_children_bytes = 0;
+    TSB_CUDA(cudaMalloc(&h.d_children, need));
+    h.d_children_bytes = need;
+  }
+  int rc = h.copy_h2d(h.d_in, parents, rec * static_cast<size_t>(count), h.stream);
+  if (rc != TSB_OK) return rc;
+  unsigned long long nc = 0, ns = 0;
+  const std::vector<PoolExtent> pieces{{0, count}};
+  rc = expand(h.d_in, pieces, h.d_children, &nc, &ns);
+  if (rc != TSB_OK) return rc;
+  *n_children = nc;
+  *n_solutions = ns;
+  if (nc > capacity) return TSB_ENOMEM;  // the caller's children array is too small; counts are valid
+  return h.copy_d2h(children, h.d_children, nc * rec, h.stream);
+}
+
+// Work stealing between device pools (SURVEY §8f row 3; the reference steals between its per-GPU host pools,
+// nqueens_multigpu_chpl.chpl:255-312): the OLDEST half of the victim's pool (popFrontBulkFree,
+// lib/commons/Pool_par.chpl:178-191: size / 2 nodes from the front, only if size >= 2 m) moves to the top of the
+// thief's pool, device to device (cudaMemcpyPeerAsync: peer-to-peer between two GPUs, a plain copy on one), order
+// preserved.  Both pools must be quiescent (no round in flight); the caller serialises access to both handles.
+// `plain()` brings both pools into their plain arenas.
+template <class Plain>
+int pool_steal(Base& victim, Base& thief, int m, int64_t* n_stolen, Plain&& plain) {
+  *n_stolen = 0;
+  DevicePool &v = victim.pool, &t = thief.pool;
+  if (v.size < 2LL * m) return TSB_OK;
+  int rc = plain();
+  if (rc != TSB_OK) return rc;
+  const long long want = v.size / 2;
+  const bool trace = std::getenv("TSB200_TRACE") != nullptr;
+  const auto tnow = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
+  const double tr0 = trace ? tnow() : 0;
+  TSB_CUDA(cudaSetDevice(thief.device));
+  rc = t.reserve(thief.stream, want);
+  if (rc != TSB_OK) return rc;
+  long long at = t.aligned_top();
+  if (at + want > t.cap) {
+    rc = t.compact(thief.stream, std::max<long long>(2 * t.cap, t.size + want + 1024));
+    if (rc != TSB_OK) return rc;
+    at = t.aligned_top();
+  }
+  TSB_CUDA(cudaSetDevice(victim.device));
+  long long left = want, dst = at;
+  while (left > 0 && !v.ext.empty()) {
+    PoolExtent& x = v.ext.front();
+    const long long n = std::min(left, x.e - x.b);
+    TSB_CUDA(cudaMemcpyPeerAsync(t.arena[t.cur] + dst * t.rec, thief.device, v.arena[v.cur] + x.b * v.rec,
+                                 victim.device, static_cast<size_t>(n) * v.rec, victim.stream));
+    x.b += n;
+    dst += n;
+    left -= n;
+    if (x.b == x.e) v.ext.erase(v.ext.begin());
+  }
+  TSB_CUDA(cudaStreamSynchronize(victim.stream));
+  const long long got = want - left;
+  v.size -= got;
+  t.push_extent(at, got);
+  *n_stolen = got;
+  if (trace)
+    std::fprintf(stderr, "[tsb200] steal: %lld nodes (%.1f MB) device %d -> %d in %.2f ms (victim keeps %lld, thief has %lld)\n",
+                 got, got * v.rec / 1e6, victim.device, thief.device, tnow() - tr0, v.size, t.size);
+  return TSB_OK;
+}
+
+void enable_peer(int a, int b) {
+  if (a == b) return;
+  int can = 0;
+  if (cudaDeviceCanAccessPeer(&can, a, b) == cudaSuccess && can) {
+    cudaSetDevice(a);
+    if (cudaDeviceEnablePeerAccess(b, 0) != cudaSuccess) (void)cudaGetLastError();  // (already enabled is fine)
+  }
+  (void)cudaGetLastError();
+}
+
+}  // namespace
+
+// ============================================================================ handles
+struct tsb_nq : Base {
+  tsb_nq* sibling[3] = {nullptr, nullptr, nullptr};  // further pools on the same device, owned by this handle (tsb_nq_sibling)
+  int N = 0, g = 1;
+  int tile_threads = 0;  // env TSB200_NQ_TILE_THREADS = 128: always the TMA-pipelined kernel (tests force it on small chunks)
+  tsb::FatNode* d_fat = nullptr;  // the pool in the self-validating 32-byte format, while the LL kernel owns it
+  long long fat_cap = 0;
+  bool in_fat = false;  // the pool currently lives in d_fat (the plain arena is stale)
+};
+
+struct tsb_pfsp : Base {
+  int jobs = 0, machines = 0, pairs = 0, mt = 0;  // mt = template machine count (5, 10 or 20)
+  tsb::PfspLb1Tables* d_tab1 = nullptr;
+  tsb::Lb2Const* lb2c = nullptr;  // packed Johnson tables, passed to the lb2 kernels by value (constant bank)
+  tsb::Lb2ConstU* lb2u = nullptr; // <= 10 machines: address of the shared-memory-resident table (tsb::Lb2TabU)
+  tsb::Lb2TabU* d_tabu = nullptr;
+  bool simd16 = false;  // lb1 / lb1_d children two per register (values < 2^16, min_tails non-increasing)
+  bool wide = false;    // MAX_JOBS = 50 build: 208-byte nodes, the general kernels of pfsp_wide.cuh
+  tsb::PfspWideTables* d_wtab = nullptr;
+  uint64_t slow_rounds = 0;
+  std::vector<tsb_pfsp_node> h_chunk, h_kids;  // slow path scratch
+  std::vector<int32_t> h_bounds;
+};
+
+namespace {
+
+// ============================================================================ N-Queens
+// small chunks (fewer than two 512-parent tiles per SM — the reference's default --M 50000 is 97 tiles) take the
+// one-parent-per-thread kernel, everything else the TMA-pipelined one
+template <int N>
+int launch_nq_n(tsb_nq* h, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
+  if (count < 2LL * h->di.sms * tsb::NQ_TILE && h->tile_threads != 128) {
+    const int grid = static_cast<int>((count + tsb::NQ_SMALL - 1) / tsb::NQ_SMALL);
+    tsb::nq_evaluate_small_kernel<N><<<grid, tsb::NQ_SMALL, 0, s>>>(in, out, static_cast<int>(count));
+    TSB_CUDA(cudaGetLastError());
+    h->launches++;
+    return TSB_OK;
+  }
+  auto kernel = tsb::nq_evaluate_kernel<N>;
+  const size_t smem = sizeof(tsb::NqSmem<N>) + 128;
+  int grid = 1;
+  int rc = h->grid_for(kernel, tsb::NQ_THREADS, smem, count, tsb::NQ_TILE, &grid);
+  if (rc != TSB_OK) return rc;
+  kernel<<<grid, tsb::NQ_THREADS, smem, s>>>(in, out, count);
+  TSB_CUDA(cudaGetLastError());
+  h->launches++;
+  return TSB_OK;
+}
+
+int launch_nq(tsb_nq* h, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
+  return with_queens(h->N, [&](auto n) { return launch_nq_n<decltype(n)::value>(h, in, out, count, s); });
+}
+
 // one evaluate + generate_children round over `pieces` of `arena` (count, build); children packed at
 // `children_d`.  Synchronous: the counts come back through the host-mapped result record.
 template <int N>
@@ -600,7 +892,7 @@ int nq_expand_n(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& 
   int rc = make_params(pieces, tsb::NQ_TILE, &prm);
   if (rc != TSB_OK) return rc;
   ExpandCtx& ex = h->ex;
-  const bool trace = !ex.attr_set && std::getenv("TSB200_TRACE");
+  const bool trace = ex.epoch == 0 && std::getenv("TSB200_TRACE");  // (the handle's first round)
   const auto tnow = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
   const double tr0 = trace ? tnow() : 0;
   // (sized for the largest round up front: the items array is 1 KB * N per tile)
@@ -610,16 +902,11 @@ int nq_expand_n(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& 
   auto k1 = tsb::nq_expand_count_kernel<N>;
   auto k3 = tsb::nq_expand_build_kernel<N>;
   const size_t smem1 = sizeof(tsb::NqCountSmem) + 128, smem3 = sizeof(tsb::NqBuildSmem) + 128;
-  if (!ex.attr_set) {
-    TSB_CUDA(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem1)));
-    TSB_CUDA(cudaFuncSetAttribute(k3, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem3)));
-    ex.attr_set = true;
-  }
   const long long recs = static_cast<long long>(prm.n_tiles) * tsb::NQ_TILE;
   int g1 = 1, g3 = 1;
-  rc = grid_for(k1, tsb::NQ_THREADS, smem1, recs, tsb::NQ_TILE, h->di.sms, &g1, &ex.occ_count);
+  rc = h->grid_for(k1, tsb::NQ_THREADS, smem1, recs, tsb::NQ_TILE, &g1);
   if (rc != TSB_OK) return rc;
-  rc = grid_for(k3, tsb::NQ_THREADS, smem3, recs, tsb::NQ_TILE, h->di.sms, &g3, &ex.occ_build);
+  rc = h->grid_for(k3, tsb::NQ_THREADS, smem3, recs, tsb::NQ_TILE, &g3);
   if (rc != TSB_OK) return rc;
   prm.epoch = ++ex.epoch;
   if ((prm.n_tiles + g3 - 1) / g3 > tsb::EXP_MAX_OWN) return TSB_EINVAL;  // (M_max * N < 2^31 keeps this far away)
@@ -643,151 +930,197 @@ int nq_expand_n(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& 
   return TSB_OK;
 }
 
-int nq_expand_dispatch(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& pieces, uint8_t* children_d,
-                       cudaStream_t s, unsigned long long* nc, unsigned long long* ns, bool early = false) {
-  switch (h->N) {
-#define TSB_NQ_CASE(n) \
-  case n:              \
-    return nq_expand_n<n>(h, arena, pieces, children_d, s, nc, ns, early);
-    TSB_NQ_CASE(1) TSB_NQ_CASE(2) TSB_NQ_CASE(3) TSB_NQ_CASE(4) TSB_NQ_CASE(5) TSB_NQ_CASE(6) TSB_NQ_CASE(7)
-    TSB_NQ_CASE(8) TSB_NQ_CASE(9) TSB_NQ_CASE(10) TSB_NQ_CASE(11) TSB_NQ_CASE(12) TSB_NQ_CASE(13)
-    TSB_NQ_CASE(14) TSB_NQ_CASE(15) TSB_NQ_CASE(16) TSB_NQ_CASE(17) TSB_NQ_CASE(18) TSB_NQ_CASE(19)
-    TSB_NQ_CASE(20)
-#undef TSB_NQ_CASE
-  }
-  return TSB_EINVAL;
+int nq_expand(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& pieces, uint8_t* children_d,
+              cudaStream_t s, unsigned long long* nc, unsigned long long* ns, bool early = false) {
+  return with_queens(h->N, [&](auto n) {
+    return nq_expand_n<decltype(n)::value>(h, arena, pieces, children_d, s, nc, ns, early);
+  });
 }
 
-// the newest n nodes of a pool, as pieces in logical order
-void pool_top_pieces(const DevicePool& p, long long n, std::vector<PoolExtent>* pieces) {
-  pieces->clear();
-  long long left = n;
-  for (size_t i = p.ext.size(); i-- > 0 && left > 0;) {
-    const long long t = std::min(left, p.ext[i].e - p.ext[i].b);
-    pieces->insert(pieces->begin(), PoolExtent{p.ext[i].e - t, p.ext[i].e});
-    left -= t;
+// what a pool may hold: depth <= N, board[0..N) < N, the bytes past N zero (every node the reference or this library
+// creates; the persistent kernel packs a node into 125 bits on these terms, nq_rounds_ll.cuh)
+bool nq_nodes_valid(int N, const tsb_nq_node* nodes, int64_t n) {
+  for (int64_t i = 0; i < n; i++) {
+    const tsb_nq_node& x = nodes[i];
+    if (x.depth > N) return false;
+    for (int j = 0; j < TSB_MAX_QUEENS; j++)
+      if (x.board[j] >= (j < N ? N : 1)) return false;
   }
-}
-// drop the newest n nodes
-void pool_pop(DevicePool& p, long long n) {
-  long long left = n;
-  while (left > 0 && !p.ext.empty()) {
-    PoolExtent& x = p.ext.back();
-    const long long t = std::min(left, x.e - x.b);
-    x.e -= t;
-    left -= t;
-    if (x.e == x.b) p.ext.pop_back();
-  }
-  p.size -= n;
+  return true;
 }
 
-}  // namespace
-
-namespace {
-// Work stealing between device pools (SURVEY §8f row 3; the reference steals between its per-GPU host pools,
-// nqueens_multigpu_chpl.chpl:255-312): the OLDEST half of the victim's pool (popFrontBulkFree,
-// lib/commons/Pool_par.chpl:178-191: size / 2 nodes from the front, only if size >= 2 m) moves to the top of the
-// thief's pool, device to device (cudaMemcpyPeerAsync: peer-to-peer between two GPUs, a plain copy on one), order
-// preserved.  Both pools must be quiescent (no round in flight); the caller serialises access to both handles.
-int pool_steal_front(DevicePool& v, int vdev, cudaStream_t vs, DevicePool& t, int tdev, cudaStream_t ts, int m,
-                     long long min_cap, long long* n_stolen) {
-  *n_stolen = 0;
-  if (v.size < 2LL * m) return TSB_OK;
-  const long long want = v.size / 2;
-  const bool trace = std::getenv("TSB200_TRACE") != nullptr;
-  const auto tnow = [] { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
-  const double tr0 = trace ? tnow() : 0;
-  TSB_CUDA(cudaSetDevice(tdev));
-  int rc = t.reserve(ts, want, min_cap);
+template <int N>
+int nq_ll_launch_n(tsb_nq* h, const tsb::LlMultiParams& prm, int grid, int pools, int ppt, cudaStream_t s) {
+  // (one pool: one CTA per SM; several: two CTAs of LL_T workers + the exchange warp per SM, capped at 112
+  // registers; three or four pools: 66 CTAs per pool with 768 parents each on 132 SMs, see ll_slice)
+  const int var = pools == 1 ? 0 : ppt == 2 ? 1 : 2;
+  auto kernel = var == 0   ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 2>
+                : var == 1 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 2>
+                           : tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 3>;
+  const size_t smem = (ppt == 2 ? sizeof(tsb::LlSmem<tsb::LL_T, 2>) : sizeof(tsb::LlSmem<tsb::LL_T, 3>)) + 128;
+  int rc = h->configure(kernel, smem);
   if (rc != TSB_OK) return rc;
-  long long at = t.top();
-  if (t.rec == sizeof(tsb_pfsp_node)) at = (at + 1) & ~1LL;  // PFSP extents start on a 16-byte boundary
-  if (at + want > t.cap) {
-    rc = t.compact(ts, std::max<long long>(2 * t.cap, t.size + want + 1024));
-    if (rc != TSB_OK) return rc;
-    at = t.top();
-    if (t.rec == sizeof(tsb_pfsp_node)) at = (at + 1) & ~1LL;
-  }
-  TSB_CUDA(cudaSetDevice(vdev));
-  long long left = want, dst = at;
-  while (left > 0 && !v.ext.empty()) {
-    PoolExtent& x = v.ext.front();
-    const long long n = std::min(left, x.e - x.b);
-    TSB_CUDA(cudaMemcpyPeerAsync(t.arena[t.cur] + dst * t.rec, tdev, v.arena[v.cur] + x.b * v.rec, vdev,
-                                 static_cast<size_t>(n) * v.rec, vs));
-    x.b += n;
-    dst += n;
-    left -= n;
-    if (x.b == x.e) v.ext.erase(v.ext.begin());
-  }
-  TSB_CUDA(cudaStreamSynchronize(vs));
-  const long long got = want - left;
-  v.size -= got;
-  if (got) {
-    t.ext.push_back({at, at + got});
-    t.size += got;
-  }
-  *n_stolen = got;
-  if (trace)
-    std::fprintf(stderr, "[tsb200] steal: %lld nodes (%.1f MB) device %d -> %d in %.2f ms (victim keeps %lld, thief has %lld)\n",
-                 got, got * v.rec / 1e6, vdev, tdev, tnow() - tr0, v.size, t.size);
+  void* args[] = {const_cast<tsb::LlMultiParams*>(&prm)};
+  // cooperative: all CTAs of all pools co-resident (two per SM when there are two pools), or the launch fails
+  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid, pools), dim3(tsb::LL_T + 32), args, smem, s));
+  h->launches++;
   return TSB_OK;
 }
-void enable_peer(int a, int b) {
-  if (a == b) return;
-  int can = 0;
-  if (cudaDeviceCanAccessPeer(&can, a, b) == cudaSuccess && can) {
-    cudaSetDevice(a);
-    if (cudaDeviceEnablePeerAccess(b, 0) != cudaSuccess) (void)cudaGetLastError();  // (already enabled is fine)
+// the plain arena's [0, pool.size) -> d_fat
+template <int N>
+int nq_fat_import(tsb_nq* h) {
+  const long long size = h->pool.size;
+  if (size > 0) {
+    tsb::nq_fat_import_kernel<N><<<static_cast<unsigned>((size + 255) / 256), 256, 0, h->stream>>>(
+        h->pool.arena[h->pool.cur], h->d_fat, size, h->rounds.epoch);
+    TSB_CUDA(cudaGetLastError());
+    h->launches++;
   }
-  (void)cudaGetLastError();
+  return TSB_OK;
 }
-}  // namespace
+int nq_ensure_fat(tsb_nq* h, long long cap) {
+  if (cap <= h->fat_cap) return TSB_OK;
+  if (h->d_fat) cudaFree(h->d_fat);
+  h->d_fat = nullptr;
+  h->fat_cap = 0;
+  TSB_CUDA(cudaMalloc(&h->d_fat, static_cast<size_t>(cap) * sizeof(tsb::FatNode)));
+  h->fat_cap = cap;
+  return TSB_OK;
+}
+// the pool back in the plain 21-byte arena (whoever needs the node records calls this first)
+int nq_materialize(tsb_nq* h) {
+  if (!h->in_fat) return TSB_OK;
+  TSB_CUDA(cudaSetDevice(h->device));
+  const long long size = h->pool.size;
+  if (size > 0) {
+    tsb::nq_fat_export_kernel<<<static_cast<unsigned>((size + 255) / 256), 256, 0, h->stream>>>(
+        h->d_fat, h->pool.arena[h->pool.cur], size);
+    TSB_CUDA(cudaGetLastError());
+    h->launches++;
+    TSB_CUDA(cudaStreamSynchronize(h->stream));
+  }
+  h->in_fat = false;
+  return TSB_OK;
+}
+// grid (CTAs per pool) of the persistent kernel for chunks of up to M parents when one launch serves `pools` pools;
+// 0: M is too large for it.  Chosen on the N = 17 search at M = 50000: one pool: 7/8 of the SMs
+// (one CTA per SM); two pools: one CTA per SM each (two per SM in all); four pools: SMs / 2 CTAs each.  An all-to-all
+// flag exchange among all SMs' CTAs costs 2-3x one among half of them (tools/flag_exchange.py); the per-CTA work grows
+// the other way.
+// *ppt: parents per thread of the kernel variant to launch (2, or 3 when the pool's CTAs would not cover M with 2).
+int nq_ll_grid(const tsb_nq* h, int M, int pools, int* ppt = nullptr) {
+  if (!h->di.coop || env_no_rounds() || pools < 1 || pools > tsb::LL_MAX_POOLS) return 0;
+  const int sms = std::min(h->di.sms, tsb::LL_MAX_SMS);
+  const int most = tsb::ll_ctas_per_pool(sms, pools);  // (ll_tiers.h: the drivers size their warm-up by the same tiers)
+  const int per = static_cast<long long>(most) * tsb::ll_slice(2) >= M ? 2 : 3;
+  const int slice = tsb::ll_slice(per);
+  int grid = pools == 1 ? std::max(1, (sms * 7 / 8) & ~1) : most;
+  while (static_cast<long long>(grid) * slice < M && grid < most) ++grid;  // (M decides)
+  if (ppt) *ppt = per;
+  return static_cast<long long>(M) <= static_cast<long long>(grid) * slice && (pools > 1 || per == 2) ? grid : 0;
+}
+// Up to `max_rounds` rounds of EACH of the K pools (handles on one device, same N) in launches of the persistent
+// kernel that serve all pools that still have work: grid (grid, pools).  out[4 i ..] += {rounds, parents, children,
+// solutions} of pool i.  A pool leaves the launch on its own (done, round budget, arena full, layer table full); the
+// launch ends when every pool has left, the pools that stopped for room grow and go again.
+int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, uint64_t* out) {
+  int64_t left[tsb::LL_MAX_POOLS];
+  bool active[tsb::LL_MAX_POOLS];
+  for (int i = 0; i < K; i++) {
+    left[i] = max_rounds;
+    active[i] = true;
+    int rc = hs[i]->rounds.ensure<tsb::LlSync>(hs[i]->stream);
+    if (rc != TSB_OK) return rc;
+  }
+  const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
+  for (;;) {
+    tsb::LlMultiParams mp;
+    std::memset(&mp, 0, sizeof(mp));
+    int map[tsb::LL_MAX_POOLS], n_act = 0;
+    long long need_of[tsb::LL_MAX_POOLS];
+    for (int i = 0; i < K; i++) {
+      tsb_nq* h = hs[i];
+      DevicePool& p = h->pool;
+      if (!active[i] || p.size < m || left[i] <= 0) {
+        active[i] = false;
+        continue;
+      }
+      const long long n = std::min<long long>(p.size, M);
+      const long long need = p.size - n + n * h->N;
+      int rc = TSB_OK;
+      if (h->in_fat && need > p.cap) rc = nq_materialize(h);  // (grows below and imports again)
+      if (rc != TSB_OK) return rc;
+      if (!h->in_fat) {
+        // room for the worst case of the next round
+        rc = p.make_stack(h->stream, need);
+        if (rc == TSB_OK) rc = nq_ensure_fat(h, p.cap);
+        if (rc == TSB_OK) rc = with_queens(h->N, [h](auto q) { return nq_fat_import<decltype(q)::value>(h); });
+        if (rc != TSB_OK) return rc;
+        h->in_fat = true;
+        if (n_act > 0) TSB_CUDA(cudaStreamSynchronize(h->stream));  // (the launch goes on the first pool's stream)
+      }
+      tsb::LlParams& prm = mp.pool[n_act];
+      prm.fat = h->d_fat;
+      prm.cap = std::min(p.cap, h->fat_cap);
+      prm.size0 = p.size;
+      prm.epoch0 = h->rounds.epoch;
+      prm.m = m;
+      prm.M = M;
+      prm.max_rounds = left[i];
+      prm.prof = prof;
+      prm.sync = h->rounds.sync<tsb::LlSync>();
+      prm.state = h->rounds.d_state;
+      h->rounds.h_state->exit_code = -1;
+      need_of[n_act] = need;
+      map[n_act++] = i;
+    }
+    if (n_act == 0) break;
+    tsb_nq* h0 = hs[map[0]];
+    // (variant and grid follow the number of pools that still run: a lone survivor gets the one-pool kernel)
+    int ppt = 2;
+    const int grid = nq_ll_grid(h0, M, n_act, &ppt);
+    if (grid == 0) return TSB_EINVAL;  // (checked by the callers for K pools, and fewer pools fit a fortiori)
+    int rc = with_queens(h0->N, [&](auto q) {
+      return nq_ll_launch_n<decltype(q)::value>(h0, mp, grid, n_act, ppt, h0->stream);
+    });
+    if (rc != TSB_OK) return rc;
+    TSB_CUDA(cudaStreamSynchronize(h0->stream));
+    for (int a = 0; a < n_act; a++) {
+      const int i = map[a];
+      tsb_nq* h = hs[i];
+      tsb::RoundsState st;
+      rc = h->finish_launch("nq_rounds_ll_kernel", "a flag exchange or a node poll did not complete", &st, &out[4 * i]);
+      if (rc != TSB_OK) return rc;
+      if (prof) {
+        const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
+        std::fprintf(stderr, "[tsb200] LL rounds kernel (pool %d of %d): %llu rounds; CTA 0 cycles per round: workers: set-up %.0f "
+                     "poll-nodes %.0f scan+items+diag %.0f build %.0f handoff-wait %.0f store %.0f | exchange warp: "
+                     "scan-wait %.0f publish+gather %.0f bookkeeping %.0f handoff-wait %.0f\n", a, n_act,
+                     static_cast<unsigned long long>(st.rounds), st.prof[tsb::LL_PROF_SETUP] / r, st.prof[tsb::LL_PROF_POLL] / r,
+                     st.prof[tsb::LL_PROF_SCAN] / r, st.prof[tsb::LL_PROF_BUILD] / r, st.prof[tsb::LL_PROF_HAND] / r,
+                     st.prof[tsb::LL_PROF_STORE] / r, st.prof[tsb::LL_PROF_X_SCAN] / r, st.prof[tsb::LL_PROF_X_GATHER] / r,
+                     st.prof[tsb::LL_PROF_X_BOOK] / r, st.prof[tsb::LL_PROF_X_HAND] / r);
+      }
+      left[i] -= static_cast<int64_t>(st.rounds);
+      if (st.exit_code == tsb::RND_EXIT_SPACE) {
+        if (st.rounds == 0 && need_of[a] <= h->pool.cap) return TSB_ENOMEM;  // (cannot happen)
+        rc = nq_materialize(h);  // back to the plain arena, which then grows
+        if (rc != TSB_OK) return rc;
+      } else if (st.exit_code != tsb::RND_EXIT_RELAUNCH) {  // (layer table full: a fresh launch trusts the whole pool)
+        active[i] = false;                                    // DONE or PAUSE
+      }
+    }
+  }
+  return TSB_OK;
+}
 
 // ============================================================================ PFSP
-struct tsb_pfsp : Base {
-  int jobs = 0, machines = 0, pairs = 0, mt = 0;  // mt = template machine count (5, 10 or 20)
-  tsb::PfspLb1Tables* d_tab1 = nullptr;
-  tsb::Lb2Const* lb2c = nullptr;  // packed Johnson tables, passed to the lb2 kernels by value (constant bank)
-  tsb::Lb2ConstU* lb2u = nullptr; // <= 10 machines: address of the shared-memory-resident table (tsb::Lb2TabU)
-  tsb::Lb2TabU* d_tabu = nullptr;
-  bool attr_set[3] = {false, false, false};
-  int occ[3] = {0, 0, 0};
-  bool simd16 = false;  // lb1 / lb1_d children two per register (values < 2^16, min_tails non-increasing)
-  bool wide = false;    // MAX_JOBS = 50 build: 208-byte nodes, the general kernels of pfsp_wide.cuh
-  tsb::PfspWideTables* d_wtab = nullptr;
-  bool wide_attr[3] = {false, false, false};
-  int wide_occ[3] = {0, 0, 0};
-  // fused expand + device-resident pool
-  ExpandCtx ex;
-  bool ex_attr[4] = {false, false, false, false};  // count lb1_d, lb1, lb2; build
-  int ex_occ[4] = {0, 0, 0, 0};
-  uint8_t* d_children = nullptr;
-  size_t d_children_bytes = 0;
-  DevicePool pool;
-  uint64_t slow_rounds = 0;
-  std::vector<tsb_pfsp_node> h_chunk, h_kids;  // slow path scratch
-  std::vector<int32_t> h_bounds;
-  // the persistent multi-round kernel (pfsp_rounds.cuh)
-  tsb::RoundsState* rnd_h = nullptr;  // pinned + mapped: written by the kernel when it leaves
-  tsb::RoundsState* rnd_d = nullptr;  // device alias of rnd_h
-  tsb::PfRoundsSync* rnd_sync = nullptr;
-  unsigned rnd_epoch = 0;
-  bool rnd_attr[2] = {false, false};  // lb1_d, lb1
-};
-
-namespace {
-
 template <int KIND, int M, bool SIMD>
 int launch_lb1_km(tsb_pfsp* h, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
   auto kernel = tsb::pfsp_lb1_kernel<KIND, M, SIMD>;
   const size_t smem = sizeof(tsb::Lb1Smem) + 128;
-  if (!h->attr_set[KIND]) {
-    TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    h->attr_set[KIND] = true;
-  }
   int grid = 1;
-  int rc = grid_for(kernel, tsb::PF_THREADS, smem, count, tsb::PF_TILE, h->di.sms, &grid, &h->occ[KIND]);
+  int rc = h->grid_for(kernel, tsb::PF_THREADS, smem, count, tsb::PF_TILE, &grid);
   if (rc != TSB_OK) return rc;
   kernel<<<grid, tsb::PF_THREADS, smem, s>>>(in, out, count, h->d_tab1);
   TSB_CUDA(cudaGetLastError());
@@ -799,12 +1132,8 @@ template <int M, typename CT>
 int launch_lb2_mc(tsb_pfsp* h, const CT& C, const uint8_t* in, uint8_t* out, long long count, int best, cudaStream_t s) {
   auto kernel = tsb::pfsp_lb2_kernel<M, CT>;
   const size_t smem = sizeof(tsb::Lb2Smem<M>) + 128;
-  if (!h->attr_set[2]) {
-    TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    h->attr_set[2] = true;
-  }
   int grid = 1;
-  int rc = grid_for(kernel, tsb::PF_THREADS, smem, count, tsb::LB2_TILE, h->di.sms, &grid, &h->occ[2]);
+  int rc = h->grid_for(kernel, tsb::PF_THREADS, smem, count, tsb::LB2_TILE, &grid);
   if (rc != TSB_OK) return rc;
   kernel<<<grid, tsb::PF_THREADS, smem, s>>>(in, out, count, h->d_tab1, C, best);
   TSB_CUDA(cudaGetLastError());
@@ -823,12 +1152,8 @@ template <int KIND, int M>
 int launch_wide_km(tsb_pfsp* h, const uint8_t* in, uint8_t* out, long long count, int best, cudaStream_t s) {
   auto kernel = tsb::pfsp_wide_kernel<KIND, M>;
   const size_t smem = sizeof(tsb::PfspWideSmem) + 128;
-  if (!h->wide_attr[KIND]) {
-    TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    h->wide_attr[KIND] = true;
-  }
   int grid = 1;
-  int rc = grid_for(kernel, tsb::PW_THREADS, smem, count + tsb::PW_TILE - 1, tsb::PW_TILE, h->di.sms, &grid, &h->wide_occ[KIND]);
+  int rc = h->grid_for(kernel, tsb::PW_THREADS, smem, count + tsb::PW_TILE - 1, tsb::PW_TILE, &grid);
   if (rc != TSB_OK) return rc;
   kernel<<<grid, tsb::PW_THREADS, smem, s>>>(in, reinterpret_cast<int32_t*>(out), count, h->d_wtab, best);
   TSB_CUDA(cudaGetLastError());
@@ -844,31 +1169,16 @@ int launch_wide_m(tsb_pfsp* h, int lb_kind, const uint8_t* in, uint8_t* out, lon
 
 int launch_pfsp(tsb_pfsp* h, int lb_kind, const uint8_t* in, uint8_t* out, long long count, int64_t best64,
                 cudaStream_t s) {
-  // bounds are int32 and `lb > best` can never hold for best >= INT32_MAX (Chapel's max(int) under --ub 0)
-  const int best = best64 > INT_MAX ? INT_MAX : best64 < INT_MIN ? INT_MIN : static_cast<int>(best64);
-  if (h->wide) {
-    if (h->mt == 5) return launch_wide_m<5>(h, lb_kind, in, out, count, best, s);
-    if (h->mt == 10) return launch_wide_m<10>(h, lb_kind, in, out, count, best, s);
-    return launch_wide_m<20>(h, lb_kind, in, out, count, best, s);
-  }
-#define TSB_PF_DISPATCH(M)                                                                                      \
-  if (lb_kind == TSB_LB1)                                                                                        \
-    return h->simd16 ? launch_lb1_km<1, M, true>(h, in, out, count, s) : launch_lb1_km<1, M, false>(h, in, out, count, s); \
-  if (lb_kind == TSB_LB1_D)                                                                                      \
-    return h->simd16 ? launch_lb1_km<0, M, true>(h, in, out, count, s) : launch_lb1_km<0, M, false>(h, in, out, count, s); \
-  return launch_lb2_m<M>(h, in, out, count, best, s);
-  if (h->mt == 5) { TSB_PF_DISPATCH(5) }
-  if (h->mt == 10) { TSB_PF_DISPATCH(10) }
-  TSB_PF_DISPATCH(20)
-#undef TSB_PF_DISPATCH
-}
-
-}  // namespace
-
-namespace {
-
-inline int clamp_best(int64_t best64) {
-  return best64 > INT_MAX ? INT_MAX : best64 < INT_MIN ? INT_MIN : static_cast<int>(best64);
+  const int best = clamp_best(best64);
+  return with_machines(h->mt, [&](auto mt) {
+    constexpr int M = decltype(mt)::value;
+    if (h->wide) return launch_wide_m<M>(h, lb_kind, in, out, count, best, s);
+    if (lb_kind == TSB_LB1)
+      return h->simd16 ? launch_lb1_km<1, M, true>(h, in, out, count, s) : launch_lb1_km<1, M, false>(h, in, out, count, s);
+    if (lb_kind == TSB_LB1_D)
+      return h->simd16 ? launch_lb1_km<0, M, true>(h, in, out, count, s) : launch_lb1_km<0, M, false>(h, in, out, count, s);
+    return launch_lb2_m<M>(h, in, out, count, best, s);
+  });
 }
 
 template <int M>
@@ -878,12 +1188,8 @@ int pfsp_expand_m(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const tsb::Exp
   const long long recs = static_cast<long long>(prm.n_tiles) * tsb::PF_TILE;
   auto k3 = tsb::pfsp_expand_build_kernel;
   const size_t smem3 = sizeof(tsb::PfBuildSmem) + 128;
-  if (!h->ex_attr[3]) {
-    TSB_CUDA(cudaFuncSetAttribute(k3, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem3)));
-    h->ex_attr[3] = true;
-  }
   int g1 = 1, g3 = 1;
-  int rc = grid_for(k3, tsb::PF_THREADS, smem3, recs, tsb::PF_TILE, h->di.sms, &g3, &h->ex_occ[3]);
+  int rc = h->grid_for(k3, tsb::PF_THREADS, smem3, recs, tsb::PF_TILE, &g3);
   if (rc != TSB_OK) return rc;
   if ((prm.n_tiles + g3 - 1) / g3 > tsb::EXP_MAX_OWN) return TSB_EINVAL;
   if (lb_kind == TSB_LB2) {
@@ -891,11 +1197,7 @@ int pfsp_expand_m(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const tsb::Exp
     // (this kernel walks the round in half tiles and accumulates the tile counts)
     TSB_CUDA(cudaMemsetAsync(ex.d_tile, 0, static_cast<size_t>(prm.n_tiles) * sizeof(int), s));
     auto go = [&](auto k1, const auto& C) -> int {
-      if (!h->ex_attr[2]) {
-        TSB_CUDA(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem1)));
-        h->ex_attr[2] = true;
-      }
-      int r2 = grid_for(k1, tsb::PF_THREADS, smem1, recs, tsb::LB2_TILE, h->di.sms, &g1, &h->ex_occ[2]);
+      int r2 = h->grid_for(k1, tsb::PF_THREADS, smem1, recs, tsb::LB2_TILE, &g1);
       if (r2 != TSB_OK) return r2;
       k1<<<g1, tsb::PF_THREADS, smem1, s>>>(arena, prm, h->d_tab1, C, ex.d_cmask, ex.d_tile, ex.d_st);
       return TSB_OK;
@@ -909,24 +1211,12 @@ int pfsp_expand_m(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const tsb::Exp
     }
     if (!done) rc = go(tsb::pfsp_expand_count_lb2_kernel<M, tsb::Lb2Const>, *h->lb2c);
     if (rc != TSB_OK) return rc;
-  } else if (lb_kind == TSB_LB1) {
-    auto k1 = h->simd16 ? tsb::pfsp_expand_count_lb1_kernel<1, M, true> : tsb::pfsp_expand_count_lb1_kernel<1, M, false>;
-    const size_t smem1 = sizeof(tsb::Lb1CountSmem) + 128;
-    if (!h->ex_attr[1]) {
-      TSB_CUDA(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem1)));
-      h->ex_attr[1] = true;
-    }
-    rc = grid_for(k1, tsb::PF_THREADS, smem1, recs, tsb::PF_TILE, h->di.sms, &g1, &h->ex_occ[1]);
-    if (rc != TSB_OK) return rc;
-    k1<<<g1, tsb::PF_THREADS, smem1, s>>>(arena, prm, h->d_tab1, ex.d_cmask, ex.d_tile, ex.d_st);
   } else {
-    auto k1 = h->simd16 ? tsb::pfsp_expand_count_lb1_kernel<0, M, true> : tsb::pfsp_expand_count_lb1_kernel<0, M, false>;
+    auto k1 = lb_kind == TSB_LB1
+                  ? (h->simd16 ? tsb::pfsp_expand_count_lb1_kernel<1, M, true> : tsb::pfsp_expand_count_lb1_kernel<1, M, false>)
+                  : (h->simd16 ? tsb::pfsp_expand_count_lb1_kernel<0, M, true> : tsb::pfsp_expand_count_lb1_kernel<0, M, false>);
     const size_t smem1 = sizeof(tsb::Lb1CountSmem) + 128;
-    if (!h->ex_attr[0]) {
-      TSB_CUDA(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem1)));
-      h->ex_attr[0] = true;
-    }
-    rc = grid_for(k1, tsb::PF_THREADS, smem1, recs, tsb::PF_TILE, h->di.sms, &g1, &h->ex_occ[0]);
+    rc = h->grid_for(k1, tsb::PF_THREADS, smem1, recs, tsb::PF_TILE, &g1);
     if (rc != TSB_OK) return rc;
     k1<<<g1, tsb::PF_THREADS, smem1, s>>>(arena, prm, h->d_tab1, ex.d_cmask, ex.d_tile, ex.d_st);
   }
@@ -972,12 +1262,9 @@ int pfsp_expand_round(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const std:
   if (rc != TSB_OK) return rc;
   prm.epoch = ++ex.epoch;
   prm.best = best_launch;
-  if (h->mt == 5)
-    rc = pfsp_expand_m<5>(h, lb_kind, arena, prm, children_d, s);
-  else if (h->mt == 10)
-    rc = pfsp_expand_m<10>(h, lb_kind, arena, prm, children_d, s);
-  else
-    rc = pfsp_expand_m<20>(h, lb_kind, arena, prm, children_d, s);
+  rc = with_machines(h->mt, [&](auto mt) {
+    return pfsp_expand_m<decltype(mt)::value>(h, lb_kind, arena, prm, children_d, s);
+  });
   if (rc != TSB_OK) return rc;
   rc = ex.wait_result(prm.epoch, s, early);
   if (rc != TSB_OK) {
@@ -1020,13 +1307,98 @@ int pfsp_expand_round(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const std:
   return TSB_OK;
 }
 
-long long pfsp_pool_min_cap(const tsb_pfsp* h) {
-  if (const long long c = env_pool_cap(); c > 0) return c;
-  return std::max<long long>(1LL << 20, 4LL * h->M_max * h->jobs);
+// (the PFSP pool only ever lives in its plain arena)
+int pfsp_plain() { return TSB_OK; }
+
+// CTAs of the persistent PFSP kernel for chunks of up to M parents (one per SM at most, each with up to PFR_SLICE
+// parents; fewer CTAs for smaller M, so that the two exchanges of a round involve only the CTAs that have parents to
+// evaluate); 0: the loop of tsb_pfsp_pool_step runs instead (lb2, M above PFR_MAX_M where the step loop is faster, M
+// beyond pf_rounds_capacity, no cooperative launch, env TSB200_NO_ROUNDS=1)
+int pfsp_rounds_grid(const tsb_pfsp* h, int lb_kind, int M) {
+  if (lb_kind == TSB_LB2 || !h->di.coop || env_no_rounds()) return 0;
+  if (M > tsb::PFR_MAX_M || M > tsb::pf_rounds_capacity(h->di.sms)) return 0;
+  const int sms = std::min(h->di.sms, tsb::PFR_MAX_CTAS);
+  return static_cast<int>(std::min<long long>(sms, (static_cast<long long>(M) + tsb::PF_TILE - 1) / tsb::PF_TILE));
 }
-void pfsp_pool_setup(tsb_pfsp* h) {
-  h->pool.rec = sizeof(tsb_pfsp_node);
-  h->pool.slack = static_cast<size_t>(tsb::PF_TILE) * sizeof(tsb_pfsp_node);
+template <int KIND, int M>
+int pfsp_rounds_launch_km(tsb_pfsp* h, const tsb::PfRoundsParams& prm, int grid, cudaStream_t s) {
+  auto kernel = h->simd16 ? tsb::pfsp_rounds_kernel<KIND, M, true> : tsb::pfsp_rounds_kernel<KIND, M, false>;
+  const size_t smem = sizeof(tsb::PfRoundsSmem) + 128;
+  int rc = h->configure(kernel, smem);
+  if (rc != TSB_OK) return rc;
+  void* args[] = {const_cast<tsb::PfRoundsParams*>(&prm)};
+  // cooperative: every CTA co-resident (the exchanges wait for all of them), or the launch fails
+  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid), dim3(tsb::PF_THREADS), args, smem, s));
+  h->launches++;
+  return TSB_OK;
+}
+// Up to max_rounds rounds in launches of the persistent kernel; out[] += {rounds, parents, children, solutions}.  A
+// launch leaves when the pool holds fewer than m nodes, after its round budget, when the next round's worst case
+// does not fit the arena (it grows and the loop relaunches) or when a leaf of the chunk improves *best (that round
+// goes through tsb_pfsp_pool_step and its sequential rule, then the loop relaunches with the new incumbent).
+int pfsp_rounds_run(tsb_pfsp* h, int lb_kind, int m, int M, int grid, int64_t max_rounds, int64_t* best, uint64_t* out) {
+  DevicePool& p = h->pool;
+  int rc = h->rounds.ensure<tsb::PfRoundsSync>(h->stream);
+  if (rc != TSB_OK) return rc;
+  const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
+  int64_t left = max_rounds;
+  while (left > 0 && p.size >= m) {
+    // room for the worst case of the next round
+    const long long n = std::min<long long>(p.size, M);
+    const long long need = p.size - n + n * h->jobs;
+    rc = p.make_stack(h->stream, need);
+    if (rc != TSB_OK) return rc;
+    tsb::PfRoundsParams prm;
+    std::memset(&prm, 0, sizeof(prm));
+    prm.arena = p.arena[p.cur];
+    prm.tables = h->d_tab1;
+    prm.cap = p.cap;
+    prm.size0 = p.size;
+    prm.max_rounds = left;
+    prm.epoch0 = h->rounds.epoch;
+    prm.m = m;
+    prm.M = M;
+    prm.best = clamp_best(*best);
+    prm.prof = prof;
+    prm.sync = h->rounds.sync<tsb::PfRoundsSync>();
+    prm.state = h->rounds.d_state;
+    h->rounds.h_state->exit_code = -1;
+    rc = with_machines(h->mt, [&](auto mt) {
+      constexpr int MT = decltype(mt)::value;
+      return lb_kind == TSB_LB1 ? pfsp_rounds_launch_km<1, MT>(h, prm, grid, h->stream)
+                                : pfsp_rounds_launch_km<0, MT>(h, prm, grid, h->stream);
+    });
+    if (rc != TSB_OK) return rc;
+    TSB_CUDA(cudaStreamSynchronize(h->stream));
+    tsb::RoundsState st;
+    rc = h->finish_launch("pfsp_rounds_kernel", "a count or store exchange did not complete", &st, out);
+    if (rc != TSB_OK) return rc;
+    if (prof) {
+      const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
+      std::fprintf(stderr, "[tsb200] PFSP rounds kernel: %llu rounds (exit %d); CTA 0 cycles per round: load %.0f bounds %.0f "
+                   "publish+items %.0f gather %.0f store %.0f store-exchange %.0f\n",
+                   static_cast<unsigned long long>(st.rounds), st.exit_code, st.prof[tsb::PFR_PROF_LOAD] / r,
+                   st.prof[tsb::PFR_PROF_BOUND] / r, st.prof[tsb::PFR_PROF_PUBLISH] / r, st.prof[tsb::PFR_PROF_GATHER] / r,
+                   st.prof[tsb::PFR_PROF_STORE] / r, st.prof[tsb::PFR_PROF_BARRIER] / r);
+    }
+    left -= static_cast<int64_t>(st.rounds);
+    if (st.exit_code == tsb::RND_EXIT_SPACE) {
+      if (st.rounds == 0 && need <= p.cap) return TSB_ENOMEM;  // (cannot happen: the arena was grown for `need`)
+    } else if (st.exit_code == tsb::PFR_EXIT_IMPROVED) {
+      int64_t np = 0;
+      uint64_t nc = 0, ns = 0;
+      rc = tsb_pfsp_pool_step(h, lb_kind, m, M, best, &np, &nc, &ns);
+      if (rc != TSB_OK) return rc;
+      out[0] += 1;
+      out[1] += static_cast<uint64_t>(np);
+      out[2] += nc;
+      out[3] += ns;
+      --left;
+    } else {
+      break;  // DONE or PAUSE
+    }
+  }
+  return TSB_OK;
 }
 
 }  // namespace
@@ -1143,6 +1515,43 @@ int tsb_init_devices(int n) {
   return TSB_OK;
 }
 
+// diagnostics: cycles per round of bare flag exchanges among co-resident CTAs (rounds_sync_bench_kernel, nq_rounds_ll.cuh)
+int tsb_debug_flag_exchange(int device, int rounds, int variant, int ctas, double* cycles_per_round) {
+  if (!cycles_per_round || rounds < 1) return TSB_EINVAL;
+  DeviceInfo di;
+  int rc = query_device(device, di);
+  if (rc != TSB_OK) return rc;
+  if (!di.coop) return TSB_EUNSUPPORTED;
+  tsb::RoundsSync* sy = nullptr;
+  uint4* scratch = nullptr;
+  long long* d_out = nullptr;
+  int grid = std::min(di.sms, tsb::LL_MAX_SMS);
+  if (ctas > 0 && ctas < grid) grid = ctas;
+  TSB_CUDA(cudaMalloc(&sy, sizeof(*sy)));
+  const size_t scratch_bytes = std::max<size_t>((static_cast<size_t>(grid) * tsb::LL_T + 2) * sizeof(uint4), 2 * 256 * 256 * 4);
+  TSB_CUDA(cudaMalloc(&scratch, scratch_bytes));
+  TSB_CUDA(cudaMemset(scratch, 0, scratch_bytes));
+  TSB_CUDA(cudaMalloc(&d_out, sizeof(long long)));
+  TSB_CUDA(cudaMemset(sy, 0, sizeof(*sy)));
+  unsigned epoch0 = 0;
+  void* args[] = {&sy, &epoch0, &rounds, &variant, &scratch, &d_out};
+  cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(tsb::rounds_sync_bench_kernel), dim3(grid),
+                                              dim3(tsb::LL_T), args, 0, nullptr);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  long long cyc = 0;
+  if (e == cudaSuccess) e = cudaMemcpy(&cyc, d_out, sizeof(cyc), cudaMemcpyDeviceToHost);
+  cudaFree(sy);
+  cudaFree(scratch);
+  cudaFree(d_out);
+  if (e != cudaSuccess) {
+    g_last_cuda_error = std::string("flag exchange bench: ") + cudaGetErrorString(e);
+    (void)cudaGetLastError();
+    return TSB_ECUDA;
+  }
+  *cycles_per_round = static_cast<double>(cyc) / rounds;
+  return TSB_OK;
+}
+
 // ---------------------------------------------------------------- N-Queens
 int tsb_nq_create(tsb_nq** out, int device, int N, int g, int M_max) {
   if (!out || N < 1 || N > TSB_MAX_QUEENS || g < 1 || M_max < 1) return TSB_EINVAL;
@@ -1151,6 +1560,8 @@ int tsb_nq_create(tsb_nq** out, int device, int N, int g, int M_max) {
   h->N = N;
   h->g = g;
   if (const char* v = std::getenv("TSB200_NQ_TILE_THREADS")) h->tile_threads = std::atoi(v);
+  // (the arena starts with room for four worst-case rounds: every slot of every parent survives)
+  h->pool.set_format(sizeof(tsb_nq_node), tsb::NQ_TILE, 1, N, std::max<long long>(1LL << 22, 4LL * M_max * N));
   int rc = h->init(device, M_max, sizeof(tsb_nq_node), static_cast<size_t>(N));
   if (rc != TSB_OK) {
     h->fini();
@@ -1167,13 +1578,8 @@ void tsb_nq_destroy(tsb_nq* h) {
     if (x) tsb_nq_destroy(x);
     x = nullptr;
   }
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  h->ex.release();
-  h->rounds.release();
-  if (h->d_children) cudaFree(h->d_children);
-  h->pool.release();
   h->fini();
+  if (h->d_fat) cudaFree(h->d_fat);
   delete h;
 }
 
@@ -1188,8 +1594,8 @@ int tsb_nq_expand_device(tsb_nq* h, const void* parents_d, int count, void* chil
   TSB_CUDA(cudaSetDevice(h->device));
   unsigned long long nc = 0, ns = 0;
   const std::vector<PoolExtent> pieces{{0, count}};
-  int rc = nq_expand_dispatch(h, static_cast<const uint8_t*>(parents_d), pieces, static_cast<uint8_t*>(children_d),
-                              stream ? static_cast<cudaStream_t>(stream) : h->stream, &nc, &ns);
+  int rc = nq_expand(h, static_cast<const uint8_t*>(parents_d), pieces, static_cast<uint8_t*>(children_d),
+                     stream ? static_cast<cudaStream_t>(stream) : h->stream, &nc, &ns);
   *n_children = nc;
   *n_solutions = ns;
   return rc;
@@ -1201,315 +1607,27 @@ int tsb_nq_expand(tsb_nq* h, const void* parents, int count, void* children, uin
   *n_children = *n_solutions = 0;
   if (count == 0) return TSB_OK;
   if (!parents || !children) return TSB_EINVAL;
-  TSB_CUDA(cudaSetDevice(h->device));
-  const size_t need = static_cast<size_t>(h->M_max) * h->N * sizeof(tsb_nq_node) + 64;
-  if (h->d_children_bytes < need) {
-    if (h->d_children) cudaFree(h->d_children);
-    h->d_children = nullptr;
-    h->d_children_bytes = 0;
-    TSB_CUDA(cudaMalloc(&h->d_children, need));
-    h->d_children_bytes = need;
-  }
-  int rc = h->copy_h2d(h->d_in, parents, sizeof(tsb_nq_node) * static_cast<size_t>(count), h->stream);
-  if (rc != TSB_OK) return rc;
-  unsigned long long nc = 0, ns = 0;
-  const std::vector<PoolExtent> pieces{{0, count}};
-  rc = nq_expand_dispatch(h, h->d_in, pieces, h->d_children, h->stream, &nc, &ns);
-  if (rc != TSB_OK) return rc;
-  *n_children = nc;
-  *n_solutions = ns;
-  if (nc > capacity) return TSB_ENOMEM;  // the caller's children array is too small; counts are valid
-  return h->copy_d2h(children, h->d_children, nc * sizeof(tsb_nq_node), h->stream);
+  return expand_host(*h, parents, count, children, capacity, n_children, n_solutions,
+                     [h](auto arena, const auto& pieces, auto kids, auto nc, auto ns) {
+                       return nq_expand(h, arena, pieces, kids, h->stream, nc, ns);
+                     });
 }
-
-}  // extern "C"
-namespace {
-// arena capacity a handle starts with: four worst-case rounds (every slot of every parent survives)
-long long nq_pool_min_cap(const tsb_nq* h) {
-  if (const long long c = env_pool_cap(); c > 0) return c;
-  return std::max<long long>(1LL << 22, 4LL * h->M_max * h->N);
-}
-void nq_pool_setup(tsb_nq* h) {
-  h->pool.rec = sizeof(tsb_nq_node);
-  h->pool.slack = static_cast<size_t>(tsb::NQ_TILE) * sizeof(tsb_nq_node);  // full-tile loads may run past the top
-}
-// what a pool may hold: depth <= N, board[0..N) < N, the bytes past N zero (every node the reference or this library
-// creates; the persistent kernel packs a node into 125 bits on these terms, nq_rounds_ll.cuh)
-bool nq_nodes_valid(int N, const tsb_nq_node* nodes, int64_t n) {
-  for (int64_t i = 0; i < n; i++) {
-    const tsb_nq_node& x = nodes[i];
-    if (x.depth > N) return false;
-    for (int j = 0; j < TSB_MAX_QUEENS; j++)
-      if (x.board[j] >= (j < N ? N : 1)) return false;
-  }
-  return true;
-}
-}  // namespace
-extern "C" {
 
 int tsb_nq_pool_push(tsb_nq* h, const void* nodes, int64_t n) {
   if (!h || n < 0 || (n && !nodes)) return TSB_EINVAL;
   if (!nq_nodes_valid(h->N, static_cast<const tsb_nq_node*>(nodes), n)) return TSB_EINVAL;
-  TSB_CUDA(cudaSetDevice(h->device));
-  nq_pool_setup(h);
-  int rc = nq_materialize(h);
-  if (rc != TSB_OK) return rc;
-  rc = h->pool.reserve(h->stream, n, nq_pool_min_cap(h));
-  if (rc != TSB_OK) return rc;
-  if (n == 0) return TSB_OK;
-  const long long at = h->pool.top();
-  // (on the handle's non-blocking stream, which the kernels of the next round are ordered after)
-  rc = h->copy_h2d(h->pool.arena[h->pool.cur] + at * sizeof(tsb_nq_node), nodes,
-                   static_cast<size_t>(n) * sizeof(tsb_nq_node), h->stream);
-  if (rc != TSB_OK) return rc;
-  if (h->pool.ext.empty())
-    h->pool.ext.push_back({at, at + n});
-  else
-    h->pool.ext.back().e += n;
-  h->pool.size += n;
-  return TSB_OK;
+  return pool_push(*h, nodes, n, [h] { return nq_materialize(h); });
 }
 
 int64_t tsb_nq_pool_size(const tsb_nq* h) { return h ? h->pool.size : -1; }
 
 int tsb_nq_pool_step(tsb_nq* h, int m, int M, int64_t* n_parents, uint64_t* n_children, uint64_t* n_solutions) {
   if (!h || m < 1 || M < 1 || M > h->M_max || !n_parents || !n_children || !n_solutions) return TSB_EINVAL;
-  *n_parents = 0;
-  *n_children = *n_solutions = 0;
-  DevicePool& p = h->pool;
-  if (p.size < m) return TSB_OK;  // popBackBulk returns 0 below m (lib/commons/Pool.chpl:50-59)
-  TSB_CUDA(cudaSetDevice(h->device));
-  int rc = nq_materialize(h);
-  if (rc != TSB_OK) return rc;
-  const long long n = std::min<long long>(p.size, M);
-  // room above the top for the worst case (every slot of every parent survives); the chunk itself is read
-  // in place, as the newest pieces of the extent stack
-  std::vector<PoolExtent> pieces;
-  pool_top_pieces(p, n, &pieces);
-  if (pieces.size() > tsb::EXP_MAX_PIECES)
-    rc = p.compact(h->stream, p.cap);
-  if (rc == TSB_OK) rc = p.reserve(h->stream, n * h->N, nq_pool_min_cap(h));
-  if (rc != TSB_OK) return rc;
-  pool_top_pieces(p, n, &pieces);  // (positions change when the pool was compacted)
-  const long long top = p.top();
-  unsigned long long nc = 0, ns = 0;
-  uint8_t* arena = p.arena[p.cur];
-  rc = nq_expand_dispatch(h, arena, pieces, arena + top * sizeof(tsb_nq_node), h->stream, &nc, &ns, /*early=*/true);
-  if (rc != TSB_OK) return rc;
-  pool_pop(p, n);
-  if (nc) {
-    p.ext.push_back({top, top + static_cast<long long>(nc)});
-    p.size += static_cast<long long>(nc);
-  }
-  *n_parents = n;
-  *n_children = nc;
-  *n_solutions = ns;
-  return TSB_OK;
+  return pool_step(*h, m, M, n_parents, n_children, n_solutions, [h] { return nq_materialize(h); },
+                   [h](auto arena, const auto& pieces, auto kids, auto nc, auto ns) {
+                     return nq_expand(h, arena, pieces, kids, h->stream, nc, ns, /*early=*/true);
+                   });
 }
-
-}  // extern "C"
-namespace {
-template <int N>
-int nq_ll_launch_n(tsb_nq* h, const tsb::LlMultiParams& prm, int grid, int pools, int ppt, cudaStream_t s) {
-  // (one pool: one CTA per SM; several: two CTAs of LL_T workers + the exchange warp per SM, capped at 112
-  // registers; three or four pools: 66 CTAs per pool with 768 parents each on 132 SMs, see ll_slice)
-  const int var = pools == 1 ? 0 : ppt == 2 ? 1 : 2;
-  auto kernel = var == 0   ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 2>
-                : var == 1 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 2>
-                           : tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 3>;
-  const size_t smem = (ppt == 2 ? sizeof(tsb::LlSmem<tsb::LL_T, 2>) : sizeof(tsb::LlSmem<tsb::LL_T, 3>)) + 128;
-  bool& attr = h->rounds.attr_llv[var];
-  if (!attr) {
-    TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    attr = true;
-  }
-  void* args[] = {const_cast<tsb::LlMultiParams*>(&prm)};
-  // cooperative: all CTAs of all pools co-resident (two per SM when there are two pools), or the launch fails
-  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid, pools), dim3(tsb::LL_T + 32), args, smem, s));
-  h->launches++;
-  return TSB_OK;
-}
-template <int N>
-int nq_ll_import_n(tsb_nq* h, long long size, cudaStream_t s) {
-  if (size > 0) {
-    tsb::nq_fat_import_kernel<N><<<static_cast<unsigned>((size + 255) / 256), 256, 0, s>>>(
-        h->pool.arena[h->pool.cur], h->rounds.d_fat, size, h->rounds.epoch);
-    TSB_CUDA(cudaGetLastError());
-    h->launches++;
-  }
-  return TSB_OK;
-}
-int nq_ll_launch(tsb_nq* h, const tsb::LlMultiParams& prm, int grid, int pools, int ppt, cudaStream_t s) {
-  switch (h->N) {
-#define TSB_NQ_CASE(n) \
-  case n:              \
-    return nq_ll_launch_n<n>(h, prm, grid, pools, ppt, s);
-    TSB_NQ_CASE(1) TSB_NQ_CASE(2) TSB_NQ_CASE(3) TSB_NQ_CASE(4) TSB_NQ_CASE(5) TSB_NQ_CASE(6) TSB_NQ_CASE(7)
-    TSB_NQ_CASE(8) TSB_NQ_CASE(9) TSB_NQ_CASE(10) TSB_NQ_CASE(11) TSB_NQ_CASE(12) TSB_NQ_CASE(13)
-    TSB_NQ_CASE(14) TSB_NQ_CASE(15) TSB_NQ_CASE(16) TSB_NQ_CASE(17) TSB_NQ_CASE(18) TSB_NQ_CASE(19)
-    TSB_NQ_CASE(20)
-#undef TSB_NQ_CASE
-  }
-  return TSB_EINVAL;
-}
-int nq_ll_import(tsb_nq* h, long long size, cudaStream_t s) {
-  switch (h->N) {
-#define TSB_NQ_CASE(n) \
-  case n:              \
-    return nq_ll_import_n<n>(h, size, s);
-    TSB_NQ_CASE(1) TSB_NQ_CASE(2) TSB_NQ_CASE(3) TSB_NQ_CASE(4) TSB_NQ_CASE(5) TSB_NQ_CASE(6) TSB_NQ_CASE(7)
-    TSB_NQ_CASE(8) TSB_NQ_CASE(9) TSB_NQ_CASE(10) TSB_NQ_CASE(11) TSB_NQ_CASE(12) TSB_NQ_CASE(13)
-    TSB_NQ_CASE(14) TSB_NQ_CASE(15) TSB_NQ_CASE(16) TSB_NQ_CASE(17) TSB_NQ_CASE(18) TSB_NQ_CASE(19)
-    TSB_NQ_CASE(20)
-#undef TSB_NQ_CASE
-  }
-  return TSB_EINVAL;
-}
-// the pool back in the plain 21-byte arena (whoever needs the node records calls this first)
-int nq_materialize(tsb_nq* h) {
-  if (!h->rounds.in_fat) return TSB_OK;
-  TSB_CUDA(cudaSetDevice(h->device));
-  const long long size = h->pool.size;
-  if (size > 0) {
-    tsb::nq_fat_export_kernel<<<static_cast<unsigned>((size + 255) / 256), 256, 0, h->stream>>>(
-        h->rounds.d_fat, h->pool.arena[h->pool.cur], size);
-    TSB_CUDA(cudaGetLastError());
-    h->launches++;
-    TSB_CUDA(cudaStreamSynchronize(h->stream));
-  }
-  h->rounds.in_fat = false;
-  return TSB_OK;
-}
-bool env_no_rounds() {
-  const char* v = std::getenv("TSB200_NO_ROUNDS");
-  return v && *v && *v != '0';
-}
-// grid (CTAs per pool) of the persistent kernel for chunks of up to M parents when one launch serves `pools` pools;
-// 0: M is too large for it.  Chosen on the N = 17 search at M = 50000: one pool: 7/8 of the SMs
-// (one CTA per SM); two pools: one CTA per SM each (two per SM in all); four pools: SMs / 2 CTAs each.  An all-to-all
-// flag exchange among all SMs' CTAs costs 2-3x one among half of them (tools/flag_exchange.py); the per-CTA work grows
-// the other way.
-// *ppt: parents per thread of the kernel variant to launch (2, or 3 when the pool's CTAs would not cover M with 2).
-int nq_ll_grid(const tsb_nq* h, int M, int pools, int* ppt = nullptr) {
-  if (!h->di.coop || env_no_rounds() || pools < 1 || pools > tsb::LL_MAX_POOLS) return 0;
-  const int sms = std::min(h->di.sms, tsb::LL_MAX_SMS);
-  const int most = tsb::ll_ctas_per_pool(sms, pools);  // (ll_tiers.h: the drivers size their warm-up by the same tiers)
-  const int per = static_cast<long long>(most) * tsb::ll_slice(2) >= M ? 2 : 3;
-  const int slice = tsb::ll_slice(per);
-  int grid = pools == 1 ? std::max(1, (sms * 7 / 8) & ~1) : most;
-  while (static_cast<long long>(grid) * slice < M && grid < most) ++grid;  // (M decides)
-  if (ppt) *ppt = per;
-  return static_cast<long long>(M) <= static_cast<long long>(grid) * slice && (pools > 1 || per == 2) ? grid : 0;
-}
-// Up to `max_rounds` rounds of EACH of the K pools (handles on one device, same N) in launches of the persistent
-// kernel that serve all pools that still have work: grid (grid, pools).  out[4 i ..] += {rounds, parents, children,
-// solutions} of pool i.  A pool leaves the launch on its own (done, round budget, arena full, layer table full); the
-// launch ends when every pool has left, the pools that stopped for room grow and go again.
-int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, uint64_t* out) {
-  int64_t left[tsb::LL_MAX_POOLS];
-  bool active[tsb::LL_MAX_POOLS];
-  for (int i = 0; i < K; i++) {
-    left[i] = max_rounds;
-    active[i] = true;
-    nq_pool_setup(hs[i]);
-    int rc = hs[i]->rounds.ensure();
-    if (rc != TSB_OK) return rc;
-  }
-  const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
-  for (;;) {
-    tsb::LlMultiParams mp;
-    std::memset(&mp, 0, sizeof(mp));
-    int map[tsb::LL_MAX_POOLS], n_act = 0;
-    long long need_of[tsb::LL_MAX_POOLS];
-    for (int i = 0; i < K; i++) {
-      tsb_nq* h = hs[i];
-      DevicePool& p = h->pool;
-      if (!active[i] || p.size < m || left[i] <= 0) {
-        active[i] = false;
-        continue;
-      }
-      const long long n = std::min<long long>(p.size, M);
-      const long long need = p.size - n + n * h->N;
-      int rc = TSB_OK;
-      if (h->rounds.in_fat && need > p.cap) rc = nq_materialize(h);  // (grows below and imports again)
-      if (rc != TSB_OK) return rc;
-      if (!h->rounds.in_fat) {
-        // the plain pool as ONE contiguous stack [0, size) with room for the worst case of the next round
-        if (need > p.cap)
-          rc = p.compact(h->stream, std::max<long long>(2 * p.cap, need + need / 2));
-        else if (p.ext.size() != 1 || p.ext[0].b != 0)
-          rc = p.compact(h->stream, p.cap);
-        if (rc == TSB_OK) rc = h->rounds.ensure_fat(p.cap, h->stream);
-        if (rc == TSB_OK) rc = nq_ll_import(h, p.size, h->stream);
-        if (rc != TSB_OK) return rc;
-        h->rounds.in_fat = true;
-        if (n_act > 0) TSB_CUDA(cudaStreamSynchronize(h->stream));  // (the launch goes on the first pool's stream)
-      }
-      tsb::LlParams& prm = mp.pool[n_act];
-      prm.fat = h->rounds.d_fat;
-      prm.cap = std::min(p.cap, h->rounds.fat_cap);
-      prm.size0 = p.size;
-      prm.epoch0 = h->rounds.epoch;
-      prm.m = m;
-      prm.M = M;
-      prm.max_rounds = left[i];
-      prm.prof = prof;
-      prm.sync = h->rounds.d_ll;
-      prm.state = h->rounds.d_state;
-      h->rounds.h_state->exit_code = -1;
-      need_of[n_act] = need;
-      map[n_act++] = i;
-    }
-    if (n_act == 0) break;
-    tsb_nq* h0 = hs[map[0]];
-    // (variant and grid follow the number of pools that still run: a lone survivor gets the one-pool kernel)
-    int ppt = 2;
-    const int grid = nq_ll_grid(h0, M, n_act, &ppt);
-    if (grid == 0) return TSB_EINVAL;  // (checked by the callers for K pools, and fewer pools fit a fortiori)
-    int rc = nq_ll_launch(h0, mp, grid, n_act, ppt, h0->stream);
-    if (rc != TSB_OK) return rc;
-    TSB_CUDA(cudaStreamSynchronize(h0->stream));
-    for (int a = 0; a < n_act; a++) {
-      const int i = map[a];
-      tsb_nq* h = hs[i];
-      DevicePool& p = h->pool;
-      const tsb::RoundsState st = *h->rounds.h_state;
-      if (st.exit_code < 0 || st.exit_code == tsb::RND_EXIT_ABORT) {
-        g_last_cuda_error = "nq_rounds_ll_kernel: watchdog abort (a flag exchange or a node poll did not complete)";
-        return TSB_ECUDA;
-      }
-      if (prof) {
-        const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
-        std::fprintf(stderr, "[tsb200] LL rounds kernel (pool %d of %d): %llu rounds; CTA 0 cycles per round: workers: set-up %.0f "
-                     "poll-nodes %.0f scan+items+diag %.0f build %.0f handoff-wait %.0f store %.0f | exchange warp: "
-                     "scan-wait %.0f publish+gather %.0f bookkeeping %.0f handoff-wait %.0f\n", a, n_act,
-                     static_cast<unsigned long long>(st.rounds), st.prof[tsb::LL_PROF_SETUP] / r, st.prof[tsb::LL_PROF_POLL] / r,
-                     st.prof[tsb::LL_PROF_SCAN] / r, st.prof[tsb::LL_PROF_BUILD] / r, st.prof[tsb::LL_PROF_HAND] / r,
-                     st.prof[tsb::LL_PROF_STORE] / r, st.prof[tsb::LL_PROF_X_SCAN] / r, st.prof[tsb::LL_PROF_X_GATHER] / r,
-                     st.prof[tsb::LL_PROF_X_BOOK] / r, st.prof[tsb::LL_PROF_X_HAND] / r);
-      }
-      h->rounds.epoch = st.epoch;
-      p.size = st.size;
-      p.ext.clear();
-      if (p.size) p.ext.push_back({0, p.size});
-      out[4 * i + 0] += st.rounds;
-      out[4 * i + 1] += st.parents;
-      out[4 * i + 2] += st.children;
-      out[4 * i + 3] += st.solutions;
-      left[i] -= static_cast<int64_t>(st.rounds);
-      if (st.exit_code == tsb::RND_EXIT_SPACE) {
-        if (st.rounds == 0 && need_of[a] <= p.cap) return TSB_ENOMEM;  // (cannot happen)
-        rc = nq_materialize(h);  // back to the plain arena, which then grows
-        if (rc != TSB_OK) return rc;
-      } else if (st.exit_code != tsb::RND_EXIT_RELAUNCH) {  // (layer table full: a fresh launch trusts the whole pool)
-        active[i] = false;                                    // DONE or PAUSE
-      }
-    }
-  }
-  return TSB_OK;
-}
-}  // namespace
-extern "C" {
 
 int tsb_nq_pool_run(tsb_nq* h, int m, int M, int64_t max_rounds, uint64_t* n_rounds, uint64_t* n_parents,
                     uint64_t* n_children, uint64_t* n_solutions) {
@@ -1517,29 +1635,21 @@ int tsb_nq_pool_run(tsb_nq* h, int m, int M, int64_t max_rounds, uint64_t* n_rou
     return TSB_EINVAL;
   *n_rounds = *n_parents = *n_children = *n_solutions = 0;
   TSB_CUDA(cudaSetDevice(h->device));
+  uint64_t out[4] = {0, 0, 0, 0};
+  int rc;
   if (nq_ll_grid(h, M, 1) > 0) {  // the whole loop in launches of the persistent kernel (nq_rounds_ll.cuh)
-    uint64_t out[4] = {0, 0, 0, 0};
     tsb_nq* one[1] = {h};
-    const int rc = nq_ll_run_multi(one, 1, m, M, max_rounds, out);
-    *n_rounds = out[0];
-    *n_parents = out[1];
-    *n_children = out[2];
-    *n_solutions = out[3];
-    return rc;
+    rc = nq_ll_run_multi(one, 1, m, M, max_rounds, out);
+  } else {  // large chunks: one round = two bandwidth-bound kernels (tsb_nq_pool_step)
+    rc = step_loop(max_rounds, out, [&](int64_t* np, uint64_t* nc, uint64_t* ns) {
+      return tsb_nq_pool_step(h, m, M, np, nc, ns);
+    });
   }
-  // large chunks: one round = two bandwidth-bound kernels (tsb_nq_pool_step)
-  while (static_cast<int64_t>(*n_rounds) < max_rounds) {
-    int64_t np = 0;
-    uint64_t nc = 0, ns = 0;
-    int rc = tsb_nq_pool_step(h, m, M, &np, &nc, &ns);
-    if (rc != TSB_OK) return rc;
-    if (np == 0) break;
-    ++*n_rounds;
-    *n_parents += static_cast<uint64_t>(np);
-    *n_children += nc;
-    *n_solutions += ns;
-  }
-  return TSB_OK;
+  *n_rounds = out[0];
+  *n_parents = out[1];
+  *n_children = out[2];
+  *n_solutions = out[3];
+  return rc;
 }
 
 int tsb_nq_sibling(tsb_nq* h, int index, tsb_nq** sibling) {
@@ -1581,77 +1691,15 @@ int tsb_nq_pool_run_multi(tsb_nq* const* handles, int n_pools, int m, int M, int
 
 int tsb_nq_pool_steal(tsb_nq* victim, tsb_nq* thief, int m, int64_t* n_stolen) {
   if (!victim || !thief || victim == thief || m < 1 || !n_stolen || victim->N != thief->N) return TSB_EINVAL;
-  nq_pool_setup(victim);
-  nq_pool_setup(thief);
-  long long n = 0;
-  if (victim->pool.size < 2LL * m) {
-    *n_stolen = 0;
-    return TSB_OK;
-  }
-  int rc = nq_materialize(victim);
-  if (rc == TSB_OK) rc = nq_materialize(thief);
-  if (rc != TSB_OK) return rc;
-  rc = pool_steal_front(victim->pool, victim->device, victim->stream, thief->pool, thief->device, thief->stream, m,
-                            nq_pool_min_cap(thief), &n);
-  *n_stolen = n;
-  return rc;
-}
-
-// diagnostics: cycles per round of bare flag exchanges among co-resident CTAs (rounds_sync_bench_kernel, nq_rounds_ll.cuh)
-int tsb_debug_flag_exchange(int device, int rounds, int variant, int ctas, double* cycles_per_round) {
-  if (!cycles_per_round || rounds < 1) return TSB_EINVAL;
-  DeviceInfo di;
-  int rc = query_device(device, di);
-  if (rc != TSB_OK) return rc;
-  if (!di.coop) return TSB_EUNSUPPORTED;
-  tsb::RoundsSync* sy = nullptr;
-  uint4* scratch = nullptr;
-  long long* d_out = nullptr;
-  int grid = std::min(di.sms, tsb::LL_MAX_SMS);
-  if (ctas > 0 && ctas < grid) grid = ctas;
-  TSB_CUDA(cudaMalloc(&sy, sizeof(*sy)));
-  const size_t scratch_bytes = std::max<size_t>((static_cast<size_t>(grid) * tsb::LL_T + 2) * sizeof(uint4), 2 * 256 * 256 * 4);
-  TSB_CUDA(cudaMalloc(&scratch, scratch_bytes));
-  TSB_CUDA(cudaMemset(scratch, 0, scratch_bytes));
-  TSB_CUDA(cudaMalloc(&d_out, sizeof(long long)));
-  TSB_CUDA(cudaMemset(sy, 0, sizeof(*sy)));
-  unsigned epoch0 = 0;
-  void* args[] = {&sy, &epoch0, &rounds, &variant, &scratch, &d_out};
-  cudaError_t e = cudaLaunchCooperativeKernel(reinterpret_cast<void*>(tsb::rounds_sync_bench_kernel), dim3(grid),
-                                              dim3(tsb::LL_T), args, 0, nullptr);
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  long long cyc = 0;
-  if (e == cudaSuccess) e = cudaMemcpy(&cyc, d_out, sizeof(cyc), cudaMemcpyDeviceToHost);
-  cudaFree(sy);
-  cudaFree(scratch);
-  cudaFree(d_out);
-  if (e != cudaSuccess) {
-    g_last_cuda_error = std::string("flag exchange bench: ") + cudaGetErrorString(e);
-    (void)cudaGetLastError();
-    return TSB_ECUDA;
-  }
-  *cycles_per_round = static_cast<double>(cyc) / rounds;
-  return TSB_OK;
+  return pool_steal(*victim, *thief, m, n_stolen, [victim, thief] {
+    const int rc = nq_materialize(victim);
+    return rc == TSB_OK ? nq_materialize(thief) : rc;
+  });
 }
 
 int tsb_nq_pool_drain(tsb_nq* h, void* nodes, int64_t capacity, int64_t* n) {
   if (!h || !n || capacity < 0) return TSB_EINVAL;
-  DevicePool& p = h->pool;
-  *n = p.size;
-  if (p.size > capacity) return TSB_ENOMEM;
-  TSB_CUDA(cudaSetDevice(h->device));
-  if (int rc = nq_materialize(h); rc != TSB_OK) return rc;
-  long long at = 0;
-  for (const PoolExtent& x : p.ext) {  // extents are the pool in logical (oldest first) order
-    int rc = h->copy_d2h(static_cast<uint8_t*>(nodes) + at * sizeof(tsb_nq_node),
-                         p.arena[p.cur] + x.b * sizeof(tsb_nq_node),
-                         static_cast<size_t>(x.e - x.b) * sizeof(tsb_nq_node), h->stream);
-    if (rc != TSB_OK) return rc;
-    at += x.e - x.b;
-  }
-  p.ext.clear();
-  p.size = 0;
-  return TSB_OK;
+  return pool_drain(*h, nodes, capacity, n, [h] { return nq_materialize(h); });
 }
 
 int tsb_nq_evaluate(tsb_nq* h, const void* parents, int count, uint8_t* labels) {
@@ -1713,6 +1761,8 @@ int tsb_pfsp_create(tsb_pfsp** out, int device, int jobs, int machines, int M_ma
   h->machines = machines;
   h->pairs = nb_pairs;
   h->mt = machines <= 5 ? 5 : machines <= 10 ? 10 : 20;
+  // (88-byte nodes: extents on even records start on a 16-byte boundary)
+  h->pool.set_format(sizeof(tsb_pfsp_node), tsb::PF_TILE, 2, jobs, std::max<long long>(1LL << 20, 4LL * M_max * jobs));
   int rc = h->init(device, M_max, sizeof(tsb_pfsp_node), static_cast<size_t>(jobs) * 4);
   // tables -> device blob (zero padding up to the template machine count is value-neutral:
   // the reference itself evaluates 20-wide zero-padded tuples, lib/pfsp/Bound_simple.chpl:125-135)
@@ -1906,19 +1956,12 @@ int tsb_pfsp_create_wide(tsb_pfsp** out, int device, int max_jobs, int jobs, int
 
 void tsb_pfsp_destroy(tsb_pfsp* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
+  h->fini();
   if (h->d_tab1) cudaFree(h->d_tab1);
   if (h->d_wtab) cudaFree(h->d_wtab);
   delete h->lb2c;
   delete h->lb2u;
   if (h->d_tabu) cudaFree(h->d_tabu);
-  h->ex.release();
-  if (h->d_children) cudaFree(h->d_children);
-  if (h->rnd_h) cudaFreeHost(h->rnd_h);
-  if (h->rnd_sync) cudaFree(h->rnd_sync);
-  h->pool.release();
-  h->fini();
   delete h;
 }
 
@@ -2002,45 +2045,16 @@ int tsb_pfsp_expand(tsb_pfsp* h, int lb_kind, const void* parents, int count, in
   *n_children = *n_solutions = 0;
   if (count == 0) return TSB_OK;
   if (!parents || !children) return TSB_EINVAL;
-  TSB_CUDA(cudaSetDevice(h->device));
-  const size_t need = static_cast<size_t>(h->M_max) * h->jobs * sizeof(tsb_pfsp_node) + 64;
-  if (h->d_children_bytes < need) {
-    if (h->d_children) cudaFree(h->d_children);
-    h->d_children = nullptr;
-    h->d_children_bytes = 0;
-    TSB_CUDA(cudaMalloc(&h->d_children, need));
-    h->d_children_bytes = need;
-  }
-  int rc = h->copy_h2d(h->d_in, parents, sizeof(tsb_pfsp_node) * static_cast<size_t>(count), h->stream);
-  if (rc != TSB_OK) return rc;
-  unsigned long long nc = 0, ns = 0;
-  const std::vector<PoolExtent> pieces{{0, count}};
-  rc = pfsp_expand_round(h, lb_kind, h->d_in, pieces, h->d_children, h->stream, best, &nc, &ns);
-  if (rc != TSB_OK) return rc;
-  *n_children = nc;
-  *n_solutions = ns;
-  if (nc > capacity) return TSB_ENOMEM;
-  return h->copy_d2h(children, h->d_children, nc * sizeof(tsb_pfsp_node), h->stream);
+  return expand_host(*h, parents, count, children, capacity, n_children, n_solutions,
+                     [h, lb_kind, best](auto arena, const auto& pieces, auto kids, auto nc, auto ns) {
+                       return pfsp_expand_round(h, lb_kind, arena, pieces, kids, h->stream, best, nc, ns);
+                     });
 }
 
 int tsb_pfsp_pool_push(tsb_pfsp* h, const void* nodes, int64_t n) {
   if (h && h->wide) return TSB_EUNSUPPORTED;  // (the fused expand / device pool exist for MAX_JOBS = 20 only)
   if (!h || n < 0 || (n && !nodes)) return TSB_EINVAL;
-  TSB_CUDA(cudaSetDevice(h->device));
-  pfsp_pool_setup(h);
-  int rc = h->pool.reserve(h->stream, n, pfsp_pool_min_cap(h));
-  if (rc != TSB_OK) return rc;
-  if (n == 0) return TSB_OK;
-  const long long at = h->pool.top();
-  rc = h->copy_h2d(h->pool.arena[h->pool.cur] + at * sizeof(tsb_pfsp_node), nodes,
-                   static_cast<size_t>(n) * sizeof(tsb_pfsp_node), h->stream);
-  if (rc != TSB_OK) return rc;
-  if (h->pool.ext.empty())
-    h->pool.ext.push_back({at, at + n});
-  else
-    h->pool.ext.back().e += n;
-  h->pool.size += n;
-  return TSB_OK;
+  return pool_push(*h, nodes, n, pfsp_plain);
 }
 
 int64_t tsb_pfsp_pool_size(const tsb_pfsp* h) { return h ? h->pool.size : -1; }
@@ -2052,188 +2066,21 @@ int tsb_pfsp_pool_step(tsb_pfsp* h, int lb_kind, int m, int M, int64_t* best, in
       !n_solutions)
     return TSB_EINVAL;
   if (lb_kind == TSB_LB2 && h->pairs == 0) return TSB_EINVAL;
-  *n_parents = 0;
-  *n_children = *n_solutions = 0;
-  DevicePool& p = h->pool;
-  if (p.size < m) return TSB_OK;  // popBackBulk returns 0 below m (lib/commons/Pool.chpl:50-59)
-  TSB_CUDA(cudaSetDevice(h->device));
-  const long long n = std::min<long long>(p.size, M);
-  std::vector<PoolExtent> pieces;
-  pool_top_pieces(p, n, &pieces);
-  int rc = TSB_OK;
-  if (pieces.size() > tsb::EXP_MAX_PIECES) rc = p.compact(h->stream, p.cap);
-  if (rc == TSB_OK) rc = p.reserve(h->stream, n * h->jobs + 2, pfsp_pool_min_cap(h));
-  if (rc != TSB_OK) return rc;
-  pool_top_pieces(p, n, &pieces);
-  const long long top = (p.top() + 1) & ~1LL;  // children start on a 16-byte boundary (88 B records)
-  unsigned long long nc = 0, ns = 0;
-  uint8_t* arena = p.arena[p.cur];
-  rc = pfsp_expand_round(h, lb_kind, arena, pieces, arena + top * sizeof(tsb_pfsp_node), h->stream, best, &nc, &ns,
-                         /*early=*/true);
-  if (rc != TSB_OK) return rc;
-  pool_pop(p, n);
-  if (nc) {
-    p.ext.push_back({top, top + static_cast<long long>(nc)});
-    p.size += static_cast<long long>(nc);
-  }
-  *n_parents = n;
-  *n_children = nc;
-  *n_solutions = ns;
-  return TSB_OK;
+  return pool_step(*h, m, M, n_parents, n_children, n_solutions, pfsp_plain,
+                   [h, lb_kind, best](auto arena, const auto& pieces, auto kids, auto nc, auto ns) {
+                     return pfsp_expand_round(h, lb_kind, arena, pieces, kids, h->stream, best, nc, ns, /*early=*/true);
+                   });
 }
 
 int tsb_pfsp_pool_steal(tsb_pfsp* victim, tsb_pfsp* thief, int m, int64_t* n_stolen) {
   if (!victim || !thief || victim == thief || m < 1 || !n_stolen || victim->jobs != thief->jobs) return TSB_EINVAL;
-  pfsp_pool_setup(victim);
-  pfsp_pool_setup(thief);
-  long long n = 0;
-  int rc = pool_steal_front(victim->pool, victim->device, victim->stream, thief->pool, thief->device, thief->stream, m,
-                            pfsp_pool_min_cap(thief), &n);
-  *n_stolen = n;
-  return rc;
+  return pool_steal(*victim, *thief, m, n_stolen, pfsp_plain);
 }
 
 int tsb_pfsp_pool_drain(tsb_pfsp* h, void* nodes, int64_t capacity, int64_t* n) {
   if (!h || !n || capacity < 0) return TSB_EINVAL;
-  DevicePool& p = h->pool;
-  *n = p.size;
-  if (p.size > capacity) return TSB_ENOMEM;
-  TSB_CUDA(cudaSetDevice(h->device));
-  long long at = 0;
-  for (const PoolExtent& x : p.ext) {
-    int rc = h->copy_d2h(static_cast<uint8_t*>(nodes) + at * sizeof(tsb_pfsp_node),
-                         p.arena[p.cur] + x.b * sizeof(tsb_pfsp_node),
-                         static_cast<size_t>(x.e - x.b) * sizeof(tsb_pfsp_node), h->stream);
-    if (rc != TSB_OK) return rc;
-    at += x.e - x.b;
-  }
-  p.ext.clear();
-  p.size = 0;
-  return TSB_OK;
+  return pool_drain(*h, nodes, capacity, n, pfsp_plain);
 }
-
-}  // extern "C"
-
-// ---- PFSP: the whole offload loop in launches of the persistent kernel (pfsp_rounds.cuh)
-namespace {
-// CTAs of the persistent PFSP kernel for chunks of up to M parents (one per SM at most, each with up to PFR_SLICE
-// parents; fewer CTAs for smaller M, so that the two exchanges of a round involve only the CTAs that have parents to
-// evaluate); 0: the loop of tsb_pfsp_pool_step runs instead (lb2, M above PFR_MAX_M where the step loop is faster, M
-// beyond pf_rounds_capacity, no cooperative launch, env TSB200_NO_ROUNDS=1)
-int pfsp_rounds_grid(const tsb_pfsp* h, int lb_kind, int M) {
-  if (lb_kind == TSB_LB2 || !h->di.coop || env_no_rounds()) return 0;
-  if (M > tsb::PFR_MAX_M || M > tsb::pf_rounds_capacity(h->di.sms)) return 0;
-  const int sms = std::min(h->di.sms, tsb::PFR_MAX_CTAS);
-  return static_cast<int>(std::min<long long>(sms, (static_cast<long long>(M) + tsb::PF_TILE - 1) / tsb::PF_TILE));
-}
-template <int KIND, int M>
-int pfsp_rounds_launch_km(tsb_pfsp* h, const tsb::PfRoundsParams& prm, int grid, cudaStream_t s) {
-  auto kernel = h->simd16 ? tsb::pfsp_rounds_kernel<KIND, M, true> : tsb::pfsp_rounds_kernel<KIND, M, false>;
-  const size_t smem = sizeof(tsb::PfRoundsSmem) + 128;
-  if (!h->rnd_attr[KIND]) {
-    TSB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    h->rnd_attr[KIND] = true;
-  }
-  void* args[] = {const_cast<tsb::PfRoundsParams*>(&prm)};
-  // cooperative: every CTA co-resident (the exchanges wait for all of them), or the launch fails
-  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid), dim3(tsb::PF_THREADS), args, smem, s));
-  h->launches++;
-  return TSB_OK;
-}
-template <int KIND>
-int pfsp_rounds_launch_k(tsb_pfsp* h, const tsb::PfRoundsParams& prm, int grid, cudaStream_t s) {
-  if (h->mt == 5) return pfsp_rounds_launch_km<KIND, 5>(h, prm, grid, s);
-  if (h->mt == 10) return pfsp_rounds_launch_km<KIND, 10>(h, prm, grid, s);
-  return pfsp_rounds_launch_km<KIND, 20>(h, prm, grid, s);
-}
-// Up to max_rounds rounds in launches of the persistent kernel; out[] += {rounds, parents, children, solutions}.  A
-// launch leaves when the pool holds fewer than m nodes, after its round budget, when the next round's worst case
-// does not fit the arena (it grows and the loop relaunches) or when a leaf of the chunk improves *best (that round
-// goes through tsb_pfsp_pool_step and its sequential rule, then the loop relaunches with the new incumbent).
-int pfsp_rounds_run(tsb_pfsp* h, int lb_kind, int m, int M, int grid, int64_t max_rounds, int64_t* best, uint64_t* out) {
-  DevicePool& p = h->pool;
-  pfsp_pool_setup(h);
-  if (!h->rnd_h) {
-    TSB_CUDA(cudaHostAlloc(&h->rnd_h, sizeof(tsb::RoundsState), cudaHostAllocPortable | cudaHostAllocMapped));
-    std::memset(h->rnd_h, 0, sizeof(tsb::RoundsState));
-    TSB_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&h->rnd_d), h->rnd_h, 0));
-  }
-  if (!h->rnd_sync) {
-    TSB_CUDA(cudaMalloc(&h->rnd_sync, sizeof(tsb::PfRoundsSync)));
-    TSB_CUDA(cudaMemsetAsync(h->rnd_sync, 0, sizeof(tsb::PfRoundsSync), h->stream));
-  }
-  const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
-  int64_t left = max_rounds;
-  while (left > 0 && p.size >= m) {
-    // the pool as ONE contiguous stack [0, size) with room for the worst case of the next round
-    const long long n = std::min<long long>(p.size, M);
-    const long long need = p.size - n + n * h->jobs;
-    int rc = TSB_OK;
-    if (need > p.cap)
-      rc = p.compact(h->stream, std::max<long long>(2 * p.cap, need + need / 2));
-    else if (p.ext.size() != 1 || p.ext[0].b != 0)
-      rc = p.compact(h->stream, p.cap);
-    if (rc != TSB_OK) return rc;
-    tsb::PfRoundsParams prm;
-    std::memset(&prm, 0, sizeof(prm));
-    prm.arena = p.arena[p.cur];
-    prm.tables = h->d_tab1;
-    prm.cap = p.cap;
-    prm.size0 = p.size;
-    prm.max_rounds = left;
-    prm.epoch0 = h->rnd_epoch;
-    prm.m = m;
-    prm.M = M;
-    prm.best = clamp_best(*best);
-    prm.prof = prof;
-    prm.sync = h->rnd_sync;
-    prm.state = h->rnd_d;
-    h->rnd_h->exit_code = -1;
-    rc = lb_kind == TSB_LB1 ? pfsp_rounds_launch_k<1>(h, prm, grid, h->stream) : pfsp_rounds_launch_k<0>(h, prm, grid, h->stream);
-    if (rc != TSB_OK) return rc;
-    TSB_CUDA(cudaStreamSynchronize(h->stream));
-    const tsb::RoundsState st = *h->rnd_h;
-    if (st.exit_code < 0 || st.exit_code == tsb::RND_EXIT_ABORT) {
-      g_last_cuda_error = "pfsp_rounds_kernel: watchdog abort (a count or store exchange did not complete)";
-      return TSB_ECUDA;
-    }
-    if (prof) {
-      const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
-      std::fprintf(stderr, "[tsb200] PFSP rounds kernel: %llu rounds (exit %d); CTA 0 cycles per round: load %.0f bounds %.0f "
-                   "publish+items %.0f gather %.0f store %.0f store-exchange %.0f\n",
-                   static_cast<unsigned long long>(st.rounds), st.exit_code, st.prof[tsb::PFR_PROF_LOAD] / r,
-                   st.prof[tsb::PFR_PROF_BOUND] / r, st.prof[tsb::PFR_PROF_PUBLISH] / r, st.prof[tsb::PFR_PROF_GATHER] / r,
-                   st.prof[tsb::PFR_PROF_STORE] / r, st.prof[tsb::PFR_PROF_BARRIER] / r);
-    }
-    h->rnd_epoch = st.epoch;
-    p.size = st.size;
-    p.ext.clear();
-    if (p.size) p.ext.push_back({0, p.size});
-    out[0] += st.rounds;
-    out[1] += st.parents;
-    out[2] += st.children;
-    out[3] += st.solutions;
-    left -= static_cast<int64_t>(st.rounds);
-    if (st.exit_code == tsb::RND_EXIT_SPACE) {
-      if (st.rounds == 0 && need <= p.cap) return TSB_ENOMEM;  // (cannot happen: the arena was grown for `need`)
-    } else if (st.exit_code == tsb::PFR_EXIT_IMPROVED) {
-      int64_t np = 0;
-      uint64_t nc = 0, ns = 0;
-      rc = tsb_pfsp_pool_step(h, lb_kind, m, M, best, &np, &nc, &ns);
-      if (rc != TSB_OK) return rc;
-      out[0] += 1;
-      out[1] += static_cast<uint64_t>(np);
-      out[2] += nc;
-      out[3] += ns;
-      --left;
-    } else {
-      break;  // DONE or PAUSE
-    }
-  }
-  return TSB_OK;
-}
-}  // namespace
-extern "C" {
 
 int tsb_pfsp_pool_run(tsb_pfsp* h, int lb_kind, int m, int M, int64_t max_rounds, int64_t* best, uint64_t* n_rounds,
                       uint64_t* n_parents, uint64_t* n_children, uint64_t* n_solutions) {
@@ -2244,28 +2091,20 @@ int tsb_pfsp_pool_run(tsb_pfsp* h, int lb_kind, int m, int M, int64_t max_rounds
   if (lb_kind == TSB_LB2 && h->pairs == 0) return TSB_EINVAL;
   *n_rounds = *n_parents = *n_children = *n_solutions = 0;
   TSB_CUDA(cudaSetDevice(h->device));
+  uint64_t out[4] = {0, 0, 0, 0};
+  int rc;
   if (const int grid = pfsp_rounds_grid(h, lb_kind, M); grid > 0) {
-    uint64_t out[4] = {0, 0, 0, 0};
-    const int rc = pfsp_rounds_run(h, lb_kind, m, M, grid, max_rounds, best, out);
-    *n_rounds = out[0];
-    *n_parents = out[1];
-    *n_children = out[2];
-    *n_solutions = out[3];
-    return rc;
+    rc = pfsp_rounds_run(h, lb_kind, m, M, grid, max_rounds, best, out);
+  } else {  // lb2, large chunks: one round = two kernels (tsb_pfsp_pool_step)
+    rc = step_loop(max_rounds, out, [&](int64_t* np, uint64_t* nc, uint64_t* ns) {
+      return tsb_pfsp_pool_step(h, lb_kind, m, M, best, np, nc, ns);
+    });
   }
-  // lb2, large chunks: one round = two kernels (tsb_pfsp_pool_step)
-  while (static_cast<int64_t>(*n_rounds) < max_rounds) {
-    int64_t np = 0;
-    uint64_t nc = 0, ns = 0;
-    const int rc = tsb_pfsp_pool_step(h, lb_kind, m, M, best, &np, &nc, &ns);
-    if (rc != TSB_OK) return rc;
-    if (np == 0) break;
-    ++*n_rounds;
-    *n_parents += static_cast<uint64_t>(np);
-    *n_children += nc;
-    *n_solutions += ns;
-  }
-  return TSB_OK;
+  *n_rounds = out[0];
+  *n_parents = out[1];
+  *n_children = out[2];
+  *n_solutions = out[3];
+  return rc;
 }
 
 }  // extern "C"

@@ -295,6 +295,17 @@ void static_split(Pool<Node>& pool, int D, std::vector<Pool<Node>>& multi);
 // rounds per library call when other tasks may want to steal (a victim serves requests between calls)
 inline int64_t rounds_per_call(const StealBoard* sb, int M) { return !sb ? INT64_MAX : small_chunks(M) ? 256 : 4; }
 
+// drain a device pool and push what it held back onto the host pool
+template <class H, class Node>
+int drain_to_host(H* h, Pool<Node>& pool, int64_t (*size)(const H*), int (*drain)(H*, void*, int64_t, int64_t*)) {
+  const int64_t left = size(h);
+  std::vector<Node> rest(static_cast<size_t>(left) + 1);
+  int64_t n = 0;
+  const int rc = drain(h, rest.data(), left, &n);
+  for (int64_t i = 0; i < n && rc == TSB_OK; i++) pool.pushBack(rest[i]);
+  return rc;
+}
+
 // the offload loop with the task's pool resident on the device (tsb_nq_pool_*): all rounds of step 2 inside the
 // library (one persistent kernel for small M, two kernels per round otherwise); the host only reads counters
 void nq_devpool_rounds(tsb_nq* h, int m, int M, StealBoard* sb, int me, GpuTaskResult& r) {
@@ -404,11 +415,7 @@ void nq_devpool_on(tsb_nq* h, int m, int M, Pool<tsb_nq_node>& pool, GpuTaskResu
     if (r.rc == TSB_OK) nq_devpool_multi_rounds(hs, m, M, sb, me, r);
     for (tsb_nq* x : hs) {
       if (r.rc != TSB_OK) break;
-      const int64_t left = tsb_nq_pool_size(x);
-      std::vector<tsb_nq_node> rest(static_cast<size_t>(left) + 1);
-      int64_t n = 0;
-      r.rc = tsb_nq_pool_drain(x, rest.data(), left, &n);
-      for (int64_t i = 0; i < n && r.rc == TSB_OK; i++) pool.pushBack(rest[i]);
+      r.rc = drain_to_host(x, pool, tsb_nq_pool_size, tsb_nq_pool_drain);
     }
     r.launches = tsb_nq_kernel_launches(h) - l0;
     return;
@@ -418,13 +425,7 @@ void nq_devpool_on(tsb_nq* h, int m, int M, Pool<tsb_nq_node>& pool, GpuTaskResu
   pool.size = 0;
   if (sb) sb->publish_handle(me, r.rc == TSB_OK ? h : nullptr, tsb_nq_pool_size(h));
   if (r.rc == TSB_OK) nq_devpool_rounds(h, m, M, sb, me, r);
-  if (r.rc == TSB_OK) {
-    const int64_t left = tsb_nq_pool_size(h);
-    std::vector<tsb_nq_node> rest(static_cast<size_t>(left) + 1);
-    int64_t n = 0;
-    r.rc = tsb_nq_pool_drain(h, rest.data(), left, &n);
-    for (int64_t i = 0; i < n && r.rc == TSB_OK; i++) pool.pushBack(rest[i]);
-  }
+  if (r.rc == TSB_OK) r.rc = drain_to_host(h, pool, tsb_nq_pool_size, tsb_nq_pool_drain);
   r.launches = tsb_nq_kernel_launches(h) - l0;
 }
 // Handles of the device-pool drivers are kept between searches (per device, N, g, M): a handle with its sibling
@@ -709,13 +710,7 @@ void pfsp_devpool_on(tsb_pfsp* h, int lb_kind, int m, int M, Pool<tsb_pfsp_node>
     if (!board_acquire(sb, me, size, steal_floor(m, M))) break;
   }
   if (r.rc != TSB_OK) board_abort(sb, me);
-  if (r.rc == TSB_OK) {
-    const int64_t left = tsb_pfsp_pool_size(h);
-    std::vector<tsb_pfsp_node> rest(static_cast<size_t>(left) + 1);
-    int64_t n = 0;
-    r.rc = tsb_pfsp_pool_drain(h, rest.data(), left, &n);
-    for (int64_t i = 0; i < n && r.rc == TSB_OK; i++) pool.pushBack(rest[i]);
-  }
+  if (r.rc == TSB_OK) r.rc = drain_to_host(h, pool, tsb_pfsp_pool_size, tsb_pfsp_pool_drain);
   r.launches = tsb_pfsp_kernel_launches(h) - l0;
 }
 void pfsp_devpool_task(int device, const tsb_pfsp_tables& t, int lb_kind, int m, int M, Pool<tsb_pfsp_node>& pool,
