@@ -1,6 +1,7 @@
 // ll_tiers.h — how large a chunk one launch of the persistent N-Queens kernel (nq_rounds_ll.cuh) takes, as a
 // function of the GPU's SM count.  Shared by the library (nq_ll_grid) and the search drivers (tsb_host.cpp), which
-// size the warm-up and the steal policy by it before any handle exists.  Plain C++: no CUDA here.
+// size the warm-up and the steal policy by it before any handle exists; and when a launch clears the 16-bit tags of
+// the pool's arena first.  Plain C++: no CUDA here.
 #pragma once
 
 namespace tsb {
@@ -24,6 +25,23 @@ constexpr long long ll_pool_capacity(int sms, int pools) {
 // beyond the one-pool capacity they run one pool in two-kernel rounds.)
 constexpr int ll_pools_for(int sms, long long M) {
   return M <= ll_pool_capacity(sms, 4) ? 4 : M <= ll_pool_capacity(sms, 3) ? 3 : M <= ll_pool_capacity(sms, 1) ? 2 : 1;
+}
+
+// epochs after a clear of the arena's tags that a launch may use (the tags of epochs repeat mod 65535; the argument
+// is at the top of nq_rounds_ll.cuh)
+constexpr unsigned LL_TAG_SPAN = 65535u;
+// Before a launch at epoch `epoch` (the last one used) that may run `max_rounds` rounds, with the arena's tags last
+// cleared at epoch `clear_epoch`: whether to clear them first (then the clear's epoch is `epoch`), and the last epoch
+// the launch may use.  A launch that would have fewer than min(max_rounds, LL_TAG_SPAN / 2) epochs left clears, so
+// a clear comes at most once per 32 767 rounds.
+struct LlTagWindow {
+  bool clear;
+  unsigned epoch_last;
+};
+constexpr LlTagWindow ll_tag_window(unsigned epoch, unsigned clear_epoch, long long max_rounds) {
+  const long long left = static_cast<long long>(clear_epoch) + LL_TAG_SPAN - epoch;
+  const long long want = max_rounds < LL_TAG_SPAN / 2 ? max_rounds : LL_TAG_SPAN / 2;
+  return left < want ? LlTagWindow{true, epoch + LL_TAG_SPAN} : LlTagWindow{false, clear_epoch + LL_TAG_SPAN};
 }
 
 }  // namespace tsb

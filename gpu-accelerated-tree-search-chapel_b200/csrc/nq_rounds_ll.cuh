@@ -15,22 +15,36 @@
 // removed in favour of this kernel.  Here the pool lives, while the kernel runs, in a SELF-VALIDATING format
 // (the "LL" idea of NCCL's low-latency protocol):
 //
-//   fat node = 4 x 8-byte words; word i = data32[i] | epoch << 32     (32 B per node = one sector, 32-byte aligned)
+//   fat node = 4 x 8-byte words; word i = data32[i] | x16[i] << 32 | tag << 48   (32 B per node = one sector,
+//   32-byte aligned), read and written as two 16-byte pieces (words 0-1 and 2-3)
 //   data32[0..3] = the node packed in 125 bits (any N <= 20: every board value is below 32):
 //     board[i] in bits 5 (i % 6) .. +4 of data32[i / 6]            (six values per word; board[18], [19] in data32[3])
 //     depth in the 2-bit tails (bits 30..31) of data32[0], [1], [2]: bits 0-1, 2-3 and 4 of the depth
 //     data32[3] bits 10..29: the node's child mask (slot k set <=> k >= depth and board[k] is not attacked: evaluate_gpu's
 //     label for slot k, nqueens_gpu_chpl.chpl:97-123), bit 30: leaf (depth == N)
-//   The diagonal masks of a parent (what its next row attacks) are not stored: a round recomputes them from the placed
-//   prefix, O(depth) independent terms (ll_parent_diag), while the child counts are on their way; a child's masks
-//   follow from its parent's in O(1) (ll_build_child), and its child mask is evaluated when it is built.  (The earlier
-//   version stored the masks in a side word next to each 21-byte node: 64 bytes per node, twice the poll loads and
-//   store pieces of a round.)
+//   x16[0..3] = the node's diagonal masks, the values its next row attacks (N bits each):
+//     ld (rising diagonals) = x16[0] | x16[1] << 16, in piece 0; rd (falling diagonals) = x16[2] | x16[3] << 16, in piece 1
+//   tag = the 16-bit tag of the epoch the word was stored in (ll_tag; 0: no round's tag, see below)
+//   A child's masks follow from its parent's in O(1) and its child mask is evaluated from them when it is built
+//   (ll_build_child), so a round reads its parents' masks instead of recomputing them from the placed prefix.  (An
+//   earlier version stored the masks in a side word next to each 21-byte node: 64 bytes per node, twice the poll loads
+//   and store pieces of a round.)
 //
 // Every 8-byte word is written by one store (an element of a st.v2.u64) and is therefore seen whole or not at all;
-// a reader that expects the children of round r polls the words of its slice until all four carry r's epoch.  No
+// a reader that expects the children of round r polls the words of its slice until all four carry r's tag.  No
 // fence, no "done" flags: the data is its own flag, and a round costs ONE flag exchange (the child counts) plus one
-// store -> L2 -> poll hop for the nodes.  Epochs are 32 bits and never repeat, so stale words cannot alias.
+// store -> L2 -> poll hop for the nodes.
+//
+// Tags are 16 bits, so they repeat, and a stale word must never carry the tag a reader expects at its position.
+// Epochs count rounds (32 bits, never repeating; the count slots of LlSync carry them whole) and tag(e) = e mod 65535
+// + 1 (ll_tag), so tag 0 belongs to no epoch and epochs less than 65535 apart have different tags.  Per pool the host
+// keeps the epoch C of the last CLEAR, which sets the tag of every word of the arena to 0 (data kept; a new arena is
+// zeroed, and the import from the plain arena stores tag 0), and a launch uses epochs up to C + LL_TAG_SPAN at most
+// (LlParams::epoch_last: the kernel leaves with RND_EXIT_RELAUNCH there; the host clears before a launch that would
+// have too few epochs left, ll_tag_window).  So every word of the arena carries tag 0 or the tag of an epoch e' with
+// C < e' < e for any live epoch e <= C + LL_TAG_SPAN: 0 < e - e' < 65535, the tags differ, and tag 0 is no live
+// round's.  A clear re-tags only the positions below the highest pool size reached since the previous clear
+// (RoundsState::size_hi: every store of a launch lies below it), about once per 65 000 rounds.
 //
 // Nodes that are NOT children of the previous round (the chunk reaches below the newest layer when a round produced
 // fewer than M children) carry the epoch of the round that stored them.  Every CTA keeps the LAYER STACK of the pool
@@ -84,6 +98,7 @@ struct RoundsState {
   int exit_code;
   unsigned long long rounds, parents, children, solutions;  // of this launch
   long long prof[12];  // (prm.prof) cycles CTA 0 spent per phase (the LL_PROF_* indices of nq_rounds_ll_kernel)
+  long long size_hi;   // (nq_rounds_ll_kernel) the largest pool size of the launch: every position it stored lies below
 };
 
 __device__ __forceinline__ void st_relaxed_u64(unsigned long long* p, unsigned long long v) {
@@ -112,11 +127,20 @@ struct SpinGuard {  // watchdog of a spin loop: ~2 s, or another CTA's abort
 constexpr int LL_CAP = 2048;
 constexpr int LL_WORDS = 4;                  // 8-byte words per fat node
 constexpr int LL_LAYERS = 1024;              // layers of the pool a CTA tracks (more: the kernel leaves and is relaunched)
-constexpr unsigned LL_TRUSTED = 0u;          // layer epoch of the nodes that were in the pool at launch (epochs start at 1)
+constexpr unsigned LL_TRUSTED = 0u;          // layer tag of the nodes that were in the pool at launch (no round's tag)
+// the 16-bit tag of epoch e: 1 .. 65535 (see above; LL_TAG_SPAN and the host's clear decision: ll_tiers.h)
+__device__ __forceinline__ unsigned ll_tag(unsigned e) { return e % LL_TAG_SPAN + 1u; }
 
 struct alignas(32) FatNode {
   unsigned long long w[LL_WORDS];
 };
+// a 16-byte piece of a fat node from two data words and the piece's diagonal mask (ld for piece 0, rd for piece 1)
+// and tag: x16 = the mask's low half in the first word, its high half in the second
+__device__ __forceinline__ void ll_piece(uint32_t d0, uint32_t d1, uint32_t mask, uint32_t tag, unsigned long long& a,
+                                         unsigned long long& b) {
+  a = static_cast<unsigned long long>(__byte_perm(mask, tag, 0x5410)) << 32 | d0;
+  b = static_cast<unsigned long long>(__byte_perm(mask, tag, 0x5432)) << 32 | d1;
+}
 // the packed node (data32[0..3], see above)
 constexpr int LL_CM_SHIFT = 10;          // child mask: data32[3] bits 10..29
 constexpr uint32_t LL_LEAF = 1u << 30;   // leaf flag: data32[3] bit 30
@@ -140,7 +164,8 @@ struct LlParams {
   FatNode* fat;
   long long cap;    // nodes the fat arena holds
   long long size0;  // nodes in the pool at launch: positions [0, size0), all stored before the launch
-  unsigned epoch0;  // last epoch used so far (the import kernel's tag or the previous launch's last round)
+  unsigned epoch0;      // last epoch used so far (the previous launch's last round)
+  unsigned epoch_last;  // the last epoch this launch may use (ll_tag_window)
   int m, M;
   long long max_rounds;
   int prof;
@@ -190,8 +215,6 @@ __device__ __forceinline__ void st_fat2(unsigned long long* p, unsigned long lon
 //   bits 40..59  the node's child mask: slot k set <=> k >= depth and board[k] is not attacked (evaluate_gpu's
 //                label for slot k, nqueens_gpu_chpl.chpl:97-123)
 //   bit  60      leaf (depth == N)
-// The import keeps only the child mask and the leaf flag.  A helper that returns just those compiles the import to
-// different (not faster) code, so the whole word is kept.
 __device__ __forceinline__ unsigned long long nq_aux_pack(uint32_t ld, uint32_t rd, uint32_t cm, bool leaf) {
   return static_cast<unsigned long long>(ld) | static_cast<unsigned long long>(rd) << 20 |
          static_cast<unsigned long long>(cm) << 40 | static_cast<unsigned long long>(leaf ? 1u : 0u) << 60;
@@ -211,9 +234,9 @@ __device__ __forceinline__ unsigned long long nq_aux_of_node(const uint8_t* node
     if (!((U >> (node[1 + k] & 31)) & 1u)) cm |= 1u << k;
   return nq_aux_pack(ld, rd, cm, d == N);
 }
+// (tag 0: the nodes are the trusted layer of the next launch)
 template <int N>
-__global__ void nq_fat_import_kernel(const uint8_t* __restrict__ arena, FatNode* __restrict__ fat, long long size,
-                                     unsigned epoch) {
+__global__ void nq_fat_import_kernel(const uint8_t* __restrict__ arena, FatNode* __restrict__ fat, long long size) {
   const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (p >= size) return;
   const uint8_t* node = arena + p * NQ_REC;
@@ -222,8 +245,18 @@ __global__ void nq_fat_import_kernel(const uint8_t* __restrict__ arena, FatNode*
   ll_set_depth(d, node[0]);
   const unsigned long long aux = nq_aux_of_node<N>(node);
   d[3] |= (static_cast<uint32_t>(aux >> 40) & 0xFFFFFu) << LL_CM_SHIFT | ((aux >> 60) & 1u ? LL_LEAF : 0u);
-  const unsigned long long e = static_cast<unsigned long long>(epoch) << 32;
-  for (int i = 0; i < LL_WORDS; i += 2) st_fat2(&fat[p].w[i], d[i] | e, d[i + 1] | e);
+  unsigned long long w[LL_WORDS];
+  ll_piece(d[0], d[1], static_cast<uint32_t>(aux) & 0xFFFFFu, 0u, w[0], w[1]);
+  ll_piece(d[2], d[3], static_cast<uint32_t>(aux >> 20) & 0xFFFFFu, 0u, w[2], w[3]);
+  for (int i = 0; i < LL_WORDS; i += 2) st_fat2(&fat[p].w[i], w[i], w[i + 1]);
+}
+// the clear: tag 0 on the `words` first words of the arena, data kept
+__global__ void nq_fat_clear_tags_kernel(FatNode* __restrict__ fat, long long words) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i < words) {
+    unsigned long long* w = &fat[0].w[0] + i;
+    *w &= 0x0000FFFFFFFFFFFFull;
+  }
 }
 __global__ void nq_fat_export_kernel(const FatNode* __restrict__ fat, uint8_t* __restrict__ arena, long long size) {
   const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -288,7 +321,7 @@ __device__ __forceinline__ bool warp_gather_slots2(const unsigned long long* slo
 struct LlPlan {
   long long s0;             // next round: position of the chunk's first parent (= of the round's first child)
   int a0, len0, a1, len1;   // next round: this CTA's two sub-slices of the chunk (first parent, parents)
-  unsigned epoch;           // next round's epoch
+  unsigned tag;             // next round's tag (ll_tag of its epoch)
   int top;                  // next round: top layer of the layer stack
   int exit;                 // -1: run the next round; else the RND_EXIT_* code all threads leave with
   int off0, off1;           // this round: first child of each of this CTA's sub-slices among the round's children
@@ -303,46 +336,23 @@ static_assert(LL_PROF_N <= 12, "RoundsState::prof");
 template <int T, int PPT>
 struct LlSmem {
   alignas(16) uint4 parent[T * PPT];   // the slice: data32[0..3] of every parent
+  alignas(8) uint2 diag[T * PPT];      // ... and its {ld, rd}
   alignas(16) uint4 stage[LL_CAP];     // the window's children: data32[0..3]
-  alignas(8) uint2 diag[T * PPT];      // {ld, rd} of the parents with children (ll_parent_diag), at their own index
+  alignas(8) uint2 stage_diag[LL_CAP]; // ... and their {ld, rd}
   alignas(16) uint16_t item[T * PPT * 20];  // (record << 5) | slot, in child order
-  uint16_t fertile[T * PPT];           // per warp (32 PPT entries each): the records of its parents with children
   unsigned long long warp_tot64[T / 32];
   LlPlan plan;
   int poll_abort;                  // a worker's poll gave up: the exchange warp leaves after the scan barrier
   long long prof[LL_PROF_N], prof_t[2];  // (prm.prof, CTA 0) cycles per phase; clock at the end of the last one
                                          // (workers, exchange warp)
   long long lay_start[LL_LAYERS];  // the pool's layers, bottom to top: first position ...
-  unsigned lay_epoch[LL_LAYERS];   // ... and the epoch its nodes were stored with (LL_TRUSTED: before the launch)
+  unsigned lay_tag[LL_LAYERS];     // ... and the tag its nodes were stored with (LL_TRUSTED: before the launch)
 };
 
-// the values a parent's next row (row `depth`) attacks along the rising (ld) and falling (rd) diagonals of its placed
-// rows 0 .. depth-1: the queen of row i attacks board[i] + (depth - i) and board[i] - (depth - i) there.  Each row's
-// term is computed on its own and the terms are ORed, with ld masked to N bits once: bits that leave [0, N) never
-// come back, so this equals moving the masks row by row as ll_build_child does (ld = ((ld | bit) << 1) mod 2^N,
-// rd = (rd | bit) >> 1), without that chain of ~3 dependent operations per row.  The variable shifts are products
-// with 2^(depth-1-i) (ld) and the high word of one with 2^(32-depth+i) (rd): multiplies run on the FMA pipe, beside
-// the shifts and ORs on the integer pipe, and the factors, shifted by the constant i, are 0 for the rows i >= depth
-// (no predicate).
+// child `item` of the slice -> its four data words (board[depth] and board[k] swapped, depth + 1, its child mask
+// evaluated here) and *cdiag its diagonal masks, from its parent's
 template <int N>
-__device__ __forceinline__ uint2 ll_parent_diag(const uint4 p) {
-  const uint32_t P[4] = {p.x, p.y, p.z, p.w};
-  const uint32_t depth = ll_depth(p.x, p.y, p.z);
-  const uint32_t pl = shl_clamp(1u, depth - 1u), pr = shl_clamp(1u, 32u - depth);  // (both 0 for depth 0)
-  uint32_t ld = 0, rd = 0;
-#pragma unroll
-  for (int i = 0; i < N; i++) {
-    const uint32_t x2 = shf_l_wrap(0u, 2u, P[ll_fw(i)] >> ll_fs(i));  // 2 << board[i] (the shift wraps mod 32)
-    ld |= x2 * (pl >> i);         // (1 << board[i]) << (depth - i); 0 for i >= depth
-    rd |= __umulhi(x2, pr << i);  // (2 << board[i]) >> (depth - i); 0 for i >= depth
-  }
-  return make_uint2(ld & ((1u << N) - 1u), rd >> 1);
-}
-
-// child `item` of the slice -> its four data words: board[depth] and board[k] swapped, depth + 1, its masks from the
-// parent's, its child mask evaluated here
-template <int N>
-__device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2* diag, int item) {
+__device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2* diag, int item, uint2* cdiag) {
   const int r = item >> 5;
   const uint32_t k = static_cast<uint32_t>(item & 31);
   const uint4 p = parent[r];
@@ -362,7 +372,9 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
   ll_set_depth(P, cd);
   const uint2 pd = diag[r];
   const uint32_t bit = 1u << v;
-  const uint32_t S = ~((((pd.x | bit) << 1) & ((1u << N) - 1u)) | ((pd.y | bit) >> 1));  // safe values of row cd
+  const uint32_t cld = ((pd.x | bit) << 1) & ((1u << N) - 1u), crd = (pd.y | bit) >> 1;
+  *cdiag = make_uint2(cld, crd);
+  const uint32_t S = ~(cld | crd);  // safe values of row cd
   uint32_t cm = 0;
 #pragma unroll
   for (int i = 0; i < N; i++) {
@@ -375,9 +387,8 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
 }
 
 // One CTA = LL_T worker threads (warps 0-7) + one EXCHANGE warp (warp 8).  A round:
-//   workers:   poll the slice -> child masks, block scan -> (LL_BAR_SCAN arrive) -> items, each warp's list of parents
-//              with children and their diagonals -> build the first window -> HANDOFF -> store the windows -> the
-//              next round's poll
+//   workers:   poll the slice -> child masks, block scan -> (LL_BAR_SCAN arrive) -> items -> build the first window
+//              -> HANDOFF -> store the windows -> the next round's poll
 //   exchange:  (LL_BAR_SCAN wait) -> publish the CTA's two count slots -> gather all 2G slots -> offsets, layer stack,
 //              pool size, counters, exit tests and the next round's geometry -> HANDOFF
 // so the gather runs while the workers build, and the bookkeeping of a round and the set-up of the next are off the
@@ -407,6 +418,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
 
   // ---- the exchange warp's pool state (every lane holds the same values; lane 0 writes shared memory)
   long long size = prm.size0, chunk_s0 = 0, chunk_n = 0;  // (the chunk of the current round)
+  long long size_hi = prm.size0;
   unsigned epoch = prm.epoch0;
   int n_lay = prm.size0 > 0 ? 1 : 0;
   long long lay_top = 0;  // lay_start[n_lay - 1] (n_lay > 0)
@@ -429,7 +441,9 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       chunk_s0 = size - chunk_n;
       if (chunk_s0 + chunk_n * N > prm.cap)  // worst case: every slot of every parent survives
         ex = RND_EXIT_SPACE;
-      else if (n_lay >= LL_LAYERS)  // (no room to record this round's children: start over with one trusted layer)
+      // (no room to record this round's children, or no epoch left whose tag cannot alias: start over with one
+      // trusted layer)
+      else if (n_lay >= LL_LAYERS || epoch == prm.epoch_last)
         ex = RND_EXIT_RELAUNCH;
     }
     if (ex < 0) {
@@ -453,7 +467,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         sm.plan.len0 = geo_len0;
         sm.plan.a1 = geo_a1;
         sm.plan.len1 = geo_len1;
-        sm.plan.epoch = epoch;
+        sm.plan.tag = ll_tag(epoch);
         sm.plan.top = n_lay - 1;
       }
     }
@@ -464,7 +478,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
   if (wid == T / 32) {
     if (lane == 0) {
       sm.lay_start[0] = 0;
-      sm.lay_epoch[0] = LL_TRUSTED;
+      sm.lay_tag[0] = LL_TRUSTED;
       sm.poll_abort = 0;
       if (prof_x)
         for (int i = 0; i < LL_PROF_N; i++) sm.prof[i] = 0;
@@ -520,7 +534,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         if (round_children > 0) {
           if (lane == 0) {
             sm.lay_start[nl] = chunk_s0;
-            sm.lay_epoch[nl] = epoch;
+            sm.lay_tag[nl] = ll_tag(epoch);
           }
           ++nl;
           below = chunk_s0;
@@ -529,6 +543,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         lay_top = below;
         // ---- (9) the pool after the round, and the next round's chunk
         size = chunk_s0 + round_children;
+        size_hi = size > size_hi ? size : size_hi;
         ++rounds;
         tot_parents += static_cast<unsigned long long>(chunk_n);
         tot_children += static_cast<unsigned long long>(round_children);
@@ -548,7 +563,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       if (sm.plan.exit >= 0) break;
       const long long s0 = sm.plan.s0;
       const int a0 = sm.plan.a0, len0 = sm.plan.len0, a1 = sm.plan.a1, len1 = sm.plan.len1;
-      const unsigned round_epoch = sm.plan.epoch;
+      const unsigned round_tag = sm.plan.tag;
       const int top = sm.plan.top;
       const int len = len0 + len1;
       bool ok = true;
@@ -556,7 +571,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
 
       // ---- (2) my slice -> shared memory, 16-byte piece by piece (2 pieces per node, consecutive lanes on
       // consecutive pieces: every warp load is 512 contiguous bytes); a piece is polled until both of its words
-      // carry the epoch of the layer its node lies in
+      // carry the tag of the layer its node lies in
       {
         SpinGuard guard;
         const unsigned long long* src0 = fat[s0 + a0].w;
@@ -567,12 +582,12 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
 #pragma unroll
         for (int j = 0; j < PCS; j++)
           if (t + j * T < 2 * len) pending |= 1u << j;
-        // the epoch node i of my slice was stored with: that of the layer its position lies in (mostly the top one)
+        // the tag node i of my slice was stored with: that of the layer its position lies in (mostly the top one)
         const auto want_of = [&](int i) {
           const long long pos = s0 + (i < len0 ? a0 + i : a1 + (i - len0));
           int L = top;
           while (L > 0 && sm.lay_start[L] > pos) --L;
-          return sm.lay_epoch[L];
+          return sm.lay_tag[L];
         };
         while (pending) {
           // all loads of a sweep are issued back to back (a dependent re-poll per piece would serialise 8 L2 round
@@ -588,10 +603,11 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
             if (pending & (1u << j)) {
               const int pc = t + j * T, i = pc >> 1;
               const unsigned want = want_of(i);
-              if (want == LL_TRUSTED ||
-                  (static_cast<unsigned>(w0[j] >> 32) == want && static_cast<unsigned>(w1[j] >> 32) == want)) {
+              const uint32_t h0 = static_cast<uint32_t>(w0[j] >> 32), h1 = static_cast<uint32_t>(w1[j] >> 32);
+              if (want == LL_TRUSTED || __byte_perm(h0, h1, 0x7632) == want * 0x10001u) {  // (both tags)
                 reinterpret_cast<uint2*>(&sm.parent[i])[pc & 1] =
                     make_uint2(static_cast<uint32_t>(w0[j]), static_cast<uint32_t>(w1[j]));
+                reinterpret_cast<uint32_t*>(&sm.diag[i])[pc & 1] = __byte_perm(h0, h1, 0x5410);  // ld or rd
                 pending &= ~(1u << j);
               }
             }
@@ -607,7 +623,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         break;
       }
       uint32_t cm[LL_PPT];
-      int leaves = 0, mine = 0, mine0 = 0, fert = 0;
+      int leaves = 0, mine = 0, mine0 = 0;
 #pragma unroll
       for (int q = 0; q < LL_PPT; q++) {
         const int i = LL_PPT * t + q;
@@ -618,15 +634,13 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
           leaves += (w3 & LL_LEAF) ? 1 : 0;
           mine += __popc(cm[q]);
           if (i < len0) mine0 += __popc(cm[q]);
-          fert += cm[q] != 0u ? 1 : 0;
         }
       }
       TSB_PROF(prof_w, 0, LL_PROF_POLL)
-      // ---- (3) block scan: children | leaves << 20 | children of the bottom sub-slice << 32 | parents with
-      // children << 52 (at most 13 056, 768, 13 056 and 768 per CTA: no field overflows into the next)
+      // ---- (3) block scan: children | leaves << 20 | children of the bottom sub-slice << 32 (at most 13 056, 768
+      // and 13 056 per CTA: no field overflows into the next)
       unsigned long long incl = static_cast<unsigned long long>(mine) | static_cast<unsigned long long>(leaves) << 20 |
-                                static_cast<unsigned long long>(mine0) << 32 |
-                                static_cast<unsigned long long>(fert) << 52;
+                                static_cast<unsigned long long>(mine0) << 32;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
         const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
@@ -645,11 +659,9 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       const int cnt0 = static_cast<int>(tot >> 32 & 0xFFFFF);
       {
         uint16_t* it = sm.item + (static_cast<int>((woff + incl) & 0xFFFFF) - mine);
-        uint16_t* f = sm.fertile + 32 * LL_PPT * wid + (static_cast<int>(incl >> 52) - fert);  // (my warp's list)
 #pragma unroll
         for (int q = 0; q < LL_PPT; q++) {
           uint32_t m = cm[q];
-          if (m) *f++ = static_cast<uint16_t>(LL_PPT * t + q);
           while (m) {
             const int s = __ffs(m) - 1;
             m &= m - 1;
@@ -657,30 +669,12 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
           }
         }
       }
-      // ---- (5) the diagonals of the parents with children (the counts are on their way meanwhile; ll_build_child
-      // reads no others: about a third of the parents have none).  Each warp takes its own list, all loads first: a
-      // list of the whole CTA costs one more CTA barrier and measured slower (DESIGN §5).
-      __syncwarp();  // (my warp's list is complete)
-      const int n_fert = static_cast<int>(__shfl_sync(0xFFFFFFFFu, incl, 31) >> 52);
-      const uint16_t* const fl = sm.fertile + 32 * LL_PPT * wid;
-      // (DG parents side by side: three do not fit the 96 registers a thread has at two CTAs per SM at N >= 19, nor,
-      // as ptxas allocates them, at N <= 5)
-      constexpr int DG = N >= 19 || N <= 5 ? 2 : LL_PPT;
-#pragma unroll
-      for (int q0 = 0; q0 < LL_PPT; q0 += DG) {
-        uint4 p[DG];
-#pragma unroll
-        for (int q = q0; q < q0 + DG && q < LL_PPT; q++)
-          if (lane + 32 * q < n_fert) p[q - q0] = sm.parent[fl[lane + 32 * q]];
-#pragma unroll
-        for (int q = q0; q < q0 + DG && q < LL_PPT; q++)
-          if (lane + 32 * q < n_fert) sm.diag[fl[lane + 32 * q]] = ll_parent_diag<N>(p[q - q0]);
-      }
-      ll_bar(T);  // items and diagonals complete
+      ll_bar(T);  // items complete
       TSB_PROF(prof_w, 0, LL_PROF_SCAN)
-      // ---- (5b) my children (first window), built and evaluated while the other CTAs' counts are on their way
+      // ---- (5) my children (first window), built and evaluated while the other CTAs' counts are on their way
       auto build_window = [&](int c0, int cnt) {
-        for (int c = t; c < cnt; c += T) sm.stage[c] = ll_build_child<N>(sm.parent, sm.diag, sm.item[c0 + c]);
+        for (int c = t; c < cnt; c += T)
+          sm.stage[c] = ll_build_child<N>(sm.parent, sm.diag, sm.item[c0 + c], &sm.stage_diag[c]);
       };
       build_window(0, min(LL_CAP, my_children));
       TSB_PROF(prof_w, 0, LL_PROF_BUILD)
@@ -689,9 +683,8 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       TSB_PROF(prof_w, 0, LL_PROF_HAND)
       const int off0 = sm.plan.off0, off1 = sm.plan.off1;
 
-      // ---- (7) my children, in place, tagged with this round's epoch (every slice of the chunk has been read: all
-      // 2G slots carried this epoch)
-      const unsigned long long tag = static_cast<unsigned long long>(round_epoch) << 32;
+      // ---- (7) my children, in place, tagged with this round's tag (every slice of the chunk has been read: all
+      // 2G slots carried this round's epoch)
       for (int c0 = 0; c0 < my_children; c0 += LL_CAP) {
         const int cnt = min(LL_CAP, my_children - c0);
         if (c0 > 0) {
@@ -705,28 +698,34 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         const int npc = 2 * cnt;  // 16-byte pieces, consecutive lanes on consecutive pieces, four in flight per thread
         for (int pc = t; pc < npc; pc += 4 * T) {
           uint2 d[4];
+          uint32_t dm[4];
 #pragma unroll
           for (int u = 0; u < 4; u++) {
             const int x = min(pc + u * T, npc - 1);
             d[u] = reinterpret_cast<const uint2*>(&sm.stage[x >> 1])[x & 1];
+            dm[u] = reinterpret_cast<const uint32_t*>(&sm.stage_diag[x >> 1])[x & 1];  // ld or rd
           }
 #pragma unroll
           for (int u = 0; u < 4; u++) {
             const int x = pc + u * T;
-            if (x < npc) st_fat2((c0 + (x >> 1) < cnt0 ? dst0 : dst1) + 2 * x, d[u].x | tag, d[u].y | tag);
+            unsigned long long a, b;
+            ll_piece(d[u].x, d[u].y, dm[u], round_tag, a, b);
+            if (x < npc) st_fat2((c0 + (x >> 1) < cnt0 ? dst0 : dst1) + 2 * x, a, b);
           }
         }
       }
       TSB_PROF(prof_w, 0, LL_PROF_STORE)
       // (straight into the next round: sm.plan holds its geometry since the handoff.  No worker barrier is needed
-      // before the next poll overwrites sm.parent: every build of this round ended before a barrier all workers
-      // passed, and sm.stage is next written after the next poll's barrier, when every store has read it.)
+      // before the next poll overwrites sm.parent and sm.diag: every build of this round ended before a barrier all
+      // workers passed, and sm.stage and sm.stage_diag are next written after the next poll's barrier, when every
+      // store has read them.)
     }
   }
   __syncthreads();  // (all CTA threads leave the loop at the same round; the profile is complete)
   if (k == 0 && t == T) {
     RoundsState* st = prm.state;
     st->size = size;
+    st->size_hi = size_hi;
     st->epoch = epoch;
     st->rounds = rounds;
     st->parents = tot_parents;

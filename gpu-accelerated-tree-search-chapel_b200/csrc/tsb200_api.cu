@@ -838,6 +838,10 @@ struct tsb_nq : Base {
   tsb::FatNode* d_fat = nullptr;  // the pool in the self-validating 32-byte format, while the LL kernel owns it
   long long fat_cap = 0;
   bool in_fat = false;  // the pool currently lives in d_fat (the plain arena is stale)
+  // 16-bit tags of d_fat (nq_rounds_ll.cuh): the epoch of its last clear, and the highest pool size since then (every
+  // word at or above it carries tag 0)
+  unsigned tag_clear = 0;
+  long long tag_hi = 0;
 };
 
 struct tsb_pfsp : Base {
@@ -972,7 +976,7 @@ int nq_fat_import(tsb_nq* h) {
   const long long size = h->pool.size;
   if (size > 0) {
     tsb::nq_fat_import_kernel<N><<<static_cast<unsigned>((size + 255) / 256), 256, 0, h->stream>>>(
-        h->pool.arena[h->pool.cur], h->d_fat, size, h->rounds.epoch);
+        h->pool.arena[h->pool.cur], h->d_fat, size);
     TSB_CUDA(cudaGetLastError());
     h->launches++;
   }
@@ -985,6 +989,27 @@ int nq_ensure_fat(tsb_nq* h, long long cap) {
   h->fat_cap = 0;
   TSB_CUDA(cudaMalloc(&h->d_fat, static_cast<size_t>(cap) * sizeof(tsb::FatNode)));
   h->fat_cap = cap;
+  // (a new arena starts cleared: tag 0 everywhere)
+  TSB_CUDA(cudaMemsetAsync(h->d_fat, 0, static_cast<size_t>(cap) * sizeof(tsb::FatNode), h->stream));
+  h->tag_clear = h->rounds.epoch;
+  h->tag_hi = 0;
+  return TSB_OK;
+}
+// the clear of d_fat's tags, if the next launch (at most max_rounds rounds) needs it; -> the last epoch it may use
+int nq_fat_tag_window(tsb_nq* h, int64_t max_rounds, unsigned* epoch_last, bool* queued) {
+  const tsb::LlTagWindow w = tsb::ll_tag_window(h->rounds.epoch, h->tag_clear, max_rounds);
+  if (w.clear) {
+    const long long words = h->tag_hi * tsb::LL_WORDS;
+    if (words > 0) {
+      tsb::nq_fat_clear_tags_kernel<<<static_cast<unsigned>((words + 255) / 256), 256, 0, h->stream>>>(h->d_fat, words);
+      TSB_CUDA(cudaGetLastError());
+      h->launches++;
+      *queued = true;
+    }
+    h->tag_clear = h->rounds.epoch;
+    h->tag_hi = 0;
+  }
+  *epoch_last = w.epoch_last;
   return TSB_OK;
 }
 // the pool back in the plain 21-byte arena (whoever needs the node records calls this first)
@@ -1050,6 +1075,7 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
       int rc = TSB_OK;
       if (h->in_fat && need > p.cap) rc = nq_materialize(h);  // (grows below and imports again)
       if (rc != TSB_OK) return rc;
+      bool queued = false;  // work on h's stream that the launch must follow
       if (!h->in_fat) {
         // room for the worst case of the next round
         rc = p.make_stack(h->stream, need);
@@ -1057,9 +1083,12 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
         if (rc == TSB_OK) rc = with_queens(h->N, [h](auto q) { return nq_fat_import<decltype(q)::value>(h); });
         if (rc != TSB_OK) return rc;
         h->in_fat = true;
-        if (n_act > 0) TSB_CUDA(cudaStreamSynchronize(h->stream));  // (the launch goes on the first pool's stream)
+        queued = true;
       }
       tsb::LlParams& prm = mp.pool[n_act];
+      rc = nq_fat_tag_window(h, left[i], &prm.epoch_last, &queued);
+      if (rc != TSB_OK) return rc;
+      if (queued && n_act > 0) TSB_CUDA(cudaStreamSynchronize(h->stream));  // (the launch goes on the first pool's stream)
       prm.fat = h->d_fat;
       prm.cap = std::min(p.cap, h->fat_cap);
       prm.size0 = p.size;
@@ -1091,10 +1120,11 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
       tsb::RoundsState st;
       rc = h->finish_launch("nq_rounds_ll_kernel", "a flag exchange or a node poll did not complete", &st, &out[4 * i]);
       if (rc != TSB_OK) return rc;
+      h->tag_hi = std::max(h->tag_hi, st.size_hi);
       if (prof) {
         const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
         std::fprintf(stderr, "[tsb200] LL rounds kernel (pool %d of %d): %llu rounds; CTA 0 cycles per round: workers: set-up %.0f "
-                     "poll-nodes %.0f scan+items+diag %.0f build %.0f handoff-wait %.0f store %.0f | exchange warp: "
+                     "poll-nodes %.0f scan+items %.0f build %.0f handoff-wait %.0f store %.0f | exchange warp: "
                      "scan-wait %.0f publish+gather %.0f bookkeeping %.0f handoff-wait %.0f\n", a, n_act,
                      static_cast<unsigned long long>(st.rounds), st.prof[tsb::LL_PROF_SETUP] / r, st.prof[tsb::LL_PROF_POLL] / r,
                      st.prof[tsb::LL_PROF_SCAN] / r, st.prof[tsb::LL_PROF_BUILD] / r, st.prof[tsb::LL_PROF_HAND] / r,
