@@ -29,20 +29,23 @@
 //       It is skipped when the next round's exit tests already end the launch (the kernel boundary orders them).
 // Every spin loop is guarded by SpinGuard: a stuck exchange ends the launch with RND_EXIT_ABORT (TSB_ECUDA on the
 // host), never a hung GPU.
+//
+// One launch serves up to PFR_MAX_POOLS INDEPENDENT pools (grid (G, pools), PfRoundsMultiParams): the CTAs with
+// blockIdx.y = i run pool i's rounds on pool i's arena, tables, exchange slots, state record and incumbent, and never
+// wait on another pool; each pool leaves on its own exit.  With several pools every SM hosts two CTAs (pfr_tiers.h),
+// so one pool's L2 round trips (count exchange, store exchange) are filled with another pool's bound work.  On an H100
+// (tools/pfsp_multi_pool.py, DESIGN §4.2) the shared launch beat the same pools run one after the other at every K and
+// M measured: 1.2-2.5x per pool-round, and two pools at M = 50 000 took 11.5-12.9 us per pool-round against 16.9-18.8
+// for the two-kernel rounds tsb_pfsp_pool_run takes there.
 #pragma once
 #include "nq_rounds_ll.cuh"  // SpinGuard, RoundsState, RND_EXIT_*
+#include "pfr_tiers.h"
 #include "pfsp_expand.cuh"
 
 namespace tsb {
 
-constexpr int PFR_TILES = 3;                     // tiles of 128 parents per CTA and round
-constexpr int PFR_SLICE = PFR_TILES * PF_TILE;   // parents per CTA and round
-constexpr int PFR_MAX_CTAS = 256;                // slots of the exchanges (PfRoundsSync)
-// largest chunk one launch takes on a GPU with `sms` SMs (one CTA per SM): 50 688 on a 132-SM H100, which covers the
-// reference's default --M 50000
-__host__ __device__ constexpr long long pf_rounds_capacity(int sms) {
-  return static_cast<long long>(sms < PFR_MAX_CTAS ? sms : PFR_MAX_CTAS) * PFR_SLICE;
-}
+constexpr int PFR_TILES = 3;  // tiles of 128 parents per CTA and round
+static_assert(PFR_TILES * PF_TILE == PFR_SLICE, "pfr_tiers.h");
 
 // largest M for which tsb_pfsp_pool_run takes this kernel.  On an H100 (ta014, lb1 and lb1_d, DESIGN §5) it beats the
 // loop of two-kernel rounds by 1.8x at M = 300 and 1.2x at M = 20 000, and loses at M = 50 000 (18.2 against 16.4 us per
@@ -71,7 +74,10 @@ struct PfRoundsParams {
   PfRoundsSync* sync;
   RoundsState* state;             // out: pool size, last epoch, exit code, counters of the committed rounds
 };
-// TSB200_ROUNDS_PROF phases (CTA 0, thread 0 cycles)
+struct PfRoundsMultiParams {
+  PfRoundsParams pool[PFR_MAX_POOLS];  // pool blockIdx.y
+};
+// TSB200_ROUNDS_PROF phases (CTA 0 of each pool, thread 0 cycles)
 enum { PFR_PROF_LOAD = 0, PFR_PROF_BOUND, PFR_PROF_PUBLISH, PFR_PROF_GATHER, PFR_PROF_STORE, PFR_PROF_BARRIER, PFR_PROF_N };
 static_assert(PFR_PROF_N <= 12, "RoundsState::prof");
 
@@ -102,8 +108,10 @@ __device__ __forceinline__ void st_relaxed_u32(unsigned* p, unsigned v) {
   asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
+// (two CTAs per SM: one of each of two pools; PfRoundsSmem fits twice)
 template <int KIND, int M, bool SIMD>
-__global__ void __launch_bounds__(PF_THREADS, 1) pfsp_rounds_kernel(const __grid_constant__ PfRoundsParams prm) {
+__global__ void __launch_bounds__(PF_THREADS, 2) pfsp_rounds_kernel(const __grid_constant__ PfRoundsMultiParams mprm) {
+  const PfRoundsParams& prm = mprm.pool[blockIdx.y];
   extern __shared__ __align__(128) uint8_t smem_raw[];
   PfRoundsSmem& sm = *reinterpret_cast<PfRoundsSmem*>(smem_raw);
   const int t = threadIdx.x, lane = t & 31, wid = t >> 5;

@@ -454,19 +454,28 @@ struct Base {
     if (cfg) *cfg = c;
     return TSB_OK;
   }
-  // persistent grid: enough CTAs to fill the GPU, never more than there are full tiles
+  // CTAs of `threads` threads and `smem` bytes of dynamic shared memory that one SM holds at once (at least 1)
   template <class K>
-  int grid_for(K kernel, int threads, size_t smem, long long count, int tile, int* grid) {
+  int per_sm(K kernel, int threads, size_t smem, int* n) {
     KernelConfig* c = nullptr;
     int rc = configure(kernel, smem, &c);
     if (rc != TSB_OK) return rc;
     if (c->per_sm <= 0) {
-      int per_sm = 0;
-      TSB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
-      c->per_sm = std::max(per_sm, 1);
+      int blocks = 0;
+      TSB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kernel, threads, smem));
+      c->per_sm = std::max(blocks, 1);
     }
+    *n = c->per_sm;
+    return TSB_OK;
+  }
+  // persistent grid: enough CTAs to fill the GPU, never more than there are full tiles
+  template <class K>
+  int grid_for(K kernel, int threads, size_t smem, long long count, int tile, int* grid) {
+    int n = 1;
+    int rc = per_sm(kernel, threads, smem, &n);
+    if (rc != TSB_OK) return rc;
     const long long tiles = std::max<long long>(1, count / tile);
-    *grid = static_cast<int>(std::min<long long>(tiles, static_cast<long long>(c->per_sm) * di.sms));
+    *grid = static_cast<int>(std::min<long long>(tiles, static_cast<long long>(n) * di.sms));
     return TSB_OK;
   }
 
@@ -845,6 +854,7 @@ struct tsb_nq : Base {
 };
 
 struct tsb_pfsp : Base {
+  tsb_pfsp* sibling[3] = {nullptr, nullptr, nullptr};  // further pools on the same device, owned by this handle (tsb_pfsp_sibling)
   int jobs = 0, machines = 0, pairs = 0, mt = 0;  // mt = template machine count (5, 10 or 20)
   tsb::PfspLb1Tables* d_tab1 = nullptr;
   tsb::Lb2Const* lb2c = nullptr;  // packed Johnson tables, passed to the lb2 kernels by value (constant bank)
@@ -1343,91 +1353,194 @@ int pfsp_plain() { return TSB_OK; }
 // CTAs of the persistent PFSP kernel for chunks of up to M parents (one per SM at most, each with up to PFR_SLICE
 // parents; fewer CTAs for smaller M, so that the two exchanges of a round involve only the CTAs that have parents to
 // evaluate); 0: the loop of tsb_pfsp_pool_step runs instead (lb2, M above PFR_MAX_M where the step loop is faster, M
-// beyond pf_rounds_capacity, no cooperative launch, env TSB200_NO_ROUNDS=1)
+// beyond pf_pool_capacity, no cooperative launch, env TSB200_NO_ROUNDS=1)
 int pfsp_rounds_grid(const tsb_pfsp* h, int lb_kind, int M) {
   if (lb_kind == TSB_LB2 || !h->di.coop || env_no_rounds()) return 0;
-  if (M > tsb::PFR_MAX_M || M > tsb::pf_rounds_capacity(h->di.sms)) return 0;
-  const int sms = std::min(h->di.sms, tsb::PFR_MAX_CTAS);
-  return static_cast<int>(std::min<long long>(sms, (static_cast<long long>(M) + tsb::PF_TILE - 1) / tsb::PF_TILE));
+  if (M > tsb::PFR_MAX_M || M > tsb::pf_pool_capacity(h->di.sms, 1)) return 0;
+  return static_cast<int>(std::min<long long>(tsb::pf_ctas_per_pool(h->di.sms, 1),
+                                              (static_cast<long long>(M) + tsb::PF_TILE - 1) / tsb::PF_TILE));
 }
-template <int KIND, int M>
-int pfsp_rounds_launch_km(tsb_pfsp* h, const tsb::PfRoundsParams& prm, int grid, cudaStream_t s) {
-  auto kernel = h->simd16 ? tsb::pfsp_rounds_kernel<KIND, M, true> : tsb::pfsp_rounds_kernel<KIND, M, false>;
-  const size_t smem = sizeof(tsb::PfRoundsSmem) + 128;
-  int rc = h->configure(kernel, smem);
-  if (rc != TSB_OK) return rc;
-  void* args[] = {const_cast<tsb::PfRoundsParams*>(&prm)};
-  // cooperative: every CTA co-resident (the exchanges wait for all of them), or the launch fails
-  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid), dim3(tsb::PF_THREADS), args, smem, s));
-  h->launches++;
-  return TSB_OK;
+// f(kernel): the persistent kernel of h's route for lb1 / lb1_d
+template <class F>
+int with_pfsp_rounds_kernel(const tsb_pfsp* h, int lb_kind, F&& f) {
+  return with_machines(h->mt, [&](auto mt) -> int {
+    constexpr int MT = decltype(mt)::value;
+    if (lb_kind == TSB_LB1) return h->simd16 ? f(tsb::pfsp_rounds_kernel<1, MT, true>) : f(tsb::pfsp_rounds_kernel<1, MT, false>);
+    return h->simd16 ? f(tsb::pfsp_rounds_kernel<0, MT, true>) : f(tsb::pfsp_rounds_kernel<0, MT, false>);
+  });
 }
-// Up to max_rounds rounds in launches of the persistent kernel; out[] += {rounds, parents, children, solutions}.  A
-// launch leaves when the pool holds fewer than m nodes, after its round budget, when the next round's worst case
-// does not fit the arena (it grows and the loop relaunches) or when a leaf of the chunk improves *best (that round
-// goes through tsb_pfsp_pool_step and its sequential rule, then the loop relaunches with the new incumbent).
-int pfsp_rounds_run(tsb_pfsp* h, int lb_kind, int m, int M, int grid, int64_t max_rounds, int64_t* best, uint64_t* out) {
-  DevicePool& p = h->pool;
-  int rc = h->rounds.ensure<tsb::PfRoundsSync>(h->stream);
-  if (rc != TSB_OK) return rc;
+constexpr size_t kPfRoundsSmem = sizeof(tsb::PfRoundsSmem) + 128;
+// CTAs per pool when one launch of the persistent kernel serves `pools` >= 2 pools with chunks of up to M parents
+// (pf_ctas_per_pool, fewer for small M as in pfsp_rounds_grid); 0: not in one launch (lb2, no cooperative launch, env
+// TSB200_NO_ROUNDS=1, M beyond pf_pool_capacity, or the kernel does not fit twice on an SM)
+int pfsp_multi_grid(tsb_pfsp* h, int lb_kind, int M, int pools) {
+  if (lb_kind == TSB_LB2 || !h->di.coop || env_no_rounds() || pools < 2 || pools > tsb::PFR_MAX_POOLS) return 0;
+  if (M > tsb::pf_pool_capacity(h->di.sms, pools)) return 0;
+  int per_sm = 0;
+  if (with_pfsp_rounds_kernel(h, lb_kind, [&](auto kernel) -> int {
+        return h->per_sm(kernel, tsb::PF_THREADS, kPfRoundsSmem, &per_sm);
+      }) != TSB_OK || per_sm < 2) {
+    (void)cudaGetLastError();
+    return 0;
+  }
+  return static_cast<int>(std::min<long long>(tsb::pf_ctas_per_pool(h->di.sms, pools),
+                                              (static_cast<long long>(M) + tsb::PF_TILE - 1) / tsb::PF_TILE));
+}
+int pfsp_rounds_launch(tsb_pfsp* h, int lb_kind, const tsb::PfRoundsMultiParams& prm, int grid, int pools, cudaStream_t s) {
+  return with_pfsp_rounds_kernel(h, lb_kind, [&](auto kernel) -> int {
+    int rc = h->configure(kernel, kPfRoundsSmem);
+    if (rc != TSB_OK) return rc;
+    void* args[] = {const_cast<tsb::PfRoundsMultiParams*>(&prm)};
+    // cooperative: every CTA of every pool co-resident (the exchanges wait for all of a pool's CTAs), or the launch fails
+    TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid, pools), dim3(tsb::PF_THREADS), args,
+                                         kPfRoundsSmem, s));
+    h->launches++;
+    return TSB_OK;
+  });
+}
+// Up to max_rounds rounds of EACH of the K pools (handles on one device, same route) in launches of the persistent
+// kernel that serve every pool that still has work: grid (G, pools).  out[4 i ..] += {rounds, parents, children,
+// solutions} of pool i, best[i] is pool i's incumbent.  A pool leaves a launch on its own: when it holds fewer than m
+// nodes, after its round budget, when its next round's worst case does not fit its arena (it grows and the pool goes
+// again) or when a leaf of its chunk improves best[i] (that round goes through tsb_pfsp_pool_step and its sequential
+// rule, then the pool goes again with the new incumbent).  The launch ends when every pool has left.  A pool that is
+// the only one left runs exactly as tsb_pfsp_pool_run runs it (pfsp_rounds_grid, or the loop of pool_step).
+int pfsp_rounds_run(tsb_pfsp* const* hs, int K, int lb_kind, int m, int M, int64_t max_rounds, int64_t* best, uint64_t* out) {
+  int64_t left[tsb::PFR_MAX_POOLS];
+  bool active[tsb::PFR_MAX_POOLS];
+  for (int i = 0; i < K; i++) {
+    left[i] = max_rounds;
+    active[i] = true;
+    int rc = hs[i]->rounds.ensure<tsb::PfRoundsSync>(hs[i]->stream);
+    if (rc != TSB_OK) return rc;
+  }
   const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
-  int64_t left = max_rounds;
-  while (left > 0 && p.size >= m) {
-    // room for the worst case of the next round
-    const long long n = std::min<long long>(p.size, M);
-    const long long need = p.size - n + n * h->jobs;
-    rc = p.make_stack(h->stream, need);
-    if (rc != TSB_OK) return rc;
-    tsb::PfRoundsParams prm;
-    std::memset(&prm, 0, sizeof(prm));
-    prm.arena = p.arena[p.cur];
-    prm.tables = h->d_tab1;
-    prm.cap = p.cap;
-    prm.size0 = p.size;
-    prm.max_rounds = left;
-    prm.epoch0 = h->rounds.epoch;
-    prm.m = m;
-    prm.M = M;
-    prm.best = clamp_best(*best);
-    prm.prof = prof;
-    prm.sync = h->rounds.sync<tsb::PfRoundsSync>();
-    prm.state = h->rounds.d_state;
-    h->rounds.h_state->exit_code = -1;
-    rc = with_machines(h->mt, [&](auto mt) {
-      constexpr int MT = decltype(mt)::value;
-      return lb_kind == TSB_LB1 ? pfsp_rounds_launch_km<1, MT>(h, prm, grid, h->stream)
-                                : pfsp_rounds_launch_km<0, MT>(h, prm, grid, h->stream);
-    });
-    if (rc != TSB_OK) return rc;
-    TSB_CUDA(cudaStreamSynchronize(h->stream));
-    tsb::RoundsState st;
-    rc = h->finish_launch("pfsp_rounds_kernel", "a count or store exchange did not complete", &st, out);
-    if (rc != TSB_OK) return rc;
-    if (prof) {
-      const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
-      std::fprintf(stderr, "[tsb200] PFSP rounds kernel: %llu rounds (exit %d); CTA 0 cycles per round: load %.0f bounds %.0f "
-                   "publish+items %.0f gather %.0f store %.0f store-exchange %.0f\n",
-                   static_cast<unsigned long long>(st.rounds), st.exit_code, st.prof[tsb::PFR_PROF_LOAD] / r,
-                   st.prof[tsb::PFR_PROF_BOUND] / r, st.prof[tsb::PFR_PROF_PUBLISH] / r, st.prof[tsb::PFR_PROF_GATHER] / r,
-                   st.prof[tsb::PFR_PROF_STORE] / r, st.prof[tsb::PFR_PROF_BARRIER] / r);
-    }
-    left -= static_cast<int64_t>(st.rounds);
-    if (st.exit_code == tsb::RND_EXIT_SPACE) {
-      if (st.rounds == 0 && need <= p.cap) return TSB_ENOMEM;  // (cannot happen: the arena was grown for `need`)
-    } else if (st.exit_code == tsb::PFR_EXIT_IMPROVED) {
-      int64_t np = 0;
-      uint64_t nc = 0, ns = 0;
-      rc = tsb_pfsp_pool_step(h, lb_kind, m, M, best, &np, &nc, &ns);
+  for (;;) {
+    tsb::PfRoundsMultiParams mp;
+    std::memset(&mp, 0, sizeof(mp));
+    int map[tsb::PFR_MAX_POOLS], n_act = 0;
+    long long need_of[tsb::PFR_MAX_POOLS];
+    for (int i = 0; i < K; i++) {
+      tsb_pfsp* h = hs[i];
+      DevicePool& p = h->pool;
+      if (!active[i] || p.size < m || left[i] <= 0) {
+        active[i] = false;
+        continue;
+      }
+      // room for the worst case of the next round
+      const long long n = std::min<long long>(p.size, M);
+      const long long need = p.size - n + n * h->jobs;
+      int rc = p.make_stack(h->stream, need);
       if (rc != TSB_OK) return rc;
-      out[0] += 1;
-      out[1] += static_cast<uint64_t>(np);
-      out[2] += nc;
-      out[3] += ns;
-      --left;
-    } else {
-      break;  // DONE or PAUSE
+      // (the launch goes on the first pool's stream: a pool_step round may still be storing on this one)
+      if (n_act > 0) TSB_CUDA(cudaStreamSynchronize(h->stream));
+      tsb::PfRoundsParams& prm = mp.pool[n_act];
+      prm.arena = p.arena[p.cur];
+      prm.tables = h->d_tab1;
+      prm.cap = p.cap;
+      prm.size0 = p.size;
+      prm.max_rounds = left[i];
+      prm.epoch0 = h->rounds.epoch;
+      prm.m = m;
+      prm.M = M;
+      prm.best = clamp_best(best[i]);
+      prm.prof = prof;
+      prm.sync = h->rounds.sync<tsb::PfRoundsSync>();
+      prm.state = h->rounds.d_state;
+      h->rounds.h_state->exit_code = -1;
+      need_of[n_act] = need;
+      map[n_act++] = i;
+    }
+    if (n_act == 0) break;
+    tsb_pfsp* h0 = hs[map[0]];
+    const int grid = n_act == 1 ? pfsp_rounds_grid(h0, lb_kind, M) : pfsp_multi_grid(h0, lb_kind, M, n_act);
+    if (grid == 0) {
+      if (n_act > 1) return TSB_EINVAL;  // (checked by the caller for K pools, and fewer pools fit a fortiori)
+      const int i = map[0];  // the last pool, at an M the persistent kernel leaves to two-kernel rounds
+      return step_loop(left[i], &out[4 * i], [&](int64_t* np, uint64_t* nc, uint64_t* ns) {
+        return tsb_pfsp_pool_step(h0, lb_kind, m, M, &best[i], np, nc, ns);
+      });
+    }
+    int rc = pfsp_rounds_launch(h0, lb_kind, mp, grid, n_act, h0->stream);
+    if (rc != TSB_OK) return rc;
+    TSB_CUDA(cudaStreamSynchronize(h0->stream));
+    for (int a = 0; a < n_act; a++) {
+      const int i = map[a];
+      tsb_pfsp* h = hs[i];
+      tsb::RoundsState st;
+      rc = h->finish_launch("pfsp_rounds_kernel", "a count or store exchange did not complete", &st, &out[4 * i]);
+      if (rc != TSB_OK) return rc;
+      if (prof) {
+        const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
+        std::fprintf(stderr, "[tsb200] PFSP rounds kernel (pool %d of %d): %llu rounds (exit %d); CTA 0 cycles per round: "
+                     "load %.0f bounds %.0f publish+items %.0f gather %.0f store %.0f store-exchange %.0f\n", a, n_act,
+                     static_cast<unsigned long long>(st.rounds), st.exit_code, st.prof[tsb::PFR_PROF_LOAD] / r,
+                     st.prof[tsb::PFR_PROF_BOUND] / r, st.prof[tsb::PFR_PROF_PUBLISH] / r, st.prof[tsb::PFR_PROF_GATHER] / r,
+                     st.prof[tsb::PFR_PROF_STORE] / r, st.prof[tsb::PFR_PROF_BARRIER] / r);
+      }
+      left[i] -= static_cast<int64_t>(st.rounds);
+      if (st.exit_code == tsb::RND_EXIT_SPACE) {
+        if (st.rounds == 0 && need_of[a] <= h->pool.cap) return TSB_ENOMEM;  // (cannot happen: the arena was grown for `need`)
+      } else if (st.exit_code == tsb::PFR_EXIT_IMPROVED) {
+        int64_t np = 0;
+        uint64_t nc = 0, ns = 0;
+        rc = tsb_pfsp_pool_step(h, lb_kind, m, M, &best[i], &np, &nc, &ns);
+        if (rc != TSB_OK) return rc;
+        out[4 * i] += 1;
+        out[4 * i + 1] += static_cast<uint64_t>(np);
+        out[4 * i + 2] += nc;
+        out[4 * i + 3] += ns;
+        --left[i];
+      } else {
+        active[i] = false;  // DONE or PAUSE
+      }
     }
   }
+  return TSB_OK;
+}
+// tsb_pfsp_pool_run of one pool, out[] += {rounds, parents, children, solutions}
+int pfsp_pool_run_one(tsb_pfsp* h, int lb_kind, int m, int M, int64_t max_rounds, int64_t* best, uint64_t* out) {
+  if (pfsp_rounds_grid(h, lb_kind, M) > 0) return pfsp_rounds_run(&h, 1, lb_kind, m, M, max_rounds, best, out);
+  // lb2, large chunks: one round = two kernels (tsb_pfsp_pool_step)
+  return step_loop(max_rounds, out, [&](int64_t* np, uint64_t* nc, uint64_t* ns) {
+    return tsb_pfsp_pool_step(h, lb_kind, m, M, best, np, nc, ns);
+  });
+}
+
+// a handle with h's device, M_max and tables (its route included) and an empty pool; the device tables are copied
+// device to device, so none of the arrays h was created from is needed
+int pfsp_clone(const tsb_pfsp* h, tsb_pfsp** out) {
+  tsb_pfsp* c = new (std::nothrow) tsb_pfsp();
+  if (!c) return TSB_ENOMEM;
+  c->jobs = h->jobs;
+  c->machines = h->machines;
+  c->pairs = h->pairs;
+  c->mt = h->mt;
+  c->simd16 = h->simd16;
+  c->pool.set_format(sizeof(tsb_pfsp_node), tsb::PF_TILE, 2, h->jobs, h->pool.default_cap);
+  auto copy = [&]() -> int {
+    int rc = c->init(h->device, h->M_max, sizeof(tsb_pfsp_node), static_cast<size_t>(h->jobs) * 4);
+    if (rc != TSB_OK) return rc;
+    TSB_CUDA(cudaMalloc(&c->d_tab1, sizeof(tsb::PfspLb1Tables)));
+    TSB_CUDA(cudaMemcpyAsync(c->d_tab1, h->d_tab1, sizeof(tsb::PfspLb1Tables), cudaMemcpyDeviceToDevice, c->stream));
+    if (h->lb2c) {
+      c->lb2c = new (std::nothrow) tsb::Lb2Const(*h->lb2c);
+      if (!c->lb2c) return TSB_ENOMEM;
+    }
+    if (h->lb2u) {
+      TSB_CUDA(cudaMalloc(&c->d_tabu, sizeof(tsb::Lb2TabU)));
+      TSB_CUDA(cudaMemcpyAsync(c->d_tabu, h->d_tabu, sizeof(tsb::Lb2TabU), cudaMemcpyDeviceToDevice, c->stream));
+      c->lb2u = new (std::nothrow) tsb::Lb2ConstU{c->d_tabu};
+      if (!c->lb2u) return TSB_ENOMEM;
+    }
+    TSB_CUDA(cudaStreamSynchronize(c->stream));
+    return TSB_OK;
+  };
+  if (const int rc = copy(); rc != TSB_OK) {
+    tsb_pfsp_destroy(c);
+    return rc;
+  }
+  *out = c;
   return TSB_OK;
 }
 
@@ -1986,6 +2099,10 @@ int tsb_pfsp_create_wide(tsb_pfsp** out, int device, int max_jobs, int jobs, int
 
 void tsb_pfsp_destroy(tsb_pfsp* h) {
   if (!h) return;
+  for (tsb_pfsp*& x : h->sibling) {
+    if (x) tsb_pfsp_destroy(x);
+    x = nullptr;
+  }
   h->fini();
   if (h->d_tab1) cudaFree(h->d_tab1);
   if (h->d_wtab) cudaFree(h->d_wtab);
@@ -2036,7 +2153,13 @@ int tsb_pfsp_set_xfer(tsb_pfsp* h, int mode) {
   h->xfer = mode;
   return TSB_OK;
 }
-uint64_t tsb_pfsp_kernel_launches(const tsb_pfsp* h) { return h ? h->launches : 0; }
+uint64_t tsb_pfsp_kernel_launches(const tsb_pfsp* h) {
+  if (!h) return 0;
+  uint64_t n = h->launches;
+  for (const tsb_pfsp* x : h->sibling)
+    if (x) n += x->launches;
+  return n;
+}
 void* tsb_pfsp_stream(const tsb_pfsp* h) { return h ? static_cast<void*>(h->stream) : nullptr; }
 
 uint64_t tsb_pfsp_slow_rounds(const tsb_pfsp* h) { return h ? h->slow_rounds : 0; }
@@ -2122,19 +2245,66 @@ int tsb_pfsp_pool_run(tsb_pfsp* h, int lb_kind, int m, int M, int64_t max_rounds
   *n_rounds = *n_parents = *n_children = *n_solutions = 0;
   TSB_CUDA(cudaSetDevice(h->device));
   uint64_t out[4] = {0, 0, 0, 0};
-  int rc;
-  if (const int grid = pfsp_rounds_grid(h, lb_kind, M); grid > 0) {
-    rc = pfsp_rounds_run(h, lb_kind, m, M, grid, max_rounds, best, out);
-  } else {  // lb2, large chunks: one round = two kernels (tsb_pfsp_pool_step)
-    rc = step_loop(max_rounds, out, [&](int64_t* np, uint64_t* nc, uint64_t* ns) {
-      return tsb_pfsp_pool_step(h, lb_kind, m, M, best, np, nc, ns);
-    });
-  }
+  const int rc = pfsp_pool_run_one(h, lb_kind, m, M, max_rounds, best, out);
   *n_rounds = out[0];
   *n_parents = out[1];
   *n_children = out[2];
   *n_solutions = out[3];
   return rc;
+}
+
+int tsb_pfsp_sibling(tsb_pfsp* h, int index, tsb_pfsp** sibling) {
+  if (h && h->wide) return TSB_EUNSUPPORTED;  // (the device pool exists for MAX_JOBS = 20 only)
+  if (!h || !sibling || index < 1 || index >= tsb::PFR_MAX_POOLS) return TSB_EINVAL;
+  if (!h->sibling[index - 1]) {
+    TSB_CUDA(cudaSetDevice(h->device));
+    int rc = pfsp_clone(h, &h->sibling[index - 1]);
+    if (rc != TSB_OK) return rc;
+  }
+  *sibling = h->sibling[index - 1];
+  return TSB_OK;
+}
+
+int tsb_pfsp_pools_per_launch(const tsb_pfsp* h, int lb_kind, int M) {
+  if (!h || h->wide || M < 1 || M > h->M_max) return 1;
+  // (const: what the occupancy query caches on the handle does not change what it computes)
+  tsb_pfsp* w = const_cast<tsb_pfsp*>(h);
+  if (cudaSetDevice(h->device) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return 1;
+  }
+  for (int pools = tsb::PFR_MAX_POOLS; pools > 1; pools--)
+    if (pfsp_multi_grid(w, lb_kind, M, pools) > 0) return pools;
+  return 1;
+}
+
+int tsb_pfsp_pool_run_multi(tsb_pfsp* const* handles, int n_pools, int lb_kind, int m, int M, int64_t max_rounds,
+                            int64_t* best, uint64_t* out) {
+  if (!handles || n_pools < 1 || n_pools > tsb::PFR_MAX_POOLS || lb_kind < 0 || lb_kind > 2 || m < 1 || M < 1 ||
+      max_rounds < 0 || !best || !out)
+    return TSB_EINVAL;
+  for (int i = 0; i < n_pools; i++) {
+    if (!handles[i]) return TSB_EINVAL;
+    if (handles[i]->wide) return TSB_EUNSUPPORTED;  // (the device pool exists for MAX_JOBS = 20 only)
+  }
+  const tsb_pfsp* h0 = handles[0];
+  for (int i = 0; i < n_pools; i++) {
+    const tsb_pfsp* h = handles[i];
+    if (M > h->M_max || h->device != h0->device || tsb_pfsp_route(h) != tsb_pfsp_route(h0)) return TSB_EINVAL;
+    for (int j = 0; j < i; j++)
+      if (handles[j] == h) return TSB_EINVAL;
+  }
+  if (lb_kind == TSB_LB2 && h0->pairs == 0) return TSB_EINVAL;
+  std::memset(out, 0, sizeof(uint64_t) * 4 * n_pools);
+  TSB_CUDA(cudaSetDevice(h0->device));
+  if (n_pools == 1 || pfsp_multi_grid(handles[0], lb_kind, M, n_pools) == 0) {  // one pool after the other
+    for (int i = 0; i < n_pools; i++) {
+      int rc = pfsp_pool_run_one(handles[i], lb_kind, m, M, max_rounds, &best[i], &out[4 * i]);
+      if (rc != TSB_OK) return rc;
+    }
+    return TSB_OK;
+  }
+  return pfsp_rounds_run(handles, n_pools, lb_kind, m, M, max_rounds, best, out);
 }
 
 }  // extern "C"

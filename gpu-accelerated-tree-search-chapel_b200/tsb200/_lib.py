@@ -108,6 +108,9 @@ SYMBOLS = {
     "tsb_pfsp_pool_step": (_i, [_vp, _i, _i, _i, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_u64), C.POINTER(_u64)]),
     "tsb_pfsp_pool_run": (_i, [_vp, _i, _i, _i, _i64, C.POINTER(_i64), C.POINTER(_u64), C.POINTER(_u64), C.POINTER(_u64),
                                C.POINTER(_u64)]),
+    "tsb_pfsp_pool_run_multi": (_i, [C.POINTER(_vp), _i, _i, _i, _i, _i64, C.POINTER(_i64), C.POINTER(_u64)]),
+    "tsb_pfsp_sibling": (_i, [_vp, _i, C.POINTER(_vp)]),
+    "tsb_pfsp_pools_per_launch": (_i, [_vp, _i, _i]),
     "tsb_pfsp_pool_drain": (_i, [_vp, _vp, _i64, C.POINTER(_i64)]),
     "tsb_pfsp_slow_rounds": (_u64, [_vp]),
     "tsb_pfsp_route": (_i, [_vp]),

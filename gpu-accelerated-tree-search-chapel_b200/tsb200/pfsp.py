@@ -53,10 +53,12 @@ class PfspEvaluator:
         else:
             check(lib().tsb_pfsp_create_from_tables(C.byref(self._h), device, M, C.byref(self.tables)), "tsb_pfsp_create")
 
+    _owner = None  # a sibling's handle belongs to the evaluator it came from
+
     def close(self):
-        if self._h:
+        if self._h and self._owner is None:
             lib().tsb_pfsp_destroy(self._h)
-            self._h = C.c_void_p()
+        self._h = C.c_void_p()
 
     __del__ = close
 
@@ -162,6 +164,24 @@ class PfspEvaluator:
               "tsb_pfsp_search_on")
         return st
 
+    def sibling(self, index: int) -> "PfspEvaluator":
+        """further device pool `index` (1..3) with this evaluator's tables, device and M (tsb_pfsp_sibling): the
+        same evaluator on every call; its handle belongs to this evaluator and is destroyed with it"""
+        sibs = self.__dict__.setdefault("_siblings", {})
+        h = C.c_void_p()
+        check(lib().tsb_pfsp_sibling(self._h, index, C.byref(h)), "tsb_pfsp_sibling")
+        if index not in sibs:
+            sib = PfspEvaluator.__new__(PfspEvaluator)
+            sib.__dict__.update(tables=self.tables, jobs=self.jobs, machines=self.machines, M=self.M, wide=self.wide,
+                                node_dtype=self.node_dtype, _h=h, _owner=self)
+            sibs[index] = sib
+        return sibs[index]
+
+    def pools_per_launch(self, lb, M: int) -> int:
+        """pools one launch of the persistent kernel can serve for chunks of M parents (tsb_pfsp_pools_per_launch)"""
+        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        return int(lib().tsb_pfsp_pools_per_launch(self._h, kind, M))
+
     def pool_steal_from(self, victim: "PfspEvaluator", m: int) -> int:
         got = C.c_int64(0)
         check(lib().tsb_pfsp_pool_steal(victim._h, self._h, m, C.byref(got)), "tsb_pfsp_pool_steal")
@@ -173,6 +193,20 @@ class PfspEvaluator:
         got = C.c_int64(0)
         check(lib().tsb_pfsp_pool_drain(self._h, out.ctypes.data, n, C.byref(got)), "tsb_pfsp_pool_drain")
         return out[: got.value].copy()
+
+
+def pfsp_pool_run_multi(evaluators, lb, m: int, M: int, bests, max_rounds: int = 2**62):
+    """up to max_rounds rounds of each evaluator's device pool, each with its own incumbent, in shared launches of the
+    persistent kernel (tsb_pfsp_pool_run_multi): [(rounds, parents, children, solutions, best_after)] per pool"""
+    kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+    K = len(evaluators)
+    if len(bests) != K:
+        raise ValueError("one incumbent per pool")
+    hs = (C.c_void_p * K)(*[ev._h for ev in evaluators])
+    b = (C.c_int64 * K)(*[int(x) for x in bests])
+    out = (C.c_uint64 * (4 * K))()
+    check(lib().tsb_pfsp_pool_run_multi(hs, K, kind, m, M, max_rounds, b, out), "tsb_pfsp_pool_run_multi")
+    return [tuple(int(out[4 * i + j]) for j in range(4)) + (int(b[i]),) for i in range(K)]
 
 
 def pfsp_search_device(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1) -> SearchStats:

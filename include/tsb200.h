@@ -255,6 +255,29 @@ int tsb_pfsp_pool_steal(tsb_pfsp* victim, tsb_pfsp* thief, int m, int64_t* n_sto
  * where the two-kernel rounds measured faster) or env TSB200_NO_ROUNDS=1: one tsb_pfsp_pool_step per round.  Totals over the rounds come back; argument checks as tsb_pfsp_pool_step, plus max_rounds >= 0. */
 int tsb_pfsp_pool_run(tsb_pfsp* h, int lb_kind, int m, int M, int64_t max_rounds, int64_t* best,
                       uint64_t* n_rounds, uint64_t* n_parents, uint64_t* n_children, uint64_t* n_solutions);
+/* The same for up to 4 INDEPENDENT pools served by ONE launch of the persistent kernel: the CTAs of pool i run pool
+ * i's rounds with pool i's tables and incumbent best[i], and never wait on another pool; with several pools every SM
+ * hosts two CTAs, so the L2 round trips of one pool's round are filled with another pool's work.  Each pool leaves
+ * the launch on its own (a round that improves best[i] is run through tsb_pfsp_pool_step on that handle, the other
+ * pools go on).  Pool i ends exactly where tsb_pfsp_pool_run(handles[i], lb_kind, m, M, max_rounds, &best[i], ...)
+ * alone would leave it: same rounds, counters, best[i], pool and tsb_pfsp_slow_rounds — the reference's multi-GPU
+ * split (pfsp_multigpu_chpl.chpl: D tasks, each with its own pool and incumbent) with several pools on one GPU.
+ * out[4 i .. 4 i + 3] = {rounds, parents, children, solutions} of pool i; max_rounds applies to each pool.  Handles:
+ * one device, pairwise distinct, equal tsb_pfsp_route (different instances may share a launch), M <= M_max
+ * (TSB_EINVAL otherwise; TSB_EUNSUPPORTED for a tsb_pfsp_create_wide handle).  The pools run one after the other
+ * through tsb_pfsp_pool_run for lb2, env TSB200_NO_ROUNDS=1, without cooperative launch, when the kernel does not fit
+ * twice on an SM, or when M is beyond the capacity of n_pools pools (see tsb_pfsp_pools_per_launch). */
+int tsb_pfsp_pool_run_multi(tsb_pfsp* const* handles, int n_pools, int lb_kind, int m, int M, int64_t max_rounds,
+                            int64_t* best, uint64_t* out);
+/* Further independent pools on h's device (index 1..3) with h's tables, route and M_max, created on first use (the
+ * same handle on later calls) and owned by `h` (destroyed with it; their launches are included in h's
+ * tsb_pfsp_kernel_launches count): what a driver groups with `h` in tsb_pfsp_pool_run_multi. */
+int tsb_pfsp_sibling(tsb_pfsp* h, int index, tsb_pfsp** sibling);
+/* How many pools one launch of the persistent kernel can serve for lb_kind and chunks of up to M parents on h's
+ * device: the most, at most 4, whose capacity holds M (csrc/pfr_tiers.h, pf_pool_capacity: 384 parents per CTA,
+ * 2 x #SMs / pools CTAs per pool; on a 132-SM H100 50 688 for 2 pools, 33 792 for 3, 25 344 for 4); 1 for lb2, for M
+ * beyond the capacity of two pools, or when the persistent kernel is not available. */
+int tsb_pfsp_pools_per_launch(const tsb_pfsp* h, int lb_kind, int M);
 int tsb_pfsp_register_host(tsb_pfsp* h, void* ptr, size_t bytes);
 int tsb_pfsp_unregister_host(tsb_pfsp* h, void* ptr);
 int tsb_pfsp_set_xfer(tsb_pfsp* h, int mode);
