@@ -32,6 +32,7 @@
 // never reads them (:137-138).  `g` repeats an idempotent AND in the reference (:115-118); the
 // result does not depend on it and the work is done once.
 #pragma once
+#include "xfer_route.h"
 #include "tsb_ptx.cuh"
 
 namespace tsb {
@@ -210,8 +211,9 @@ __global__ void __launch_bounds__(NQ_THREADS) nq_evaluate_kernel(const uint8_t* 
 
 // ---- small chunks (the reference's default --M 50000 is 97 tiles of 512 parents: two thirds of the SMs, each thread
 // working through four parents, behind a TMA pipeline set up for one tile): one parent per thread, 128 parents per
-// CTA, plain coalesced 16-byte loads and stores — the shortest path from launch to labels.  The chunk's tail reads
-// at most 15 bytes past the last record (as the TMA path does).
+// CTA, plain coalesced 16-byte loads and stores — the shortest path from launch to labels.  The last CTA's bytes past
+// its last whole 16-byte word are loaded one by one (nq_small_words, as the TMA path's partial tile): in zero-copy
+// mode `parents` is the caller's registered host array, and nothing past its last record may be read.
 __device__ __forceinline__ void nq_parent_words(const uint8_t* src, uint32_t (&P)[6]) {  // any byte alignment
   const uint32_t mis = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(src)) & 3u, a8 = mis * 8u;
   const uint32_t* sw = reinterpret_cast<const uint32_t*>(src - mis);
@@ -233,9 +235,10 @@ __global__ void __launch_bounds__(NQ_SMALL) nq_evaluate_small_kernel(const uint8
   const int p0 = blockIdx.x * NQ_SMALL;
   const int np = min(NQ_SMALL, count - p0);
   {
-    const uint4* src = reinterpret_cast<const uint4*>(parents + static_cast<size_t>(p0) * NQ_REC);  // 128 * 21 = 168 * 16
-    uint4* dst = reinterpret_cast<uint4*>(in);
-    for (int i = t; i < (np * NQ_REC + 15) / 16; i += NQ_SMALL) dst[i] = src[i];
+    const uint8_t* src = parents + static_cast<size_t>(p0) * NQ_REC;  // 128 * 21 = 168 * 16: 16-byte aligned
+    const int n16 = nq_small_words(np, NQ_REC);
+    for (int i = t; i < n16; i += NQ_SMALL) reinterpret_cast<uint4*>(in)[i] = reinterpret_cast<const uint4*>(src)[i];
+    for (int i = 16 * n16 + t; i < np * NQ_REC; i += NQ_SMALL) in[i] = src[i];
   }
   __syncthreads();
   if (t < np) {

@@ -17,6 +17,7 @@
 #include <type_traits>
 #include <vector>
 
+#include "xfer_route.h"
 #include "nq_expand.cuh"
 #include "nq_rounds_ll.cuh"
 #include "pfsp_expand.cuh"
@@ -384,6 +385,7 @@ struct Base {
   uint8_t *h_in = nullptr, *h_out = nullptr;  // pinned+mapped staging, used when the caller's arrays cannot be locked
   size_t in_rec = 0, out_rec = 0;
   HostRegistry reg;
+  int last_xfer = 0;  // TSB_XFER_ROUTE_* bits of the last host-buffer evaluate call
   uint64_t launches = 0;
   // fused expand (evaluate + generate_children on the device) and the device-resident pool
   ExpandCtx ex;
@@ -565,12 +567,10 @@ struct Base {
     // AUTO: zero-copy whenever the caller registered its arrays (tsb_*_register_host) and they are 16-byte
     // aligned (fastest at every chunk size in tools/xfer_sweep.py's comparison); otherwise copies, pipelined
     // when large, through the handle's pinned staging buffers for arrays that are not registered
-    const bool aligned = ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
-    const bool zc_ok = in_locked && out_locked && aligned && di.can_use_host_ptr;
-    int mode = xfer == TSB_XFER_AUTO ? (zc_ok ? TSB_XFER_ZEROCOPY : TSB_XFER_MEMCPY) : xfer;
-    if (mode == TSB_XFER_ZEROCOPY && !zc_ok) mode = TSB_XFER_MEMCPY;
+    last_xfer = tsb::xfer_route(xfer, in_locked, out_locked, reinterpret_cast<uintptr_t>(in),
+                                reinterpret_cast<uintptr_t>(out), di.can_use_host_ptr, count, pipe_min, pipe_chunk);
 
-    if (mode == TSB_XFER_ZEROCOPY) {
+    if (last_xfer & TSB_XFER_ROUTE_ZEROCOPY) {
       // the kernel's TMA engine pulls the chunk over PCIe and pushes the results back: one launch,
       // reads and writes overlap on the full-duplex link
       int rc = launch(static_cast<const uint8_t*>(in), static_cast<uint8_t*>(out), count, stream);
@@ -586,7 +586,7 @@ struct Base {
     }
     if (!in_locked) src = h_in;
     if (!out_locked) dst = h_out;
-    if (count >= pipe_min && count > pipe_chunk) {
+    if (last_xfer & TSB_XFER_ROUTE_PIPELINED) {
       // large chunk: sub-chunks alternate between two streams so that the upload of one overlaps the
       // download of the previous one (PCIe is full duplex) and the kernel of the one in between; the host
       // memcpy into the staging buffer of sub-chunk i+1 overlaps the device work of sub-chunk i
@@ -1881,6 +1881,7 @@ int tsb_nq_set_xfer(tsb_nq* h, int mode) {
   h->xfer = mode;
   return TSB_OK;
 }
+int tsb_nq_last_xfer(const tsb_nq* h) { return h ? h->last_xfer : TSB_EINVAL; }
 uint64_t tsb_nq_kernel_launches(const tsb_nq* h) {
   if (!h) return 0;
   uint64_t n = h->launches;
@@ -2153,6 +2154,7 @@ int tsb_pfsp_set_xfer(tsb_pfsp* h, int mode) {
   h->xfer = mode;
   return TSB_OK;
 }
+int tsb_pfsp_last_xfer(const tsb_pfsp* h) { return h ? h->last_xfer : TSB_EINVAL; }
 uint64_t tsb_pfsp_kernel_launches(const tsb_pfsp* h) {
   if (!h) return 0;
   uint64_t n = h->launches;

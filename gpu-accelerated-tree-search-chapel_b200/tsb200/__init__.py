@@ -12,6 +12,7 @@ arrays standing for the Chapel records.  There is no CPU fallback: without libts
 device every call raises.
 """
 from ._lib import (LB1, LB1_D, LB2, ROUTE_LB2, ROUTE_LB2U, ROUTE_MT_MASK, ROUTE_SIMD16, XFER_AUTO, XFER_MEMCPY,
+                   XFER_ROUTE_IN_STAGED, XFER_ROUTE_OUT_STAGED, XFER_ROUTE_PIPELINED, XFER_ROUTE_ZEROCOPY,
                    XFER_ZEROCOPY, PfspTables, PfspTables50, SearchStats, TsbError, check, lib)
 from .nqueens import (NQ_NODE_DTYPE, NQueensEvaluator, nqueens_search, nqueens_search_device,
                       nqueens_pool_run_multi, nqueens_search_device_part, nqueens_warmup)
@@ -23,4 +24,5 @@ __all__ = ["NQueensEvaluator", "PfspEvaluator", "nqueens_warmup", "nqueens_pool_
            "taillard_tables",
            "NQ_NODE_DTYPE", "PFSP_NODE_DTYPE", "PFSP_NODE50_DTYPE", "LB2_VARIANTS", "taillard_tables50", "LB_NAMES", "LB1", "LB1_D", "LB2", "TsbError", "lib", "check",
            "PfspTables", "PfspTables50", "SearchStats", "XFER_AUTO", "XFER_MEMCPY", "XFER_ZEROCOPY",
+           "XFER_ROUTE_ZEROCOPY", "XFER_ROUTE_PIPELINED", "XFER_ROUTE_IN_STAGED", "XFER_ROUTE_OUT_STAGED",
            "ROUTE_MT_MASK", "ROUTE_SIMD16", "ROUTE_LB2", "ROUTE_LB2U"]

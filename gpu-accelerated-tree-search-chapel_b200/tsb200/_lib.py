@@ -15,6 +15,8 @@ MAX_PAIRS = 190
 OK, EINVAL, ECUDA, ENOMEM, ENODEV, EALIGN, EUNSUPPORTED = 0, -1, -2, -3, -4, -5, -6
 LB1_D, LB1, LB2 = 0, 1, 2
 XFER_AUTO, XFER_MEMCPY, XFER_ZEROCOPY = 0, 1, 2
+# tsb_*_last_xfer: the route of the last host-buffer evaluate call
+XFER_ROUTE_ZEROCOPY, XFER_ROUTE_PIPELINED, XFER_ROUTE_IN_STAGED, XFER_ROUTE_OUT_STAGED = 1, 2, 4, 8
 # tsb_pfsp_route: template machine count in the low byte, and which kernel specialisations the handle uses
 ROUTE_MT_MASK, ROUTE_SIMD16, ROUTE_LB2, ROUTE_LB2U = 0xFF, 0x100, 0x200, 0x400
 
@@ -93,6 +95,7 @@ SYMBOLS = {
     "tsb_nq_unregister_host": (_i, [_vp, _vp]),
     "tsb_debug_flag_exchange": (_i, [_i, _i, _i, _i, C.POINTER(C.c_double)]),
     "tsb_nq_set_xfer": (_i, [_vp, _i]),
+    "tsb_nq_last_xfer": (_i, [_vp]),
     "tsb_nq_kernel_launches": (_u64, [_vp]),
     "tsb_pfsp_create": (_i, [C.POINTER(_vp), _i, _i, _i, _i, _pi32, _pi32, _pi32, _i, _pi32, _pi32, _pi32, _pi32, _pi32]),
     "tsb_pfsp_create_wide": (_i, [C.POINTER(_vp), _i, _i, _i, _i, _i, _pi32, _pi32, _pi32, _i, _pi32, _pi32, _pi32, _pi32, _pi32]),
@@ -117,6 +120,7 @@ SYMBOLS = {
     "tsb_pfsp_register_host": (_i, [_vp, _vp, C.c_size_t]),
     "tsb_pfsp_unregister_host": (_i, [_vp, _vp]),
     "tsb_pfsp_set_xfer": (_i, [_vp, _i]),
+    "tsb_pfsp_last_xfer": (_i, [_vp]),
     "tsb_pfsp_kernel_launches": (_u64, [_vp]),
     "tsb_taillard_nb_jobs": (_i, [_i]),
     "tsb_taillard_nb_machines": (_i, [_i]),

@@ -49,6 +49,13 @@ class NQueensEvaluator:
         return int(lib().tsb_nq_kernel_launches(self._h))
 
     @property
+    def last_xfer(self) -> int:
+        """route of the last evaluate call: XFER_ROUTE_ZEROCOPY | _PIPELINED | _IN_STAGED | _OUT_STAGED bits"""
+        r = int(lib().tsb_nq_last_xfer(self._h))
+        check(min(r, 0), "tsb_nq_last_xfer")
+        return r
+
+    @property
     def stream(self) -> int:
         """the handle's cudaStream_t (pool / expand / host-buffer entry points launch on it)"""
         return int(lib().tsb_nq_stream(self._h) or 0)

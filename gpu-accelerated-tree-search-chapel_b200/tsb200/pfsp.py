@@ -82,6 +82,13 @@ class PfspEvaluator:
     def kernel_launches(self) -> int:
         return int(lib().tsb_pfsp_kernel_launches(self._h))
 
+    @property
+    def last_xfer(self) -> int:
+        """route of the last evaluate call: XFER_ROUTE_ZEROCOPY | _PIPELINED | _IN_STAGED | _OUT_STAGED bits"""
+        r = int(lib().tsb_pfsp_last_xfer(self._h))
+        check(min(r, 0), "tsb_pfsp_last_xfer")
+        return r
+
     def evaluate_gpu(self, parents: np.ndarray, size: int, best: int, lb, bounds: np.ndarray) -> None:
         """evaluate_gpu(parents_d, size, best, lbound1_d, lbound2_d, bounds_d) of pfsp_gpu_chpl.chpl:257-270 with
         the copies of :384/:386; `size` = jobs * poolSize; lb is "lb1" | "lb1_d" | "lb2" or the int code"""
@@ -118,6 +125,15 @@ class PfspEvaluator:
         check(lib().tsb_pfsp_expand(self._h, kind, parents.ctypes.data, parents.shape[0], C.byref(b), out.ctypes.data,
                                     cap, C.byref(nc), C.byref(ns)), "tsb_pfsp_expand")
         return out[: nc.value].copy(), int(ns.value), int(b.value)
+
+    def expand_device(self, lb, parents_ptr: int, count: int, best: int, children_ptr: int, stream: int = 0):
+        """(n_children, n_solutions, best_after) of expand on device arrays (parents 16-byte aligned, children 8-byte
+        aligned), ordered on `stream` (0: the handle's stream)"""
+        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        nc, ns, b = C.c_uint64(0), C.c_uint64(0), C.c_int64(int(best))
+        check(lib().tsb_pfsp_expand_device(self._h, kind, parents_ptr, count, C.byref(b), children_ptr, C.byref(nc),
+                                           C.byref(ns), stream), "tsb_pfsp_expand_device")
+        return int(nc.value), int(ns.value), int(b.value)
 
     def pool_push(self, nodes: np.ndarray) -> None:
         assert nodes.dtype == PFSP_NODE_DTYPE and nodes.flags.c_contiguous

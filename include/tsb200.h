@@ -81,6 +81,16 @@ enum {
   TSB_XFER_MEMCPY = 1,  /* cudaMemcpyAsync of the live prefix, kernel, cudaMemcpyAsync back */
   TSB_XFER_ZEROCOPY = 2 /* the kernel's TMA engine reads/writes page-locked host memory over PCIe */
 };
+/* the route the last tsb_*_evaluate call took (tsb_nq_last_xfer / tsb_pfsp_last_xfer), a bit mask: zero-copy on the
+ * caller's registered arrays, or copies, split over two streams for large chunks, through the handle's pinned
+ * staging buffers for an array that is not registered (0: one stream, both arrays registered, but not both 16-byte
+ * aligned or TSB_XFER_MEMCPY) */
+enum {
+  TSB_XFER_ROUTE_ZEROCOPY = 1,
+  TSB_XFER_ROUTE_PIPELINED = 2,
+  TSB_XFER_ROUTE_IN_STAGED = 4,
+  TSB_XFER_ROUTE_OUT_STAGED = 8
+};
 
 const char* tsb_strerror(int code);
 const char* tsb_last_cuda_error(void); /* thread-local text of the last failing CUDA call */
@@ -125,6 +135,8 @@ int tsb_nq_evaluate_device(tsb_nq* h, const void* parents_d, int count, uint8_t*
  * smaller than the actual number, TSB_ENOMEM is returned with the counts set.  Synchronous. */
 int tsb_nq_expand(tsb_nq* h, const void* parents, int count, void* children, uint64_t capacity_nodes,
                   uint64_t* n_children, uint64_t* n_solutions);
+/* the device-resident form: ordered on `stream` (NULL = the handle's stream), synchronous; writes exactly the
+ * n_children nodes at children_d (room for count*N nodes covers every chunk) */
 int tsb_nq_expand_device(tsb_nq* h, const void* parents_d /*16-B aligned*/, int count,
                          void* children_d /*any alignment*/, uint64_t* n_children, uint64_t* n_solutions,
                          void* stream);
@@ -176,10 +188,14 @@ int tsb_nq_sibling(tsb_nq* h, int index, tsb_nq** sibling);
 int tsb_nq_pools_per_launch(const tsb_nq* h, int M);
 
 /* page-lock + map a caller-owned host array for the lifetime of the handle (see the header comment);
- * TSB_EINVAL if the range partly overlaps a registered one / was not registered */
+ * TSB_EINVAL if the range partly overlaps a registered one / was not registered.  Registering a range inside a
+ * registered one does nothing; disjoint arrays that share a page may both be registered; unregister takes the
+ * pointer the range was registered with. */
 int tsb_nq_register_host(tsb_nq* h, void* ptr, size_t bytes);
 int tsb_nq_unregister_host(tsb_nq* h, void* ptr);
 int tsb_nq_set_xfer(tsb_nq* h, int mode);
+/* TSB_XFER_ROUTE_* bits of the last tsb_nq_evaluate call with count > 0 (0 before the first), TSB_EINVAL for NULL */
+int tsb_nq_last_xfer(const tsb_nq* h);
 uint64_t tsb_nq_kernel_launches(const tsb_nq* h); /* kernels launched through this handle so far */
 void* tsb_nq_stream(const tsb_nq* h); /* the handle's cudaStream_t: the pool / expand / host-buffer entry points launch
                                         * on it (to bracket them with CUDA events) */
@@ -235,6 +251,8 @@ int tsb_pfsp_evaluate_device(tsb_pfsp* h, int lb_kind, const void* parents_d, in
  * *n_solutions = evaluated leaf children (:283-288).  children come back packed, reference order. */
 int tsb_pfsp_expand(tsb_pfsp* h, int lb_kind, const void* parents, int count, int64_t* best, void* children,
                     uint64_t capacity_nodes, uint64_t* n_children, uint64_t* n_solutions);
+/* children_d must have room for count * jobs nodes: a round redone by the sequential rule (a leaf improved *best) has
+ * first written the launch-value children there, so past the n_children it returns its content is unspecified */
 int tsb_pfsp_expand_device(tsb_pfsp* h, int lb_kind, const void* parents_d /*16-B aligned*/, int count,
                            int64_t* best, void* children_d /*8-B aligned*/, uint64_t* n_children,
                            uint64_t* n_solutions, void* stream);
@@ -281,6 +299,7 @@ int tsb_pfsp_pools_per_launch(const tsb_pfsp* h, int lb_kind, int M);
 int tsb_pfsp_register_host(tsb_pfsp* h, void* ptr, size_t bytes);
 int tsb_pfsp_unregister_host(tsb_pfsp* h, void* ptr);
 int tsb_pfsp_set_xfer(tsb_pfsp* h, int mode);
+int tsb_pfsp_last_xfer(const tsb_pfsp* h); /* as tsb_nq_last_xfer, for tsb_pfsp_evaluate */
 uint64_t tsb_pfsp_kernel_launches(const tsb_pfsp* h);
 void* tsb_pfsp_stream(const tsb_pfsp* h);
 uint64_t tsb_pfsp_slow_rounds(const tsb_pfsp* h); /* expand rounds redone on the host because a leaf improved best */
