@@ -43,9 +43,11 @@ int main(int argc, char** argv) {
   std::printf("\nInitial search on CPU completed\nElapsed time: %f [s]\n\nSearch on GPU completed\n"
               "Elapsed time: %f [s]\n\nSearch on CPU completed\nElapsed time: %f [s]\n\nExploration terminated.\n",
               st.t_step1, st.t_step2, st.t_step3);
-  if (D > 1) {
+  if (D > 1) {  // shares of the step-2 tree, as nqueens_multigpu_chpl.chpl:337 divides (exploredTree - res1[1])
+    uint64_t step2 = 0;
+    for (int i = 0; i < D; i++) step2 += st.per_gpu_tree[i];
     std::printf("workload per GPU:");
-    for (int i = 0; i < D; i++) std::printf(" %.2f", 100.0 * st.per_gpu_tree[i] / (double)st.explored_tree);
+    for (int i = 0; i < D; i++) std::printf(" %.2f", step2 ? 100.0 * st.per_gpu_tree[i] / (double)step2 : 0.0);
     std::printf("\nsteals between device pools: %llu\n", (unsigned long long)st.steals);
   }
   const double t = st.t_step1 + st.t_step2 + st.t_step3;

@@ -57,6 +57,9 @@ class SearchResult(C.Structure):
         ("live_slots", C.c_uint64),
         ("depth_hist", C.c_uint64 * (MAX_JOBS + 2)),
         ("seconds", C.c_double),
+        ("task_tree", C.c_uint64 * 8),
+        ("task_sol", C.c_uint64 * 8),
+        ("task_best", C.c_int64 * 8),
     ]
 
 
@@ -106,6 +109,8 @@ def lib() -> C.CDLL:
         L.or_nq_search_offload.argtypes = [i32, i32, i32, i32, i32, C.POINTER(SearchResult)]
         L.or_pfsp_search_seq.argtypes = [i32, i32, i32, i32, C.POINTER(SearchResult)]
         L.or_pfsp_search_offload.argtypes = [i32, i32, i32, i32, i32, i32, i32, C.POINTER(SearchResult)]
+        L.or_nq_search_offload_part.argtypes = [i32, i32, i32, i32, i32, i32, i32, C.POINTER(SearchResult)]
+        L.or_pfsp_search_offload_part.argtypes = [i32, i32, i32, i32, i32, i32, i32, i32, C.POINTER(SearchResult)]
         L.or_nq_capture_chunk.argtypes = [i32, i32, i32, i32, i32, vp, i32]
         L.or_pfsp_capture_chunk.argtypes = [i32, i32, i32, i32, i32, i32, vp, i32, C.POINTER(C.c_int64)]
         _lib = L
@@ -208,6 +213,27 @@ def pfsp_search_seq(inst, lb_kind, ub=1, heads_mode=0):
 def pfsp_search_offload(inst, lb_kind, ub=1, m=25, M=50000, D=1, heads_mode=0):
     r = SearchResult()
     lib().or_pfsp_search_offload(inst, lb_kind, ub, m, M, D, heads_mode, C.byref(r))
+    return r
+
+
+def _check_part(D, part):
+    if not (1 <= D <= 8 and 0 <= part < D):
+        raise ValueError(f"part {part} of a {D}-way split")
+
+
+def nq_search_offload_part(N, g=1, m=25, M=50000, D=1, part=0, warm=None):
+    """task `part` of the D-way split run alone (or_nq_search_offload_part); warm: the step-1 pool size, D * m by
+    default"""
+    _check_part(D, part)
+    r = SearchResult()
+    lib().or_nq_search_offload_part(N, g, m, M, D, part, D * m if warm is None else warm, C.byref(r))
+    return r
+
+
+def pfsp_search_offload_part(inst, lb_kind, ub=1, m=25, M=50000, D=1, part=0, heads_mode=0):
+    _check_part(D, part)
+    r = SearchResult()
+    lib().or_pfsp_search_offload_part(inst, lb_kind, ub, m, M, D, part, heads_mode, C.byref(r))
     return r
 
 

@@ -650,9 +650,19 @@ static void nq_offload_loop(int N, int g, int m, int M, or_pool* pool, or_search
   }
 }
 
+/* step-2 counts of task `gpu`: what the task added to r since `tree0` / `sol0` */
+static void note_task(or_search_result* r, int gpu, uint64_t tree0, uint64_t sol0, int64_t best) {
+  if (gpu < 0 || gpu >= 8) return;
+  r->task_tree[gpu] = r->tree - tree0;
+  r->task_sol[gpu] = r->sol - sol0;
+  r->task_best[gpu] = best;
+}
+
 /* nqueens_gpu_chpl.chpl:152-248 (D == 1) and nqueens_multigpu_chpl.chpl:158-352 (D > 1,
- * static strided split :199-226, no work stealing — counts are split-invariant) */
-static void nq_search_offload_impl(int N, int g, int m, int M, int D, or_search_result* r, capture_t* cap) {
+ * static strided split :199-226, no work stealing — counts are split-invariant).  part >= 0: that task alone
+ * (or_nq_search_offload_part); warm: the step-1 pool size */
+static void nq_search_offload_impl(int N, int g, int m, int M, int D, int part, int64_t warm, or_search_result* r,
+                                   capture_t* cap) {
   memset(r, 0, sizeof(*r));
   or_pool pool;
   pool_init(&pool, sizeof(or_nq_node));
@@ -664,13 +674,16 @@ static void nq_search_offload_impl(int N, int g, int m, int M, int D, or_search_
   const double t0 = now_s();
 
   /* step 1 */
-  while (pool.size < (int64_t)D * m) {
+  while (pool.size < warm) {
     if (!pool_pop_front(&pool, &parent)) break;
     nq_decompose(N, g, &parent, &r->tree, &r->sol, &pool);
   }
+  if (part > 0) r->tree = r->sol = 0; /* step 1 is credited to part 0 */
   /* step 2 */
   if (D <= 1) {
+    const uint64_t tree0 = r->tree, sol0 = r->sol;
     nq_offload_loop(N, g, m, M, &pool, r, parents, labels, cap);
+    note_task(r, 0, tree0, sol0, 0);
   } else {
     const int64_t poolSize = pool.size, c = poolSize / D, l = poolSize - (int64_t)(D - 1) * c, f = pool.front;
     pool.front = 0;
@@ -685,8 +698,12 @@ static void nq_search_offload_impl(int N, int g, int m, int M, int D, or_search_
           pool_push_back(&multi[gpu], pool.elements + (size_t)(D * c + f + i) * pool.elt);
     }
     for (int gpu = 0; gpu < D; gpu++) {
-      nq_offload_loop(N, g, m, M, &multi[gpu], r, parents, labels, NULL);
-      while (pool_pop_back(&multi[gpu], &parent)) pool_push_back(&pool, &parent); /* :315-320 */
+      if (part < 0 || gpu == part) { /* a part leaves the other tasks' nodes to the other parts */
+        const uint64_t tree0 = r->tree, sol0 = r->sol;
+        nq_offload_loop(N, g, m, M, &multi[gpu], r, parents, labels, NULL);
+        note_task(r, gpu, tree0, sol0, 0);
+        while (pool_pop_back(&multi[gpu], &parent)) pool_push_back(&pool, &parent); /* :315-320 */
+      }
       pool_free(&multi[gpu]);
     }
     free(multi);
@@ -700,13 +717,17 @@ static void nq_search_offload_impl(int N, int g, int m, int M, int D, or_search_
 }
 
 void or_nq_search_offload(int N, int g, int m, int M, int D, or_search_result* r) {
-  nq_search_offload_impl(N, g, m, M, D, r, NULL);
+  nq_search_offload_impl(N, g, m, M, D, -1, (int64_t)D * m, r, NULL);
+}
+
+void or_nq_search_offload_part(int N, int g, int m, int M, int D, int part, int warm, or_search_result* r) {
+  nq_search_offload_impl(N, g, m, M, D, part, warm, r, NULL);
 }
 
 int or_nq_capture_chunk(int N, int g, int m, int M, int which, or_nq_node* out, int cap) {
   capture_t c = {which, out, cap, -1, 0, 0};
   or_search_result r;
-  nq_search_offload_impl(N, g, m, M, 1, &r, &c);
+  nq_search_offload_impl(N, g, m, M, 1, -1, m, &r, &c);
   return c.got;
 }
 
@@ -844,8 +865,9 @@ static void pfsp_offload_loop(const or_pfsp_tables* t, int lb_kind, int m, int M
 }
 
 /* pfsp_gpu_chpl.chpl:306-431 (D == 1); pfsp_multigpu_chpl.chpl:316-560 (D > 1: per-task best_l
- * starting from `best` :384, `min reduce` at the end :520, static split, no stealing) */
-static void pfsp_search_offload_impl(int inst, int lb_kind, int ub, int m, int M, int D, int heads_mode,
+ * starting from `best` :384, `min reduce` at the end :520, static split, no stealing).  part >= 0: that task
+ * alone (or_pfsp_search_offload_part), whose step 3 then runs with its own best_l */
+static void pfsp_search_offload_impl(int inst, int lb_kind, int ub, int m, int M, int D, int part, int heads_mode,
                                      or_search_result* r, capture_t* cap) {
   memset(r, 0, sizeof(*r));
   or_pfsp_tables* t = (or_pfsp_tables*)malloc(sizeof(*t));
@@ -869,8 +891,11 @@ static void pfsp_search_offload_impl(int inst, int lb_kind, int ub, int m, int M
     if (!pool_pop_front(&pool, &parent)) break;
     pfsp_decompose(t, lb_kind, &parent, &r->tree, &r->sol, &best, &pool);
   }
+  if (part > 0) r->tree = r->sol = 0; /* step 1 is credited to part 0 */
   if (D <= 1) {
+    const uint64_t tree0 = r->tree, sol0 = r->sol;
     pfsp_offload_loop(t, lb_kind, m, M, &pool, &best, r, parents, bounds, cap);
+    note_task(r, 0, tree0, sol0, best);
   } else {
     const int64_t poolSize = pool.size, c = poolSize / D, l = poolSize - (int64_t)(D - 1) * c, f = pool.front;
     pool.front = 0;
@@ -886,10 +911,14 @@ static void pfsp_search_offload_impl(int inst, int lb_kind, int ub, int m, int M
           pool_push_back(&multi[gpu], pool.elements + (size_t)(D * c + f + i) * pool.elt);
     }
     for (int gpu = 0; gpu < D; gpu++) {
-      int64_t best_l = best;
-      pfsp_offload_loop(t, lb_kind, m, M, &multi[gpu], &best_l, r, parents, bounds, NULL);
-      best_min = OR_MIN(best_min, best_l);
-      while (pool_pop_back(&multi[gpu], &parent)) pool_push_back(&pool, &parent);
+      if (part < 0 || gpu == part) { /* a part leaves the other tasks' nodes to the other parts */
+        int64_t best_l = best;
+        const uint64_t tree0 = r->tree, sol0 = r->sol;
+        pfsp_offload_loop(t, lb_kind, m, M, &multi[gpu], &best_l, r, parents, bounds, NULL);
+        note_task(r, gpu, tree0, sol0, best_l);
+        best_min = OR_MIN(best_min, best_l);
+        while (pool_pop_back(&multi[gpu], &parent)) pool_push_back(&pool, &parent);
+      }
       pool_free(&multi[gpu]);
     }
     free(multi);
@@ -906,14 +935,19 @@ static void pfsp_search_offload_impl(int inst, int lb_kind, int ub, int m, int M
 
 void or_pfsp_search_offload(int inst, int lb_kind, int ub, int m, int M, int D, int heads_mode,
                             or_search_result* r) {
-  pfsp_search_offload_impl(inst, lb_kind, ub, m, M, D, heads_mode, r, NULL);
+  pfsp_search_offload_impl(inst, lb_kind, ub, m, M, D, -1, heads_mode, r, NULL);
+}
+
+void or_pfsp_search_offload_part(int inst, int lb_kind, int ub, int m, int M, int D, int part, int heads_mode,
+                                 or_search_result* r) {
+  pfsp_search_offload_impl(inst, lb_kind, ub, m, M, D, part, heads_mode, r, NULL);
 }
 
 int or_pfsp_capture_chunk(int inst, int lb_kind, int ub, int m, int M, int which, or_pfsp_node* out, int cap,
                           int64_t* best_at_launch) {
   capture_t c = {which, out, cap, -1, 0, 0};
   or_search_result r;
-  pfsp_search_offload_impl(inst, lb_kind, ub, m, M, 1, 0, &r, &c);
+  pfsp_search_offload_impl(inst, lb_kind, ub, m, M, 1, -1, 0, &r, &c);
   if (best_at_launch) *best_at_launch = c.best_at_launch;
   return c.got;
 }

@@ -108,6 +108,10 @@ typedef struct {
   uint64_t offloads, offloaded_parents, live_slots;
   uint64_t depth_hist[OR_MAX_JOBS + 2];
   double seconds;
+  /* step 2 of each task of the D-way split (the reference's eachExploredTree / eachExploredSol, and the task's
+   * best_l when step 2 ends); task 0 alone for D = 1 */
+  uint64_t task_tree[8], task_sol[8];
+  int64_t task_best[8];
 } or_search_result;
 
 /* nqueens_chpl.chpl:92-113 (sequential DFS) */
@@ -115,13 +119,20 @@ void or_nq_search_seq(int N, int g, or_search_result* r);
 void or_nq_search_from(int N, int g, const or_nq_node* nodes, int n, uint64_t* tree, uint64_t* sol);
 int or_nq_frontier(int N, int g, int depth, or_nq_node* out, int cap, uint64_t* tree, uint64_t* sol);
 /* nqueens_gpu_chpl.chpl:152-248 / nqueens_multigpu_chpl.chpl:158-352 with the oracle as evaluator;
- * D >= 1 emulates the static strided split (no work stealing) sequentially. */
+ * D >= 1 emulates the static strided split (no work stealing) sequentially, task after task (D <= 8). */
 void or_nq_search_offload(int N, int g, int m, int M, int D, or_search_result* r);
 /* pfsp_chpl.chpl:191-215 */
 void or_pfsp_search_seq(int inst, int lb_kind, int ub, int heads_mode, or_search_result* r);
 /* pfsp_gpu_chpl.chpl:306-431 / pfsp_multigpu_chpl.chpl with the oracle as evaluator */
 void or_pfsp_search_offload(int inst, int lb_kind, int ub, int m, int M, int D, int heads_mode,
                             or_search_result* r);
+/* one task `part` (0 <= part < D) of those searches run alone, as one process of a process-per-GPU launch runs it:
+ * the same step 1 (credited to part 0 only) and static split, then step 2 of task `part` only, and step 3 on that
+ * task's own leftovers with that task's own best.  The N-Queens step 1 grows the pool to `warm` nodes (D * m in the
+ * reference; more when a task keeps several pools). */
+void or_nq_search_offload_part(int N, int g, int m, int M, int D, int part, int warm, or_search_result* r);
+void or_pfsp_search_offload_part(int inst, int lb_kind, int ub, int m, int M, int D, int part, int heads_mode,
+                                 or_search_result* r);
 
 /* capture the parents of offload number `which` (0-based) of the single-GPU N-Queens / PFSP driver
  * into out (capacity cap nodes); returns the chunk size or -1 */
