@@ -190,7 +190,13 @@ int tsb_nq_pools_per_launch(const tsb_nq* h, int M);
 /* page-lock + map a caller-owned host array for the lifetime of the handle (see the header comment);
  * TSB_EINVAL if the range partly overlaps a registered one / was not registered.  Registering a range inside a
  * registered one does nothing; disjoint arrays that share a page may both be registered; unregister takes the
- * pointer the range was registered with. */
+ * pointer the range was registered with.
+ * Page-locking is process-wide, the registry is per handle.  A range another handle has registered cannot be registered
+ * again: TSB_ECUDA (cudaHostRegister refuses it; the text is in the calling thread's tsb_last_cuda_error), and this
+ * handle's calls on it are staged (and correct) while the other handle's stay zero-copy; once the other handle has
+ * unregistered it, it can be registered here.  Disjoint arrays of different handles that share a page may be
+ * registered at the same time from different threads; each stays usable zero-copy until its own handle unregisters it,
+ * whichever unregisters first. */
 int tsb_nq_register_host(tsb_nq* h, void* ptr, size_t bytes);
 int tsb_nq_unregister_host(tsb_nq* h, void* ptr);
 int tsb_nq_set_xfer(tsb_nq* h, int mode);
