@@ -292,8 +292,8 @@ inline void board_abort(StealBoard* sb, int me) {
 template <class Node>
 void static_split(Pool<Node>& pool, int D, std::vector<Pool<Node>>& multi);
 
-// rounds per library call when other tasks may want to steal (a victim serves requests between calls)
-inline int64_t rounds_per_call(const StealBoard* sb, int M) { return !sb ? INT64_MAX : small_chunks(M) ? 256 : 4; }
+// rounds per library call when nodes may move between pools (a victim serves requests between calls)
+inline int64_t rounds_per_call(bool moves, int M) { return !moves ? INT64_MAX : small_chunks(M) ? 256 : 4; }
 
 // drain a device pool and push what it held back onto the host pool
 template <class H, class Node>
@@ -681,10 +681,92 @@ void pfsp_gpu_task(int device, const tsb_pfsp_tables& t, int lb_kind, int m, int
   tsb_pfsp_destroy(h);
 }
 
+// Several device pools per task, as many as the caller asks for (tsb_pfsp_search_device_pools): the PFSP twin of
+// nq_devpool_multi_rounds.  Every pool is one reference task with its own incumbent best[i]
+// (pfsp_multigpu_chpl.chpl:384); the pools' rounds share the launches of the persistent kernel
+// (tsb_pfsp_pool_run_multi, which runs them one after the other where one launch cannot take them: same rounds).
+// `balance` (ub = 1 only: moves keep the counts only while best is constant): a pool of the group that runs dry takes
+// the oldest half of the fullest one, and a thief task is served from the fullest pool.
+void pfsp_devpool_multi_rounds(std::vector<tsb_pfsp*>& hs, int lb_kind, int m, int M, bool balance, StealBoard* sb,
+                               int me, std::vector<int64_t>& best, GpuTaskResult& r) {
+  const int P = static_cast<int>(hs.size());
+  const auto fullest = [&] {
+    int v = 0;
+    for (int i = 1; i < P; i++)
+      if (tsb_pfsp_pool_size(hs[i]) > tsb_pfsp_pool_size(hs[v])) v = i;
+    return v;
+  };
+  const auto steal = [&](void*, void* t, int64_t* got) {
+    return tsb_pfsp_pool_steal(hs[fullest()], static_cast<tsb_pfsp*>(t), m, got);
+  };
+  const long long floor_ = steal_floor(m, M);
+  std::vector<uint64_t> out(4 * P);
+  while (r.rc == TSB_OK) {
+    if (balance) {
+      for (int i = 0; i < P && r.rc == TSB_OK; i++) {
+        if (tsb_pfsp_pool_size(hs[i]) >= m) continue;
+        const int v = fullest();
+        if (v == i || tsb_pfsp_pool_size(hs[v]) < floor_) break;
+        int64_t got = 0;
+        r.rc = tsb_pfsp_pool_steal(hs[v], hs[i], m, &got);
+      }
+      if (r.rc != TSB_OK) break;
+    }
+    long long most = 0, total = 0;
+    for (tsb_pfsp* x : hs) {
+      most = std::max<long long>(most, tsb_pfsp_pool_size(x));
+      total += tsb_pfsp_pool_size(x);
+    }
+    if (most < m) {
+      if (!board_acquire(sb, me, total, floor_)) break;
+      continue;
+    }
+    r.rc = tsb_pfsp_pool_run_multi(hs.data(), P, lb_kind, m, M, rounds_per_call(balance || sb, M), best.data(),
+                                   out.data());
+    if (r.rc != TSB_OK) break;
+    for (int i = 0; i < P; i++) {
+      r.offloads += out[4 * i];
+      r.parents += out[4 * i + 1];
+      r.tree += out[4 * i + 2];
+      r.sol += out[4 * i + 3];
+    }
+    r.rc = board_service(sb, me, tsb_pfsp_pool_size(hs[fullest()]), floor_, steal);
+  }
+  if (r.rc != TSB_OK) board_abort(sb, me);
+}
+
 // the same loop with the task's pool resident on the device (tsb_pfsp_pool_*)
 void pfsp_devpool_on(tsb_pfsp* h, int lb_kind, int m, int M, Pool<tsb_pfsp_node>& pool, GpuTaskResult& r,
-                     StealBoard* sb = nullptr, int me = 0) {
+                     StealBoard* sb = nullptr, int me = 0, int pools = 1, bool balance = false) {
   const uint64_t l0 = tsb_pfsp_kernel_launches(h);
+  if (pools > 1) {  // the task's share split once more (the same strided split) into `pools` device pools
+    std::vector<tsb_pfsp*> hs{h};
+    for (int i = 1; i < pools && r.rc == TSB_OK; i++) {
+      tsb_pfsp* sib = nullptr;
+      r.rc = tsb_pfsp_sibling(h, i, &sib);
+      hs.push_back(sib);
+    }
+    std::vector<Pool<tsb_pfsp_node>> part;
+    if (r.rc == TSB_OK) static_split(pool, pools, part);
+    long long most = 0;
+    for (int i = 0; i < pools && r.rc == TSB_OK; i++) {
+      r.rc = tsb_pfsp_pool_push(hs[i], &part[i].el[part[i].front], static_cast<int64_t>(part[i].size));
+      most = std::max<long long>(most, tsb_pfsp_pool_size(hs[i]));
+    }
+    if (sb) sb->publish_handle(me, r.rc == TSB_OK ? h : nullptr, most);
+    std::vector<int64_t> best(pools, r.best);
+    if (r.rc == TSB_OK) pfsp_devpool_multi_rounds(hs, lb_kind, m, M, balance, sb, me, best, r);
+    r.best = *std::min_element(best.begin(), best.end());
+    // leftovers pool by pool, each handed back as a reference task hands back its own (popBack onto the pool)
+    for (tsb_pfsp* x : hs) {
+      if (r.rc != TSB_OK) break;
+      Pool<tsb_pfsp_node> rest;
+      r.rc = drain_to_host(x, rest, tsb_pfsp_pool_size, tsb_pfsp_pool_drain);
+      for (tsb_pfsp_node n; rest.popBack(n);) pool.pushBack(n);
+    }
+    r.launches = tsb_pfsp_kernel_launches(h) - l0;
+    return;
+  }
   r.rc = tsb_pfsp_pool_push(h, &pool.el[pool.front], static_cast<int64_t>(pool.size));
   pool.front = 0;
   pool.size = 0;
@@ -714,18 +796,18 @@ void pfsp_devpool_on(tsb_pfsp* h, int lb_kind, int m, int M, Pool<tsb_pfsp_node>
   r.launches = tsb_pfsp_kernel_launches(h) - l0;
 }
 void pfsp_devpool_task(int device, const tsb_pfsp_tables& t, int lb_kind, int m, int M, Pool<tsb_pfsp_node>& pool,
-                       GpuTaskResult& r, StealBoard* sb = nullptr, int me = 0) {
+                       GpuTaskResult& r, StealBoard* sb = nullptr, int me = 0, int pools = 1, bool balance = false) {
   tsb_pfsp* h = nullptr;
   r.rc = tsb_pfsp_create_from_tables(&h, device, M, &t);
   if (r.rc != TSB_OK) {
     if (sb) sb->publish_handle(me, nullptr, 0);
     return;
   }
-  pfsp_devpool_on(h, lb_kind, m, M, pool, r, sb, me);
+  pfsp_devpool_on(h, lb_kind, m, M, pool, r, sb, me, pools, balance);
   tsb_pfsp_destroy(h);
 }
 void pfsp_gpu_task_nosteal(int device, const tsb_pfsp_tables& t, int lb_kind, int m, int M, Pool<tsb_pfsp_node>& pool,
-                           GpuTaskResult& r, StealBoard*, int) {
+                           GpuTaskResult& r, StealBoard*, int, int, bool) {
   pfsp_gpu_task(device, t, lb_kind, m, M, pool, r);
 }
 
@@ -972,9 +1054,11 @@ static int nq_search_device_impl(int N, int g, int m, int M, int D, int part, in
   return TSB_OK;
 }
 
+// pools > 1 (device pools only): every task's share split once more into `pools` device pools (pfsp_devpool_on)
 static int pfsp_search_impl(int inst, int lb_kind, int ub, int m, int M, int D, bool devpool, int part, int device,
-                            tsb_pfsp* on, tsb_search_stats* out) {
-  if (!out || lb_kind < 0 || lb_kind > 2 || (ub != 0 && ub != 1) || m < 1 || M < 1 || D < 1 || D > 8 || part >= D)
+                            tsb_pfsp* on, tsb_search_stats* out, int pools = 1) {
+  if (!out || lb_kind < 0 || lb_kind > 2 || (ub != 0 && ub != 1) || m < 1 || M < 1 || D < 1 || D > 8 || part >= D ||
+      pools < 1 || pools > 4)
     return TSB_EINVAL;
   std::memset(out, 0, sizeof(*out));
   std::vector<tsb_pfsp_tables> tv(1);
@@ -993,7 +1077,7 @@ static int pfsp_search_impl(int inst, int lb_kind, int ub, int m, int M, int D, 
   uint64_t tree = 0, sol = 0;
   tsb_pfsp_node parent;
   double t0 = now_s();
-  while (pool.size < static_cast<size_t>(D) * m) {
+  while (pool.size < static_cast<size_t>(D) * m * pools) {  // m nodes for every pool
     if (!pool.popFront(parent)) break;
     pfsp_decompose(hb, lb_kind, parent, tree, sol, best, pool);
   }
@@ -1003,8 +1087,18 @@ static int pfsp_search_impl(int inst, int lb_kind, int ub, int m, int M, int D, 
   const int ndev = std::max(1, tsb_device_count());
   for (auto& r : res) r.best = best;  // per-task best_l = best (pfsp_multigpu_chpl.chpl:384)
   auto task = devpool ? pfsp_devpool_task : pfsp_gpu_task_nosteal;
+  // moves between the pools of one task, as between tasks: only where they keep the counts (ub = 1)
+  const bool balance = pools > 1 && ub == 1 && !std::getenv("TSB200_NO_STEAL");
+  // a task's leftovers back to the global pool (:315-320); several pools per task already handed theirs back to
+  // the task's pool one by one, as the reference's tasks do, so that order stays
+  const auto hand_back = [&](Pool<tsb_pfsp_node>& from) {
+    if (pools > 1)
+      for (size_t i = 0; i < from.size; i++) pool.pushBack(from.el[from.front + i]);
+    else
+      while (from.popBack(parent)) pool.pushBack(parent);
+  };
   if (on) {
-    pfsp_devpool_on(on, lb_kind, m, M, pool, res[0]);
+    pfsp_devpool_on(on, lb_kind, m, M, pool, res[0], nullptr, 0, pools, balance);
   } else if (part >= 0) {  // one task of the split (see nq_search_device_impl)
     if (part != 0) tree = sol = 0;
     std::vector<Pool<tsb_pfsp_node>> multi;
@@ -1014,10 +1108,10 @@ static int pfsp_search_impl(int inst, int lb_kind, int ub, int m, int M, int D, 
     } else {
       static_split(pool, D, multi);
     }
-    task(device, t, lb_kind, m, M, multi[part], res[part], nullptr, 0);
-    while (multi[part].popBack(parent)) pool.pushBack(parent);
+    task(device, t, lb_kind, m, M, multi[part], res[part], nullptr, 0, pools, balance);
+    hand_back(multi[part]);
   } else if (D == 1) {
-    task(0, t, lb_kind, m, M, pool, res[0], nullptr, 0);
+    task(0, t, lb_kind, m, M, pool, res[0], nullptr, 0, pools, balance);
   } else {
     std::vector<Pool<tsb_pfsp_node>> multi;
     static_split(pool, D, multi);
@@ -1028,11 +1122,10 @@ static int pfsp_search_impl(int inst, int lb_kind, int ub, int m, int M, int D, 
     for (int gid = 0; gid < D; gid++)
       th.emplace_back([&, gid] {
         bind_task(gid % ndev, true);
-        task(gid % ndev, t, lb_kind, m, M, multi[gid], res[gid], sb, gid);
+        task(gid % ndev, t, lb_kind, m, M, multi[gid], res[gid], sb, gid, pools, balance);
       });
     for (auto& x : th) x.join();
-    for (int gid = 0; gid < D; gid++)
-      while (multi[gid].popBack(parent)) pool.pushBack(parent);
+    for (int gid = 0; gid < D; gid++) hand_back(multi[gid]);
     out->steals = board.steals;
   }
   for (int gid = 0; gid < D; gid++) {
@@ -1101,6 +1194,19 @@ int tsb_pfsp_search_device_part(int inst, int lb_kind, int ub, int m, int M, int
 int tsb_pfsp_search_on(tsb_pfsp* h, int inst, int lb_kind, int ub, int m, int M, tsb_search_stats* out) {
   if (!h) return TSB_EINVAL;
   return pfsp_search_impl(inst, lb_kind, ub, m, M, 1, true, -1, 0, h, out);
+}
+int tsb_pfsp_search_device_pools(int inst, int lb_kind, int ub, int m, int M, int D, int pools, tsb_search_stats* out) {
+  return pfsp_search_impl(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out, pools);
+}
+int tsb_pfsp_search_device_pools_part(int inst, int lb_kind, int ub, int m, int M, int D, int pools, int part,
+                                      int device, tsb_search_stats* out) {
+  if (part < 0) return TSB_EINVAL;
+  return pfsp_search_impl(inst, lb_kind, ub, m, M, D, true, part, device, nullptr, out, pools);
+}
+int tsb_pfsp_search_on_pools(tsb_pfsp* h, int inst, int lb_kind, int ub, int m, int M, int pools,
+                             tsb_search_stats* out) {
+  if (!h) return TSB_EINVAL;
+  return pfsp_search_impl(inst, lb_kind, ub, m, M, 1, true, -1, 0, h, out, pools);
 }
 
 }  // extern "C"

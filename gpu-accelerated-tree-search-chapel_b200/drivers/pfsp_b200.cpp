@@ -8,13 +8,16 @@
 #include "tsb200.h"
 
 int main(int argc, char** argv) {
-  int inst = 14, ub = 1, m = 25, M = 50000, D = 1, lb = TSB_LB1, devpool = 0;
+  int inst = 14, ub = 1, m = 25, M = 50000, D = 1, lb = TSB_LB1, devpool = 0, pools = 1;
   const char* lbs = "lb1";
   for (int i = 1; i < argc; i++) {
     if (!std::strcmp(argv[i], "-h") || !std::strcmp(argv[i], "--help")) {
       std::printf("\n  PFSP Benchmark Parameters:\n\n   --inst   int   Taillard's instance to solve (between 001 and 120)\n"
                   "   --lb     str   lower bound function (lb1, lb1_d, lb2)\n"
-                  "   --ub     int   initial upper bound (0, 1)\n   --m --M --D as for N-Queens\n\n");
+                  "   --ub     int   initial upper bound (0, 1)\n   --m --M --D as for N-Queens\n"
+                  "   --devpool int  1: the pool(s) of step 2 stay on the GPU(s)\n"
+                  "   --pools  int   device pools per GPU task (1..4; > 1 needs --devpool 1): each is one task\n"
+                  "                  of the reference, with its own incumbent, sharing the GPU's launches\n\n");
       return 1;
     }
     if (i + 1 >= argc) break;
@@ -27,10 +30,15 @@ int main(int argc, char** argv) {
     int* dst = !std::strcmp(argv[i], "--inst") ? &inst : !std::strcmp(argv[i], "--ub") ? &ub
              : !std::strcmp(argv[i], "--m") ? &m : !std::strcmp(argv[i], "--M") ? &M
              : !std::strcmp(argv[i], "--D") ? &D
-             : !std::strcmp(argv[i], "--devpool") ? &devpool : nullptr;  // 1: pool(s) of step 2 resident on the GPU
+             : !std::strcmp(argv[i], "--devpool") ? &devpool  // 1: pool(s) of step 2 resident on the GPU
+             : !std::strcmp(argv[i], "--pools") ? &pools : nullptr;
     if (dst) *dst = std::atoi(argv[++i]);
   }
   if (m <= 0 || M <= 0) { std::fprintf(stderr, "Error: m and M must be positive integers.\n"); return 2; }
+  if (pools < 1 || pools > 4 || (pools > 1 && !devpool)) {
+    std::fprintf(stderr, "Error: --pools must be 1..4, and more than 1 needs --devpool 1\n");
+    return 2;
+  }
   if (inst < 1 || inst > 120) { std::fprintf(stderr, "Error: unsupported Taillard's instance\n"); return 2; }
   if (lb < 0) { std::fprintf(stderr, "Error - Unsupported lower bound\n"); return 2; }
   if (ub != 0 && ub != 1) { std::fprintf(stderr, "Error: unsupported upper bound initialization\n"); return 2; }
@@ -40,7 +48,9 @@ int main(int argc, char** argv) {
               D > 1 ? "Multi-GPU" : "Single-GPU", inst, tsb_taillard_nb_machines(inst), tsb_taillard_nb_jobs(inst),
               ub ? "opt" : "inf", lbs);
   tsb_search_stats st;
-  const int rc = devpool ? tsb_pfsp_search_device(inst, lb, ub, m, M, D, &st) : tsb_pfsp_search(inst, lb, ub, m, M, D, &st);
+  const int rc = !devpool    ? tsb_pfsp_search(inst, lb, ub, m, M, D, &st)
+                 : pools > 1 ? tsb_pfsp_search_device_pools(inst, lb, ub, m, M, D, pools, &st)
+                             : tsb_pfsp_search_device(inst, lb, ub, m, M, D, &st);
   if (rc != TSB_OK) {
     std::fprintf(stderr, "tsb_pfsp_search: %s (%s)\n", tsb_strerror(rc), tsb_last_cuda_error());
     return 3;

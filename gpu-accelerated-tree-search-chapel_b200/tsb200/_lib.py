@@ -139,6 +139,9 @@ SYMBOLS = {
     "tsb_pfsp_search_on": (_i, [_vp, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
     "tsb_nq_search_device_part": (_i, [_i, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
     "tsb_pfsp_search_device_part": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
+    "tsb_pfsp_search_device_pools": (_i, [_i, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
+    "tsb_pfsp_search_device_pools_part": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
+    "tsb_pfsp_search_on_pools": (_i, [_vp, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
 }
 
 _lib = None

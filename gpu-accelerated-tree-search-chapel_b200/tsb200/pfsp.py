@@ -172,12 +172,17 @@ class PfspEvaluator:
                                       C.byref(nc), C.byref(ns)), "tsb_pfsp_pool_run")
         return int(nr.value), int(np_.value), int(nc.value), int(ns.value), int(b.value)
 
-    def search(self, inst: int, lb, ub: int = 1, m: int = 25, M: int | None = None) -> SearchStats:
-        """the whole 3-step search (pfsp_gpu_chpl.chpl:306-431) with the pool of step 2 on this handle's device"""
+    def search(self, inst: int, lb, ub: int = 1, m: int = 25, M: int | None = None, pools: int = 1) -> SearchStats:
+        """the whole 3-step search (pfsp_gpu_chpl.chpl:306-431) with the pool of step 2 on this handle's device;
+        pools > 1: on this handle and its first pools - 1 siblings (tsb_pfsp_search_on_pools)"""
         kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
         st = SearchStats()
-        check(lib().tsb_pfsp_search_on(self._h, inst, kind, ub, m, self.M if M is None else M, C.byref(st)),
-              "tsb_pfsp_search_on")
+        M = self.M if M is None else M
+        if pools == 1:
+            check(lib().tsb_pfsp_search_on(self._h, inst, kind, ub, m, M, C.byref(st)), "tsb_pfsp_search_on")
+        else:
+            check(lib().tsb_pfsp_search_on_pools(self._h, inst, kind, ub, m, M, pools, C.byref(st)),
+                  "tsb_pfsp_search_on_pools")
         return st
 
     def sibling(self, index: int) -> "PfspEvaluator":
@@ -225,11 +230,17 @@ def pfsp_pool_run_multi(evaluators, lb, m: int, M: int, bests, max_rounds: int =
     return [tuple(int(out[4 * i + j]) for j in range(4)) + (int(b[i]),) for i in range(K)]
 
 
-def pfsp_search_device(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1) -> SearchStats:
-    """same search, the pool(s) of step 2 resident on the device(s) (tsb_pfsp_pool_*)"""
+def pfsp_search_device(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1,
+                       pools: int = 1) -> SearchStats:
+    """same search, the pool(s) of step 2 resident on the device(s) (tsb_pfsp_pool_*); pools > 1: that many device
+    pools per task (tsb_pfsp_search_device_pools)"""
     kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
     st = SearchStats()
-    check(lib().tsb_pfsp_search_device(inst, kind, ub, m, M, D, C.byref(st)), "tsb_pfsp_search_device")
+    if pools == 1:
+        check(lib().tsb_pfsp_search_device(inst, kind, ub, m, M, D, C.byref(st)), "tsb_pfsp_search_device")
+    else:
+        check(lib().tsb_pfsp_search_device_pools(inst, kind, ub, m, M, D, pools, C.byref(st)),
+              "tsb_pfsp_search_device_pools")
     return st
 
 
@@ -241,9 +252,14 @@ def pfsp_search(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: int = 500
     return st
 
 
-def pfsp_search_device_part(inst: int, lb, ub: int, m: int, M: int, D: int, part: int, device: int = 0) -> SearchStats:
+def pfsp_search_device_part(inst: int, lb, ub: int, m: int, M: int, D: int, part: int, device: int = 0,
+                            pools: int = 1) -> SearchStats:
     kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
     st = SearchStats()
-    check(lib().tsb_pfsp_search_device_part(inst, kind, ub, m, M, D, part, device, C.byref(st)),
-          "tsb_pfsp_search_device_part")
+    if pools == 1:
+        check(lib().tsb_pfsp_search_device_part(inst, kind, ub, m, M, D, part, device, C.byref(st)),
+              "tsb_pfsp_search_device_part")
+    else:
+        check(lib().tsb_pfsp_search_device_pools_part(inst, kind, ub, m, M, D, pools, part, device, C.byref(st)),
+              "tsb_pfsp_search_device_pools_part")
     return st

@@ -401,6 +401,29 @@ int tsb_pfsp_search_device(int inst, int lb_kind, int ub, int m, int M, int D, t
 int tsb_pfsp_search_device_part(int inst, int lb_kind, int ub, int m, int M, int D, int part, int device,
                                 tsb_search_stats* out);
 int tsb_pfsp_search_on(tsb_pfsp* h, int inst, int lb_kind, int ub, int m, int M, tsb_search_stats* out);
+/* The same searches with `pools` (1..4, TSB_EINVAL otherwise) device pools per task instead of one; every other
+ * argument is checked as by the twin without `_pools`.  pools = 1 is exactly that twin.  pools = K:
+ *   - step 1 runs until the pool holds D*K*m nodes; the strided split (pfsp_multigpu_chpl.chpl) gives every task its
+ *     share, and each share is split the same way again into K device pools;
+ *   - every pool is one reference task: it follows popBackBulk(m, M) on its own nodes with its own incumbent, which
+ *     starts from the step-1 best; the incumbents are min-reduced at the end; each pool hands its leftovers back to
+ *     the task in pool order as a reference task does (popBack), and the tasks' leftovers keep that order;
+ *   - ub = 0: nothing moves between pools, so the counts are those of D*K reference tasks under that two-level split
+ *     (D = 1: exactly the reference's run with D = K tasks);
+ *   - ub = 1: a pool that runs dry takes the oldest half of the fullest pool of its task, and a task that runs dry
+ *     steals from the fullest pool of another task (TSB200_NO_STEAL=1: neither); the totals stay the reference's;
+ *   - the K pools of a task share every launch of the persistent kernel when tsb_pfsp_pools_per_launch(h, lb_kind,
+ *     M) >= K; otherwise (lb2, M beyond the K-pool capacity, TSB200_NO_ROUNDS=1) they run one after the other
+ *     (tsb_pfsp_pool_run_multi).  Chunks and counts depend on K, never on the device.
+ * per_gpu_tree[g] is task g's step-2 tree summed over its pools, steals counts moves between tasks only and
+ * kernel_launches counts the launches of all pools.  _part: one task of the split, step 1 credited to part 0 (as
+ * tsb_pfsp_search_device_part).  _on_pools: D = 1 on `h` and its siblings 1..K-1 (tsb_pfsp_sibling; siblings that do
+ * not exist yet are created inside the search, so create them first to keep that out of the timers). */
+int tsb_pfsp_search_device_pools(int inst, int lb_kind, int ub, int m, int M, int D, int pools, tsb_search_stats* out);
+int tsb_pfsp_search_device_pools_part(int inst, int lb_kind, int ub, int m, int M, int D, int pools, int part,
+                                      int device, tsb_search_stats* out);
+int tsb_pfsp_search_on_pools(tsb_pfsp* h, int inst, int lb_kind, int ub, int m, int M, int pools,
+                             tsb_search_stats* out);
 
 #ifdef __cplusplus
 }
