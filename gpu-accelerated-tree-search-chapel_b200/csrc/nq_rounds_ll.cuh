@@ -268,51 +268,108 @@ __global__ void nq_fat_export_kernel(const FatNode* __restrict__ fat, uint8_t* _
   for (int i = 0; i < NQ_REC - 1; i++) node[1 + i] = static_cast<uint8_t>(d[ll_fw(i)] >> ll_fs(i) & 31u);
 }
 
-// the exchange warp: until all n slots carry `epoch`; sums of {leaves << 32 | children} over all slots and over the slots
-// before k0 / before k1 (valid in every lane); false = abort
-__device__ __forceinline__ bool warp_gather_slots2(const unsigned long long* slot, int n, int k0, int k1, unsigned epoch,
-                                                   unsigned* abort_flag, unsigned long long& before0,
-                                                   unsigned long long& before1, unsigned long long& all) {
-  const int lane = threadIdx.x & 31;
-  // slot pairs per lane in flight: a sweep of up to 64 B slots (2 G on GPUs of up to 160 SMs) is ONE L2 round trip.
-  // (A loop that sums each pair before it loads the next one issued them one after the other: two or three dependent
-  // round trips per sweep at 2 G = 132, all of the last sweep exposed in the round.)
-  constexpr int B = 5;
+// The exchange warp's count gather: 2G slots {epoch << 32 | leaves << 20 | children}, lane l holds the slot pairs
+// 2l + 64u.  Its first LL_GB pairs are loaded back to back, so a sweep over up to 64 LL_GB slots (2G on GPUs of up to
+// 160 SMs) is ONE L2 round trip.  (A loop that summed each pair before it loaded the next one issued them one after
+// the other: two or three dependent round trips per sweep at 2G = 132, all of the last sweep exposed in the round.)
+// Further pairs (more than 160 CTAs per pool) are loaded one by one.
+constexpr int LL_GB = 5;
+__device__ __forceinline__ void ll_load_pair(const unsigned long long* p, unsigned long long& a, unsigned long long& b) {
+  asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "l"(p) : "memory");
+}
+static_assert(64 * LL_GB <= 2 * LL_MAX_SMS, "a lane's first LL_GB pairs lie inside LlSync::slot");
+__device__ __forceinline__ bool ll_pair_carries(int n, int i, unsigned epoch, unsigned long long a, unsigned long long b) {
+  return static_cast<unsigned>(a >> 32) == epoch && (i + 1 >= n || static_cast<unsigned>(b >> 32) == epoch);
+}
+// Which of the lane's first 2 LL_GB slots (bit 2u + e: slot 2 lane + 64u + e) exist and lie before k0 / k1.  They are
+// the same in every round, so a sweep and the sums test bits instead of comparing slot numbers.
+struct LlLaneSlots {
+  unsigned in, lt0, lt1;
+};
+__device__ __forceinline__ LlLaneSlots ll_lane_slots(int n, int k0, int k1) {
+  const int c0 = 2 * (threadIdx.x & 31);
+  LlLaneSlots m = {0u, 0u, 0u};
+#pragma unroll
+  for (int j = 0; j < 2 * LL_GB; j++) {
+    const int i = c0 + 64 * (j >> 1) + (j & 1);
+    m.in |= (i < n ? 1u : 0u) << j;
+    m.lt0 |= (i < k0 ? 1u : 0u) << j;
+    m.lt1 |= (i < k1 ? 1u : 0u) << j;
+  }
+  // (opaque to the compiler: the masks stay in three registers instead of being recomputed from the compares in
+  // every round's sums)
+  asm volatile("" : "+r"(m.in), "+r"(m.lt0), "+r"(m.lt1));
+  return m;
+}
+// Sweeps until all n slots carry `epoch`; the lane's first LL_GB pairs of the sweep that saw every slot stay in v0 /
+// v1.  A sweep only tests the epochs: the sums run once, after it (warp_sum_slots2).  `in_flight()` runs once, while
+// the first sweep's loads are on their way.  false = abort.  (Group u is skipped by the whole warp when 64u >= n; in
+// a group that is loaded, a lane past n loads a slot inside the array and ignores it.)
+template <class F>
+__device__ __forceinline__ bool warp_gather_slots2(const unsigned long long* slot, int n, unsigned epoch,
+                                                   unsigned* abort_flag, const LlLaneSlots& ls,
+                                                   unsigned long long (&v0)[LL_GB], unsigned long long (&v1)[LL_GB],
+                                                   F&& in_flight) {
+  const int c0 = 2 * (threadIdx.x & 31);
+  const auto load = [&]() {
+#pragma unroll
+    for (int u = 0; u < LL_GB; u++)
+      if (64 * u < n) ll_load_pair(slot + c0 + 64 * u, v0[u], v1[u]);
+  };
   SpinGuard guard;
+  load();
+  in_flight();
   for (;;) {
     bool ok = true;
-    before0 = before1 = all = 0;
-    for (int i0 = 2 * lane; i0 < n; i0 += 64 * B) {
-      unsigned long long v0[B], v1[B];
 #pragma unroll
-      for (int u = 0; u < B; u++)
-        if (i0 + 64 * u < n)
-          asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];" : "=l"(v0[u]), "=l"(v1[u]) : "l"(slot + i0 + 64 * u) : "memory");
-#pragma unroll
-      for (int u = 0; u < B; u++) {
-        const int i = i0 + 64 * u;
-        if (i >= n) break;
-        const bool has1 = i + 1 < n;
-        ok &= static_cast<unsigned>(v0[u] >> 32) == epoch && (!has1 || static_cast<unsigned>(v1[u] >> 32) == epoch);
-        const unsigned long long p0 = (v0[u] & 0xFFFFFull) | ((v0[u] >> 20) & 0xFFFull) << 32;
-        const unsigned long long p1 = has1 ? (v1[u] & 0xFFFFFull) | ((v1[u] >> 20) & 0xFFFull) << 32 : 0ull;
-        all += p0 + p1;
-        if (i < k0) before0 += p0;
-        if (i + 1 < k0) before0 += p1;
-        if (i < k1) before1 += p0;
-        if (i + 1 < k1) before1 += p1;
-      }
+    for (int u = 0; u < LL_GB; u++)
+      if (64 * u < n)
+        ok &= (static_cast<unsigned>(v0[u] >> 32) == epoch || !(ls.in >> (2 * u) & 1u)) &&
+              (static_cast<unsigned>(v1[u] >> 32) == epoch || !(ls.in >> (2 * u + 1) & 1u));
+    for (int i = c0 + 64 * LL_GB; i < n; i += 64) {
+      unsigned long long a, b;
+      ll_load_pair(slot + i, a, b);
+      ok &= ll_pair_carries(n, i, epoch, a, b);
     }
-    if (__all_sync(0xFFFFFFFFu, ok)) break;
+    if (__all_sync(0xFFFFFFFFu, ok)) return true;
     if (__any_sync(0xFFFFFFFFu, guard.expired(abort_flag))) return false;
+    load();
   }
+}
+// The gathered children over all slots and over the slots before k0 / k1 (in every lane: at most 2G x 13 056, 32
+// bits), and this lane's share of the leaves
+__device__ __forceinline__ void warp_sum_slots2(const unsigned long long* slot, const unsigned long long (&v0)[LL_GB],
+                                                const unsigned long long (&v1)[LL_GB], int n, int k0, int k1,
+                                                const LlLaneSlots& ls, unsigned& all, unsigned& before0,
+                                                unsigned& before1, unsigned& leaves) {
+  const int c0 = 2 * (threadIdx.x & 31);
+  all = before0 = before1 = leaves = 0;
+  const auto add = [&](unsigned x, bool in, bool lt0, bool lt1) {
+    x = in ? x : 0u;
+    const unsigned y = x & 0xFFFFFu;
+    all += y;
+    leaves += x >> 20;
+    before0 += lt0 ? y : 0u;
+    before1 += lt1 ? y : 0u;
+  };
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    before0 += __shfl_xor_sync(0xFFFFFFFFu, before0, o);
-    before1 += __shfl_xor_sync(0xFFFFFFFFu, before1, o);
-    all += __shfl_xor_sync(0xFFFFFFFFu, all, o);
+  for (int u = 0; u < LL_GB; u++)
+    if (64 * u < n) {
+      add(static_cast<unsigned>(v0[u]), ls.in >> (2 * u) & 1u, ls.lt0 >> (2 * u) & 1u, ls.lt1 >> (2 * u) & 1u);
+      add(static_cast<unsigned>(v1[u]), ls.in >> (2 * u + 1) & 1u, ls.lt0 >> (2 * u + 1) & 1u, ls.lt1 >> (2 * u + 1) & 1u);
+    }
+  // (further pairs are loaded again: they still hold this round's values, because another CTA writes this parity's
+  // slots again two rounds on, after it has seen this CTA's slots of the next round)
+  for (int i = c0 + 64 * LL_GB; i < n; i += 64) {
+    unsigned long long a, b;
+    ll_load_pair(slot + i, a, b);
+    add(static_cast<unsigned>(a), true, i < k0, i < k1);
+    add(static_cast<unsigned>(b), i + 1 < n, i + 1 < k0, i + 1 < k1);
   }
-  return true;
+  // (three independent warp reductions, redux.sync)
+  all = __reduce_add_sync(0xFFFFFFFFu, all);
+  before0 = __reduce_add_sync(0xFFFFFFFFu, before0);
+  before1 = __reduce_add_sync(0xFFFFFFFFu, before1);
 }
 
 // what the exchange warp hands the workers at the end of a round's gather (one record: the workers copy the offsets
@@ -329,7 +386,7 @@ struct LlPlan {
 // TSB200_ROUNDS_PROF phases (CTA 0 cycles; workers: thread 0, exchange warp: its lane 0)
 enum {
   LL_PROF_SETUP = 0, LL_PROF_POLL, LL_PROF_SCAN, LL_PROF_BUILD, LL_PROF_HAND, LL_PROF_STORE,  // workers
-  LL_PROF_X_SCAN, LL_PROF_X_GATHER, LL_PROF_X_BOOK, LL_PROF_X_HAND,                         // exchange warp
+  LL_PROF_X_SCAN, LL_PROF_X_AHEAD, LL_PROF_X_GATHER, LL_PROF_X_TAIL, LL_PROF_X_HAND,        // exchange warp
   LL_PROF_N
 };
 static_assert(LL_PROF_N <= 12, "RoundsState::prof");
@@ -389,10 +446,14 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
 // One CTA = LL_T worker threads (warps 0-7) + one EXCHANGE warp (warp 8).  A round:
 //   workers:   poll the slice -> child masks, block scan -> (LL_BAR_SCAN arrive) -> items -> build the first window
 //              -> HANDOFF -> store the windows -> the next round's poll
-//   exchange:  (LL_BAR_SCAN wait) -> publish the CTA's two count slots -> gather all 2G slots -> offsets, layer stack,
-//              pool size, counters, exit tests and the next round's geometry -> HANDOFF
+//   exchange:  (LL_BAR_SCAN wait) -> publish the CTA's two count slots -> issue the first sweep over all 2G slots ->
+//              while it is in flight: layer-stack pop and new top entry, next tag and top layer, the interval of the
+//              round's total R for which the next round is plan()'s common case -> sweeps that only test epochs ->
+//              sums of the last sweep (offsets, R) -> common case: next chunk start; else plan() -> HANDOFF ->
+//              counters
 // so the gather runs while the workers build, and the bookkeeping of a round and the set-up of the next are off the
-// workers' chain: after their stores they go straight into the next poll.  The pool state (size, epoch, layers,
+// workers' chain: after their stores they go straight into the next poll.  Between the last slot's arrival and the
+// handoff only the sums, a range test and a few shared-memory stores remain.  The pool state (size, epoch, layers,
 // counters) is the exchange warp's alone; the workers get what they need through sm.plan.
 template <int N, int T, int MINB, int PPT>
 __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid_constant__ LlMultiParams mprm) {
@@ -490,6 +551,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
 
   if (wid == T / 32) {
     // ------------------------------------------------------------------------------------------ the exchange warp
+    const LlLaneSlots lane_slots = ll_lane_slots(G2, k, G2 - 1 - k);
     while (exit_code < 0) {
       ll_wait(LL_BAR_SCAN, TX);  // the workers' warp totals are in sm.warp_tot64 (they have read their slices)
       TSB_PROF(prof_x, 1, LL_PROF_X_SCAN)
@@ -508,54 +570,77 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       if (lane < 2)
         st_relaxed_u64(&slots[lane == 0 ? k : G2 - 1 - k],
                        lane == 0 ? e | static_cast<unsigned long long>(my_leaves) << 20 | cnt0 : e | (my_children - cnt0));
-      // ---- (6) all-to-all: everybody's {leaves, children}; my child offsets and the round's totals (the workers
-      // build their first window meanwhile)
-      unsigned long long before0 = 0, before1 = 0, all = 0;
-      const bool ok = warp_gather_slots2(slots, G2, k, G2 - 1 - k, epoch, &sy->abort, before0, before1, all);
-      TSB_PROF(prof_x, 1, LL_PROF_X_GATHER)
-      if (ok) {
-        if (lane == 0) {
-          sm.plan.off0 = static_cast<int>(before0 & 0xFFFFFFFFull);
-          sm.plan.off1 = static_cast<int>(before1 & 0xFFFFFFFFull);
-        }
-        const long long round_children = static_cast<long long>(all & 0xFFFFFFFFull);
-        // ---- (8) the pool's layers after the round: every layer that starts inside the chunk is consumed, the
-        // round's children form the new top layer (same computation in every CTA).  The workers read the stack only
-        // in their poll, and all of them have finished this round's poll (they arrived at LL_BAR_SCAN) and start
-        // the next one after the handoff: nobody reads an entry while it changes.  (lay_top = lay_start[n_lay - 1]:
-        // the loop ends at the top layer in most rounds, without waiting for a shared-memory load.)
-        int nl = n_lay;
-        long long below = lay_top;
+      // ---- (6) all-to-all: everybody's {leaves, children} (the workers build their first window meanwhile).
+      // While the first sweep's loads are on their way, everything of the round's bookkeeping that does not depend
+      // on its total R of children:
+      // (8) the pool's layers after the round: every layer that starts inside the chunk is consumed, the round's
+      // children form the new top layer (same computation in every CTA).  The workers read the stack only in their
+      // poll, and all of them have finished this round's poll (they arrived at LL_BAR_SCAN) and start the next one
+      // after the handoff: nobody reads an entry while it changes.  So the new top entry is written now; if R == 0 it
+      // lies above the top the stack keeps (nl entries) and is never read.  (lay_top = lay_start[n_lay - 1]: the loop
+      // ends at the top layer in most rounds, without waiting for a shared-memory load.)
+      // (9) the next round's tag and top layer for the common case, straight into sm.plan: the workers read them
+      // before their poll, i.e. before LL_BAR_SCAN this round and after the handoff next round; if plan() runs
+      // instead it writes them again.  And the interval of R for which plan() would take the common case: the pool
+      // keeps at least max(M, m) nodes, so the next chunk is M == geo_n parents and its geometry stands, and no exit
+      // applies (arena room for the next chunk's children, round budget, layer table, epoch window).
+      const long long n_prev = chunk_n;
+      int nl = n_lay;
+      long long below = lay_top, r_lo = 1, r_hi = 0;
+      const auto plan_ahead = [&]() {
         while (nl > 0 && below >= chunk_s0) {
           --nl;
           below = nl > 0 ? sm.lay_start[nl - 1] : -1;
         }
         __syncwarp();  // (every lane has read the entry lane 0 may overwrite)
-        if (round_children > 0) {
-          if (lane == 0) {
-            sm.lay_start[nl] = chunk_s0;
-            sm.lay_tag[nl] = ll_tag(epoch);
-          }
-          ++nl;
-          below = chunk_s0;
+        if (lane == 0) {
+          sm.lay_start[nl] = chunk_s0;
+          sm.lay_tag[nl] = ll_tag(epoch);
+          sm.plan.tag = ll_tag(epoch + 1u);
+          sm.plan.top = nl;
         }
-        n_lay = nl;
-        lay_top = below;
-        // ---- (9) the pool after the round, and the next round's chunk
-        size = chunk_s0 + round_children;
-        size_hi = size > size_hi ? size : size_hi;
+        const long long Mx = prm.M > prm.m ? prm.M : prm.m;
+        r_lo = Mx - chunk_s0 > 1 ? Mx - chunk_s0 : 1;  // (R > 0: the new top layer exists)
+        if (geo_n == prm.M && static_cast<long long>(rounds) + 1 < prm.max_rounds && nl + 1 < LL_LAYERS &&
+            epoch != prm.epoch_last)
+          r_hi = prm.cap - static_cast<long long>(prm.M) * N + prm.M - chunk_s0;  // (chunk_s0 + R - M) + M N <= cap
+        TSB_PROF(prof_x, 1, LL_PROF_X_AHEAD)
+      };
+      unsigned long long v0[LL_GB], v1[LL_GB];
+      const bool ok = warp_gather_slots2(slots, G2, epoch, &sy->abort, lane_slots, v0, v1, plan_ahead);
+      TSB_PROF(prof_x, 1, LL_PROF_X_GATHER)
+      unsigned R = 0, leaves = 0;
+      if (ok) {
+        // my child offsets and the round's total; then the rest of (8) and (9)
+        unsigned before0, before1;
+        warp_sum_slots2(slots, v0, v1, G2, k, G2 - 1 - k, lane_slots, R, before0, before1, leaves);
+        if (lane == 0) {
+          sm.plan.off0 = static_cast<int>(before0);
+          sm.plan.off1 = static_cast<int>(before1);
+        }
         ++rounds;
-        tot_parents += static_cast<unsigned long long>(chunk_n);
-        tot_children += static_cast<unsigned long long>(round_children);
-        tot_solutions += all >> 32;
-        exit_code = plan();
+        size = chunk_s0 + R;
+        n_lay = R > 0 ? nl + 1 : nl;
+        lay_top = R > 0 ? chunk_s0 : below;
+        if (R >= r_lo && R <= r_hi) {  // plan()'s common case: chunk_n, the geometry, tag, top and exit stand
+          ++epoch;
+          chunk_s0 = size - chunk_n;
+          if (lane == 0) sm.plan.s0 = chunk_s0;
+        } else {
+          exit_code = plan();
+        }
       }
-      TSB_PROF(prof_x, 1, LL_PROF_X_BOOK)
+      TSB_PROF(prof_x, 1, LL_PROF_X_TAIL)
       if (ll_bar_or(LL_BAR_HAND, TX, !ok)) {  // the handoff (an abort reaches the workers here)
         exit_code = RND_EXIT_ABORT;
         break;
       }
       TSB_PROF(prof_x, 1, LL_PROF_X_HAND)
+      // the round's counters, after the handoff
+      size_hi = size > size_hi ? size : size_hi;
+      tot_parents += static_cast<unsigned long long>(n_prev);
+      tot_children += R;
+      tot_solutions += __reduce_add_sync(0xFFFFFFFFu, leaves);
     }
   } else {
     // ------------------------------------------------------------------------------------------ the workers

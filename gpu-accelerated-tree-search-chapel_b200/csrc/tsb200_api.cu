@@ -1135,11 +1135,11 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
         const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
         std::fprintf(stderr, "[tsb200] LL rounds kernel (pool %d of %d): %llu rounds; CTA 0 cycles per round: workers: set-up %.0f "
                      "poll-nodes %.0f scan+items %.0f build %.0f handoff-wait %.0f store %.0f | exchange warp: "
-                     "scan-wait %.0f publish+gather %.0f bookkeeping %.0f handoff-wait %.0f\n", a, n_act,
+                     "scan-wait %.0f publish+plan-ahead %.0f gather-wait %.0f sums+plan %.0f handoff-wait %.0f\n", a, n_act,
                      static_cast<unsigned long long>(st.rounds), st.prof[tsb::LL_PROF_SETUP] / r, st.prof[tsb::LL_PROF_POLL] / r,
                      st.prof[tsb::LL_PROF_SCAN] / r, st.prof[tsb::LL_PROF_BUILD] / r, st.prof[tsb::LL_PROF_HAND] / r,
-                     st.prof[tsb::LL_PROF_STORE] / r, st.prof[tsb::LL_PROF_X_SCAN] / r, st.prof[tsb::LL_PROF_X_GATHER] / r,
-                     st.prof[tsb::LL_PROF_X_BOOK] / r, st.prof[tsb::LL_PROF_X_HAND] / r);
+                     st.prof[tsb::LL_PROF_STORE] / r, st.prof[tsb::LL_PROF_X_SCAN] / r, st.prof[tsb::LL_PROF_X_AHEAD] / r,
+                     st.prof[tsb::LL_PROF_X_GATHER] / r, st.prof[tsb::LL_PROF_X_TAIL] / r, st.prof[tsb::LL_PROF_X_HAND] / r);
       }
       left[i] -= static_cast<int64_t>(st.rounds);
       if (st.exit_code == tsb::RND_EXIT_SPACE) {
