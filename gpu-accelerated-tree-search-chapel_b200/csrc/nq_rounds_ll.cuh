@@ -99,7 +99,22 @@ struct RoundsState {
   unsigned long long rounds, parents, children, solutions;  // of this launch
   long long prof[12];  // (prm.prof) cycles CTA 0 spent per phase (the LL_PROF_* indices of nq_rounds_ll_kernel)
   long long size_hi;   // (nq_rounds_ll_kernel) the largest pool size of the launch: every position it stored lies below
+  // (nq_rounds_ll_kernel, prm.prof) %globaltimer (ns) read by CTA 0's exchange warp when the pool starts and when it
+  // leaves the launch (a launch ends when its last pool leaves), and where each CTA k of the pool ran: %smid and the
+  // low 32 bits of %globaltimer at its start
+  unsigned long long t_start, t_exit;
+  unsigned cta_sm[LL_MAX_SMS], cta_t0[LL_MAX_SMS];
 };
+__device__ __forceinline__ unsigned long long ll_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ unsigned ll_smid() {
+  unsigned s;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+  return s;
+}
 
 __device__ __forceinline__ void st_relaxed_u64(unsigned long long* p, unsigned long long v) {
   asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
@@ -415,13 +430,15 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
   const uint4 p = parent[r];
   uint32_t P[4] = {p.x, p.y, p.z, p.w};
   const uint32_t depth = ll_depth(p.x, p.y, p.z);
-  const auto word = [&](uint32_t w) { return w == 0 ? P[0] : w == 1 ? P[1] : w == 2 ? P[2] : P[3]; };
   // first bit of board[i] in the four data words read as one 128-bit value: 32 (i / 6) + 5 (i % 6) = 5 i + 2 (i / 6),
   // with i / 6 = (43 i) >> 8 for every i < 20 (no division)
   const uint32_t bd = 5u * depth + 2u * (depth * 43u >> 8), bk = 5u * k + 2u * (k * 43u >> 8);
-  const uint32_t wd = bd >> 5, sd = bd & 31u, wk = bk >> 5, sk = bk & 31u;
-  const uint32_t v = word(wk) >> sk & 31u;  // the queen placed on row `depth`
-  const uint32_t D = (word(wd) >> sd & 31u) ^ v;
+  // (a clamped right shift by b - 32 j is the field at bit b in word j and 0 in every other word)
+  const auto field = [&](uint32_t b) {
+    return (shr_clamp(P[0], b) | shr_clamp(P[1], b - 32u) | shr_clamp(P[2], b - 64u) | shr_clamp(P[3], b - 96u)) & 31u;
+  };
+  const uint32_t v = field(bk);  // the queen placed on row `depth`
+  const uint32_t D = field(bd) ^ v;
   // (a clamped shift by bd - 32 j is D << sd in word wd and 0 in every other word: no field straddles two words)
 #pragma unroll
   for (uint32_t j = 0; j < 4; j++) P[j] ^= shl_clamp(D, bd - 32u * j) ^ shl_clamp(D, bk - 32u * j);
@@ -541,6 +558,12 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       sm.lay_start[0] = 0;
       sm.lay_tag[0] = LL_TRUSTED;
       sm.poll_abort = 0;
+      if (prm.prof != 0) {
+        const unsigned long long now = ll_globaltimer();
+        prm.state->cta_sm[k] = ll_smid();
+        prm.state->cta_t0[k] = static_cast<unsigned>(now);
+        if (k == 0) prm.state->t_start = now;
+      }
       if (prof_x)
         for (int i = 0; i < LL_PROF_N; i++) sm.prof[i] = 0;
     }
@@ -642,6 +665,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       tot_children += R;
       tot_solutions += __reduce_add_sync(0xFFFFFFFFu, leaves);
     }
+    if (prof_x) prm.state->t_exit = ll_globaltimer();
   } else {
     // ------------------------------------------------------------------------------------------ the workers
     for (;;) {
@@ -668,7 +692,13 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         for (int j = 0; j < PCS; j++)
           if (t + j * T < 2 * len) pending |= 1u << j;
         // the tag node i of my slice was stored with: that of the layer its position lies in (mostly the top one)
+        // (in almost every round both sub-slices lie in the top layer: then every piece is checked against one tag in a
+        // register, and the sweeps make no shared-memory loads of the stack)
+        const long long top_start = sm.lay_start[top];
+        const unsigned top_tag = sm.lay_tag[top];
+        const bool in_top = s0 + min(a0, a1) >= top_start;
         const auto want_of = [&](int i) {
+          if (in_top) return top_tag;
           const long long pos = s0 + (i < len0 ? a0 + i : a1 + (i - len0));
           int L = top;
           while (L > 0 && sm.lay_start[L] > pos) --L;
@@ -690,9 +720,8 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
               const unsigned want = want_of(i);
               const uint32_t h0 = static_cast<uint32_t>(w0[j] >> 32), h1 = static_cast<uint32_t>(w1[j] >> 32);
               if (want == LL_TRUSTED || __byte_perm(h0, h1, 0x7632) == want * 0x10001u) {  // (both tags)
-                reinterpret_cast<uint2*>(&sm.parent[i])[pc & 1] =
-                    make_uint2(static_cast<uint32_t>(w0[j]), static_cast<uint32_t>(w1[j]));
-                reinterpret_cast<uint32_t*>(&sm.diag[i])[pc & 1] = __byte_perm(h0, h1, 0x5410);  // ld or rd
+                reinterpret_cast<uint2*>(sm.parent)[pc] = make_uint2(static_cast<uint32_t>(w0[j]), static_cast<uint32_t>(w1[j]));
+                reinterpret_cast<uint32_t*>(sm.diag)[pc] = __byte_perm(h0, h1, 0x5410);  // ld or rd
                 pending &= ~(1u << j);
               }
             }
@@ -787,8 +816,8 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
 #pragma unroll
           for (int u = 0; u < 4; u++) {
             const int x = min(pc + u * T, npc - 1);
-            d[u] = reinterpret_cast<const uint2*>(&sm.stage[x >> 1])[x & 1];
-            dm[u] = reinterpret_cast<const uint32_t*>(&sm.stage_diag[x >> 1])[x & 1];  // ld or rd
+            d[u] = reinterpret_cast<const uint2*>(sm.stage)[x];
+            dm[u] = reinterpret_cast<const uint32_t*>(sm.stage_diag)[x];  // ld or rd
           }
 #pragma unroll
           for (int u = 0; u < 4; u++) {

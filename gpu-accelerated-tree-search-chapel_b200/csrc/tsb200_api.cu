@@ -1068,6 +1068,7 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
     if (rc != TSB_OK) return rc;
   }
   const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
+  std::vector<tsb::RoundsState> pace(prof ? tsb::LL_MAX_POOLS : 0);  // (each pool's record of the last launch)
   for (;;) {
     tsb::LlMultiParams mp;
     std::memset(&mp, 0, sizeof(mp));
@@ -1140,6 +1141,7 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
                      st.prof[tsb::LL_PROF_SCAN] / r, st.prof[tsb::LL_PROF_BUILD] / r, st.prof[tsb::LL_PROF_HAND] / r,
                      st.prof[tsb::LL_PROF_STORE] / r, st.prof[tsb::LL_PROF_X_SCAN] / r, st.prof[tsb::LL_PROF_X_AHEAD] / r,
                      st.prof[tsb::LL_PROF_X_GATHER] / r, st.prof[tsb::LL_PROF_X_TAIL] / r, st.prof[tsb::LL_PROF_X_HAND] / r);
+        pace[a] = st;
       }
       left[i] -= static_cast<int64_t>(st.rounds);
       if (st.exit_code == tsb::RND_EXIT_SPACE) {
@@ -1149,6 +1151,54 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
       } else if (st.exit_code != tsb::RND_EXIT_RELAUNCH) {  // (layer table full: a fresh launch trusts the whole pool)
         active[i] = false;                                    // DONE or PAUSE
       }
+    }
+    if (prof) {
+      // the pace of the launch: it ends when its last pool leaves, so a pool that leaves early idles its CTAs' SMs
+      // share for the rest of it
+      unsigned long long t0 = ~0ull, t1 = 0;
+      for (int a = 0; a < n_act; a++) {
+        t0 = std::min(t0, pace[a].t_start);
+        t1 = std::max(t1, pace[a].t_exit);
+      }
+      for (int a = 0; a < n_act; a++) {
+        const tsb::RoundsState& st = pace[a];
+        const double wall = 1e-3 * static_cast<double>(st.t_exit - st.t_start);
+        std::fprintf(stderr, "[tsb200] LL pace (pool %d of %d, handle %d): start +%.2f us, wall %.2f us, %llu rounds, "
+                     "%.4f us per round, stagger %.2f us, parents %llu, children %llu\n", a, n_act, map[a],
+                     1e-3 * static_cast<double>(st.t_start - t0), wall, static_cast<unsigned long long>(st.rounds),
+                     wall / static_cast<double>(std::max<unsigned long long>(1, st.rounds)),
+                     1e-3 * static_cast<double>(t1 - st.t_exit), static_cast<unsigned long long>(st.parents),
+                     static_cast<unsigned long long>(st.children));
+      }
+      // residency: which pools' CTAs share an SM, and which of them started there first
+      int row_of[2][tsb::LL_MAX_SMS * 2], n_on[tsb::LL_MAX_SMS * 2] = {};
+      unsigned t_of[2][tsb::LL_MAX_SMS * 2];
+      for (int a = 0; a < n_act; a++)
+        for (int c = 0; c < grid; c++) {
+          const unsigned s = pace[a].cta_sm[c] % (tsb::LL_MAX_SMS * 2);
+          if (n_on[s] < 2) {
+            row_of[n_on[s]][s] = a;
+            t_of[n_on[s]][s] = pace[a].cta_t0[c];
+          }
+          n_on[s]++;
+        }
+      int pairs[tsb::LL_MAX_POOLS][tsb::LL_MAX_POOLS] = {}, first[tsb::LL_MAX_POOLS] = {}, over = 0;
+      for (int s = 0; s < tsb::LL_MAX_SMS * 2; s++) {
+        if (n_on[s] > 2) over++;
+        if (n_on[s] < 2) continue;
+        const bool zero_first = static_cast<int>(t_of[1][s] - t_of[0][s]) >= 0;
+        const int lo = std::min(row_of[0][s], row_of[1][s]), hi = std::max(row_of[0][s], row_of[1][s]);
+        pairs[lo][hi]++;
+        first[zero_first ? row_of[0][s] : row_of[1][s]]++;
+      }
+      std::string sh;
+      for (int x = 0; x < n_act; x++)
+        for (int y = x; y < n_act; y++)
+          if (pairs[x][y]) sh += " " + std::to_string(x) + "+" + std::to_string(y) + ": " + std::to_string(pairs[x][y]);
+      std::string fs;
+      for (int x = 0; x < n_act; x++) fs += " " + std::to_string(x) + ": " + std::to_string(first[x]);
+      std::fprintf(stderr, "[tsb200] LL residency: SMs shared by pools%s | started first on a shared SM, by pool%s | SMs "
+                   "with more than two CTAs: %d\n", sh.c_str(), fs.c_str(), over);
     }
   }
   return TSB_OK;
