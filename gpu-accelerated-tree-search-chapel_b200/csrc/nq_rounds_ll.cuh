@@ -104,6 +104,9 @@ struct RoundsState {
   // low 32 bits of %globaltimer at its start
   unsigned long long t_start, t_exit;
   unsigned cta_sm[LL_MAX_SMS], cta_t0[LL_MAX_SMS];
+  // (prm.prof) per CTA k: parents of its sub-slices that had children, and rounds whose children took more than one
+  // staging window (LL_CAP)
+  unsigned cta_fertile[LL_MAX_SMS], cta_wide[LL_MAX_SMS];
 };
 __device__ __forceinline__ unsigned long long ll_globaltimer() {
   unsigned long long t;
@@ -417,12 +420,13 @@ struct LlSmem {
   int poll_abort;                  // a worker's poll gave up: the exchange warp leaves after the scan barrier
   long long prof[LL_PROF_N], prof_t[2];  // (prm.prof, CTA 0) cycles per phase; clock at the end of the last one
                                          // (workers, exchange warp)
+  unsigned prof_fertile, prof_wide;  // (prm.prof, every CTA) parents with children; rounds of more than one window
   long long lay_start[LL_LAYERS];  // the pool's layers, bottom to top: first position ...
   unsigned lay_tag[LL_LAYERS];     // ... and the tag its nodes were stored with (LL_TRUSTED: before the launch)
 };
 
 // child `item` of the slice -> its four data words (board[depth] and board[k] swapped, depth + 1, its child mask
-// evaluated here) and *cdiag its diagonal masks, from its parent's
+// evaluated here over the board words that hold a slot >= depth + 1) and *cdiag its diagonal masks, from its parent's
 template <int N>
 __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2* diag, int item, uint2* cdiag) {
   const int r = item >> 5;
@@ -450,10 +454,17 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
   *cdiag = make_uint2(cld, crd);
   const uint32_t S = ~(cld | crd);  // safe values of row cd
   uint32_t cm = 0;
+  // only slots i >= cd exist (none for a leaf): a data word whose six slots all lie below cd is skipped (word 0 for
+  // children of depth 6 and more, word 1 from depth 12); the slots of the words that are read are masked below
 #pragma unroll
-  for (int i = 0; i < N; i++) {
-    const uint32_t x = shf_r_wrap(S, 0u, P[ll_fw(i)] >> ll_fs(i)) & 1u;  // bit board[i] of S (the shift wraps mod 32)
-    asm("mad.lo.u32 %0, %1, %2, %0;" : "+r"(cm) : "r"(x), "r"(1u << i));  // cm |= x << i on the FMA pipe
+  for (int j = 0; j < 4; j++) {
+    if (6 * j >= N) break;
+    if (6 * j + 6 < N && cd >= static_cast<uint32_t>(6 * j + 6)) continue;
+#pragma unroll
+    for (int i = 6 * j; i < 6 * j + 6 && i < N; i++) {
+      const uint32_t x = shf_r_wrap(S, 0u, P[j] >> ll_fs(i)) & 1u;  // bit board[i] of S (the shift wraps mod 32)
+      asm("mad.lo.u32 %0, %1, %2, %0;" : "+r"(cm) : "r"(x), "r"(1u << i));  // cm |= x << i on the FMA pipe
+    }
   }
   cm &= shl_clamp(0xFFFFFFFFu, cd);  // only slots i >= depth + 1 exist (none for a leaf)
   P[3] = (P[3] & 0x3FFu) | cm << LL_CM_SHIFT | (cd == static_cast<uint32_t>(N) ? LL_LEAF : 0u);
@@ -558,6 +569,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       sm.lay_start[0] = 0;
       sm.lay_tag[0] = LL_TRUSTED;
       sm.poll_abort = 0;
+      sm.prof_fertile = sm.prof_wide = 0;
       if (prm.prof != 0) {
         const unsigned long long now = ll_globaltimer();
         prm.state->cta_sm[k] = ll_smid();
@@ -668,6 +680,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
     if (prof_x) prm.state->t_exit = ll_globaltimer();
   } else {
     // ------------------------------------------------------------------------------------------ the workers
+    unsigned prof_fertile = 0;  // (prm.prof) parents of this thread's records that had children
     for (;;) {
       if (sm.plan.exit >= 0) break;
       const long long s0 = sm.plan.s0;
@@ -751,6 +764,9 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         }
       }
       TSB_PROF(prof_w, 0, LL_PROF_POLL)
+      if (prm.prof != 0)
+#pragma unroll
+        for (int q = 0; q < LL_PPT; q++) prof_fertile += cm[q] != 0u ? 1u : 0u;
       // ---- (3) block scan: children | leaves << 20 | children of the bottom sub-slice << 32 (at most 13 056, 768
       // and 13 056 per CTA: no field overflows into the next)
       unsigned long long incl = static_cast<unsigned long long>(mine) | static_cast<unsigned long long>(leaves) << 20 |
@@ -771,6 +787,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       }
       const int my_children = static_cast<int>(tot & 0xFFFFF);
       const int cnt0 = static_cast<int>(tot >> 32 & 0xFFFFF);
+      if (prm.prof != 0 && t == 0 && my_children > LL_CAP) ++sm.prof_wide;
       {
         uint16_t* it = sm.item + (static_cast<int>((woff + incl) & 0xFFFFF) - mine);
 #pragma unroll
@@ -834,8 +851,13 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       // workers passed, and sm.stage and sm.stage_diag are next written after the next poll's barrier, when every
       // store has read them.)
     }
+    if (prm.prof != 0) atomicAdd(&sm.prof_fertile, prof_fertile);
   }
   __syncthreads();  // (all CTA threads leave the loop at the same round; the profile is complete)
+  if (prm.prof != 0 && t == T) {
+    prm.state->cta_fertile[k] = sm.prof_fertile;
+    prm.state->cta_wide[k] = sm.prof_wide;
+  }
   if (k == 0 && t == T) {
     RoundsState* st = prm.state;
     st->size = size;

@@ -1163,12 +1163,18 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
       for (int a = 0; a < n_act; a++) {
         const tsb::RoundsState& st = pace[a];
         const double wall = 1e-3 * static_cast<double>(st.t_exit - st.t_start);
+        unsigned long long fertile = 0, wide = 0;  // (over the pool's CTAs)
+        for (int c = 0; c < grid; c++) {
+          fertile += st.cta_fertile[c];
+          wide += st.cta_wide[c];
+        }
         std::fprintf(stderr, "[tsb200] LL pace (pool %d of %d, handle %d): start +%.2f us, wall %.2f us, %llu rounds, "
-                     "%.4f us per round, stagger %.2f us, parents %llu, children %llu\n", a, n_act, map[a],
+                     "%.4f us per round, stagger %.2f us, parents %llu, children %llu, parents with children %llu, "
+                     "CTA rounds over one window %llu\n", a, n_act, map[a],
                      1e-3 * static_cast<double>(st.t_start - t0), wall, static_cast<unsigned long long>(st.rounds),
                      wall / static_cast<double>(std::max<unsigned long long>(1, st.rounds)),
                      1e-3 * static_cast<double>(t1 - st.t_exit), static_cast<unsigned long long>(st.parents),
-                     static_cast<unsigned long long>(st.children));
+                     static_cast<unsigned long long>(st.children), fertile, wide);
       }
       // residency: which pools' CTAs share an SM, and which of them started there first
       int row_of[2][tsb::LL_MAX_SMS * 2], n_on[tsb::LL_MAX_SMS * 2] = {};

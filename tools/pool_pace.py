@@ -10,6 +10,8 @@ their CTAs' share of the SMs after they leave.  Per pool (runs after the first, 
   idle          share of the launches' time the pool spent after leaving, waiting for the last pool
   children per parent / per round   from the pool's own counters: does a slow pool do more work per round, or the
                 same work issued more slowly
+  fertile parents   share of the pool's parents that had at least one child (all CTAs)
+  wide CTA rounds   rounds of a CTA whose children took more than one staging window (LL_CAP), summed over CTAs
   phases        CTA 0's cycles per round in each phase (TSB200_ROUNDS_PROF), averaged over the pool's rounds
 and which pools' CTAs share an SM (%smid), with the pool whose CTA started first there."""
 import argparse
@@ -34,13 +36,14 @@ out = subprocess.run(cmd, env=env, stdout=subprocess.PIPE, stderr=subprocess.STD
 PHASE = re.compile(r"LL rounds kernel \(pool (\d+) of (\d+)\): (\d+) rounds; CTA 0 cycles per round: (.*)")
 PACE = re.compile(r"LL pace \(pool (\d+) of (\d+), handle (\d+)\): start \+([\d.]+) us, wall ([\d.]+) us, (\d+) rounds, "
                   r"[\d.]+ us per round, stagger ([\d.]+) us, parents (\d+), children (\d+)")
+EXTRA = re.compile(r"parents with children (\d+), CTA rounds over one window (\d+)")
 RES = re.compile(r"LL residency: (.*)")
 RUN = re.compile(r"N=\d+ M=\d+ K=\d+: .*\s([\d.]+) ms\s")
 
 
 def new_pool():
-    return {"rounds": 0, "wall": 0.0, "idle": 0.0, "span": 0.0, "parents": 0, "children": 0,
-            "phases": collections.Counter()}
+    return {"rounds": 0, "wall": 0.0, "idle": 0.0, "span": 0.0, "parents": 0, "children": 0, "fertile": 0,
+            "wide": 0, "phases": collections.Counter()}
 
 
 pools = collections.defaultdict(new_pool)
@@ -61,13 +64,13 @@ for line in out.splitlines():
         continue
     m = PACE.search(line)
     if m:
-        launch.append(m)
+        launch.append((m, EXTRA.search(line)))
         continue
     m = RES.search(line)
     if m:
         if launch and run > 0:
-            span = max(float(x.group(5)) + float(x.group(4)) + float(x.group(7)) for x in launch)
-            for x in launch:
+            span = max(float(x.group(5)) + float(x.group(4)) + float(x.group(7)) for x, _ in launch)
+            for x, ex in launch:
                 p = pools[int(x.group(3))]
                 r = int(x.group(6))
                 p["rounds"] += r
@@ -76,6 +79,9 @@ for line in out.splitlines():
                 p["span"] += span
                 p["parents"] += int(x.group(8))
                 p["children"] += int(x.group(9))
+                if ex:
+                    p["fertile"] += int(ex.group(1))
+                    p["wide"] += int(ex.group(2))
                 pr, ph = phase_of.get(int(x.group(1)), (0, {}))
                 for k, v in ph.items():
                     p["phases"][k] += v * pr
@@ -90,12 +96,14 @@ for line in out.splitlines():
         print(line)
 
 print(f"\nN={N} M={M} K={K}: {len(runs_ms)} runs after the first: " + ", ".join(f"{x:.1f}" for x in runs_ms) + " ms")
-print(f"{'pool':>4} {'rounds':>9} {'period us':>10} {'cycles':>8} {'idle':>6} {'children/parent':>16} {'children/round':>15}")
+print(f"{'pool':>4} {'rounds':>9} {'period us':>10} {'cycles':>8} {'idle':>6} {'children/parent':>16} {'children/round':>15} "
+      f"{'fertile parents':>16} {'wide CTA rounds':>16}")
 for h in sorted(pools):
     p = pools[h]
     per = p["wall"] / max(1, p["rounds"])
     print(f"{h:>4} {p['rounds']:>9} {per:>10.4f} {per * a.mhz:>8.0f} {p['idle'] / max(p['span'], 1e-9):>6.1%} "
-          f"{p['children'] / max(1, p['parents']):>16.4f} {p['children'] / max(1, p['rounds']):>15.0f}")
+          f"{p['children'] / max(1, p['parents']):>16.4f} {p['children'] / max(1, p['rounds']):>15.0f} "
+          f"{p['fertile'] / max(1, p['parents']):>16.2%} {p['wide']:>16}")
 names = list(dict.fromkeys(k for p in pools.values() for k in p["phases"]))  # (in the order of a round)
 if names:
     print("\nCTA 0 cycles per round by phase (x: exchange warp)")
