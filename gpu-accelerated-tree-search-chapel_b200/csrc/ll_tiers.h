@@ -10,7 +10,8 @@ constexpr int LL_MAX_SMS = 256;  // CTAs per pool at most (the count slots of a 
 constexpr int LL_SLICE2 = 512;   // parents per CTA with two parents per thread (256 threads)
 constexpr int LL_SLICE3 = 768;   // ... with three
 
-// CTAs per pool when one launch serves `pools` pools: one pool: one CTA per SM; several: two CTAs per SM in all
+// CTAs per pool when one launch serves `pools` pools: one pool: one CTA per SM; several: two pools' CTAs per SM in all
+// (with four pools, as the two halves of one CTA: nq_rounds_ll_kernel)
 constexpr int ll_ctas_per_pool(int sms, int pools) {
   return pools <= 1 ? (sms < LL_MAX_SMS ? sms : LL_MAX_SMS) : 2 * (sms < LL_MAX_SMS ? sms : LL_MAX_SMS) / pools;
 }

@@ -72,8 +72,9 @@
 //
 // One launch serves up to LL_MAX_POOLS INDEPENDENT pools (grid (G, pools), LlMultiParams): even so a pool's round stays
 // a chain of L2 round trips with little work in between, and nothing inside one pool can fill the waits — another
-// pool's CTA on the same SM can: on the N = 17 search at M = 50000 three or four pools per launch (two CTAs per SM in
-// all, 768 parents per CTA) take little more than half the time of one pool.
+// pool's CTA on the same SM can: on the N = 17 search at M = 50000 three or four pools per launch (two pools per SM in
+// all, 768 parents per CTA) take little more than half the time of one pool.  Four pools run as grid (G, 2) of CTAs
+// that each hold two pools' CTAs as halves (HALVES, above nq_rounds_ll_kernel).
 //
 // A spin loop that waits longer than ~2 s raises a global abort flag and every CTA leaves (exit code ABORT): a logic
 // error must never hang the GPU.
@@ -198,9 +199,9 @@ struct LlMultiParams {
 };
 
 // ---- named barriers of the persistent kernel: LL_BAR_W among the worker warps only, LL_BAR_SCAN workers -> exchange
-// warp (bar.arrive / bar.sync: the counts are scanned), LL_BAR_HAND exchange warp <-> workers (the handoff)
-constexpr int LL_BAR_W = 1, LL_BAR_SCAN = 2, LL_BAR_HAND = 3;
-__device__ __forceinline__ void ll_bar(int threads) { asm volatile("bar.sync %0, %1;" ::"n"(LL_BAR_W), "r"(threads) : "memory"); }
+// warp (bar.arrive / bar.sync: the counts are scanned), LL_BAR_HAND exchange warp <-> workers (the handoff, and the
+// start and the end of the kernel).  The second half of a two-pool CTA uses the same three ids + LL_BAR_HALF.
+constexpr int LL_BAR_W = 1, LL_BAR_SCAN = 2, LL_BAR_HAND = 3, LL_BAR_HALF = 3;
 __device__ __forceinline__ void ll_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 __device__ __forceinline__ void ll_wait(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 __device__ __forceinline__ bool ll_bar_or(int id, int threads, bool pred) {
@@ -483,14 +484,29 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
 // workers' chain: after their stores they go straight into the next poll.  Between the last slot's arrival and the
 // handoff only the sums, a range test and a few shared-memory stores remain.  The pool state (size, epoch, layers,
 // counters) is the exchange warp's alone; the workers get what they need through sm.plan.
-template <int N, int T, int MINB, int PPT>
-__global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid_constant__ LlMultiParams mprm) {
-  const LlParams& prm = mprm.pool[blockIdx.y];
+//
+// HALVES = 2 (four pools per launch): a CTA of 2 (T + 32) threads runs two pools, one per HALF, so no pool is the
+// second CTA on its SMs.  Half h is threads [h TX, (h + 1) TX) = warps 9h .. 9h + 8 and runs pool blockIdx.y + 2h
+// exactly as a CTA of HALVES = 1 would: its own LlSmem (the second right after the first), its own barrier ids
+// (+ LL_BAR_HALF), no barrier over the whole CTA; a half whose pool has left has exited.  Pools 0 + 2 and 1 + 3 share
+// a CTA: in the steps where pools run dry (the host's steals), 0 and 1 or 2 and 3 leave early together, and the two
+// that run on then hold one SM each, where pairs 0 + 1 / 2 + 3 would leave them sharing half the SMs while the other
+// half idles (DESIGN §5).  The warps of an SM's
+// sub-partition are those of equal warp id mod 4: nine warps per half put both halves' warps on every sub-partition,
+// two workers of each half on each, the exchange warps (8 and 17) on sub-partitions 0 and 1.  With two CTAs per SM the
+// CTA that became resident second ran the slower pool (DESIGN §5).
+template <int N, int T, int MINB, int PPT, int HALVES = 1>
+__global__ void __launch_bounds__(HALVES * (T + 32), MINB) nq_rounds_ll_kernel(const __grid_constant__ LlMultiParams mprm) {
+  static_assert(HALVES == 1 || (HALVES == 2 && MINB == 1), "two pools per CTA: one CTA per SM");
   constexpr int LL_PPT = PPT;
-  constexpr int TX = T + 32;  // the whole CTA: workers + exchange warp
+  constexpr int TX = T + 32;  // the whole CTA (HALVES = 1) or half: workers + exchange warp
+  const int half = HALVES == 2 && threadIdx.x >= TX ? 1 : 0;
+  const LlParams& prm = mprm.pool[blockIdx.y + gridDim.y * half];
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  LlSmem<T, PPT>& sm = *reinterpret_cast<LlSmem<T, PPT>*>(smem_raw);
-  const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  LlSmem<T, PPT>& sm = reinterpret_cast<LlSmem<T, PPT>*>(smem_raw)[half];
+  const int bar_w = LL_BAR_W + LL_BAR_HALF * half, bar_scan = LL_BAR_SCAN + LL_BAR_HALF * half,
+            bar_hand = LL_BAR_HAND + LL_BAR_HALF * half;
+  const int t = threadIdx.x - TX * half, lane = t & 31, wid = t >> 5;
   const int k = blockIdx.x, G = gridDim.x, G2 = 2 * G;
   LlSync* const sy = prm.sync;
   FatNode* const fat = prm.fat;
@@ -581,14 +597,14 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
     }
     exit_code = plan();
   }
-  __syncthreads();
+  ll_bar_or(bar_hand, TX, false);  // (sm.plan of the first round)
   if (prm.prof != 0 && k == 0 && (t == 0 || t == T)) sm.prof_t[t == T] = clock64();
 
   if (wid == T / 32) {
     // ------------------------------------------------------------------------------------------ the exchange warp
     const LlLaneSlots lane_slots = ll_lane_slots(G2, k, G2 - 1 - k);
     while (exit_code < 0) {
-      ll_wait(LL_BAR_SCAN, TX);  // the workers' warp totals are in sm.warp_tot64 (they have read their slices)
+      ll_wait(bar_scan, TX);  // the workers' warp totals are in sm.warp_tot64 (they have read their slices)
       TSB_PROF(prof_x, 1, LL_PROF_X_SCAN)
       if (sm.poll_abort) {
         exit_code = RND_EXIT_ABORT;
@@ -666,7 +682,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         }
       }
       TSB_PROF(prof_x, 1, LL_PROF_X_TAIL)
-      if (ll_bar_or(LL_BAR_HAND, TX, !ok)) {  // the handoff (an abort reaches the workers here)
+      if (ll_bar_or(bar_hand, TX, !ok)) {  // the handoff (an abort reaches the workers here)
         exit_code = RND_EXIT_ABORT;
         break;
       }
@@ -744,9 +760,9 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
           }
         }
       }
-      if (ll_bar_or(LL_BAR_W, T, !ok)) {  // the slice is in shared memory
+      if (ll_bar_or(bar_w, T, !ok)) {  // the slice is in shared memory
         if (t == 0) sm.poll_abort = 1;
-        ll_arrive(LL_BAR_SCAN, TX);  // (the exchange warp waits there, sees the flag and leaves too)
+        ll_arrive(bar_scan, TX);  // (the exchange warp waits there, sees the flag and leaves too)
         break;
       }
       uint32_t cm[LL_PPT];
@@ -777,8 +793,8 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
         if (lane >= o) incl += y;
       }
       if (lane == 31) sm.warp_tot64[wid] = incl;
-      ll_arrive(LL_BAR_SCAN, TX);  // the exchange warp publishes the totals and gathers everybody's
-      ll_bar(T);
+      ll_arrive(bar_scan, TX);  // the exchange warp publishes the totals and gathers everybody's
+      ll_wait(bar_w, T);
       unsigned long long woff = 0, tot = 0;
 #pragma unroll
       for (int i = 0; i < T / 32; i++) {
@@ -800,7 +816,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
           }
         }
       }
-      ll_bar(T);  // items complete
+      ll_wait(bar_w, T);  // items complete
       TSB_PROF(prof_w, 0, LL_PROF_SCAN)
       // ---- (5) my children (first window), built and evaluated while the other CTAs' counts are on their way
       auto build_window = [&](int c0, int cnt) {
@@ -810,7 +826,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       build_window(0, min(LL_CAP, my_children));
       TSB_PROF(prof_w, 0, LL_PROF_BUILD)
       // ---- the handoff: my offsets from the exchange warp (also: the first window is complete)
-      if (ll_bar_or(LL_BAR_HAND, TX, false)) break;  // (an abort of the gather)
+      if (ll_bar_or(bar_hand, TX, false)) break;  // (an abort of the gather)
       TSB_PROF(prof_w, 0, LL_PROF_HAND)
       const int off0 = sm.plan.off0, off1 = sm.plan.off1;
 
@@ -819,9 +835,9 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
       for (int c0 = 0; c0 < my_children; c0 += LL_CAP) {
         const int cnt = min(LL_CAP, my_children - c0);
         if (c0 > 0) {
-          ll_bar(T);  // the previous window has been copied out
+          ll_wait(bar_w, T);  // the previous window has been copied out
           build_window(c0, cnt);
-          ll_bar(T);
+          ll_wait(bar_w, T);
         }
         // child c of my share goes to position s0 + off0 + c (bottom sub-slice) or s0 + off1 + (c - cnt0) (top one)
         unsigned long long* const dst0 = fat[s0 + off0 + c0].w;
@@ -853,7 +869,7 @@ __global__ void __launch_bounds__(T + 32, MINB) nq_rounds_ll_kernel(const __grid
     }
     if (prm.prof != 0) atomicAdd(&sm.prof_fertile, prof_fertile);
   }
-  __syncthreads();  // (all CTA threads leave the loop at the same round; the profile is complete)
+  ll_bar_or(bar_hand, TX, false);  // (all threads of the half leave the loop at the same round; the profile is complete)
   if (prm.prof != 0 && t == T) {
     prm.state->cta_fertile[k] = sm.prof_fertile;
     prm.state->cta_wide[k] = sm.prof_wide;

@@ -965,18 +965,24 @@ bool nq_nodes_valid(int N, const tsb_nq_node* nodes, int64_t n) {
 
 template <int N>
 int nq_ll_launch_n(tsb_nq* h, const tsb::LlMultiParams& prm, int grid, int pools, int ppt, cudaStream_t s) {
-  // (one pool: one CTA per SM; several: two CTAs of LL_T workers + the exchange warp per SM, capped at 112
-  // registers; three or four pools: 66 CTAs per pool with 768 parents each on 132 SMs, see ll_slice)
-  const int var = pools == 1 ? 0 : ppt == 2 ? 1 : 2;
+  // (one pool: one CTA per SM; two or three: two CTAs of LL_T workers + the exchange warp per SM, capped at 112
+  // registers; three or four pools: 66 CTAs per pool with 768 parents each on 132 SMs, see ll_slice.  Four pools:
+  // one CTA per SM of two such halves, each running one pool (nq_rounds_ll_kernel, HALVES = 2), grid (grid, 2).)
+  const int halves = pools == tsb::LL_MAX_POOLS ? 2 : 1;
+  const int var = pools == 1 ? 0 : (ppt == 2 ? 1 : 2) + (halves == 2 ? 2 : 0);
   auto kernel = var == 0   ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 2>
                 : var == 1 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 2>
-                           : tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 3>;
-  const size_t smem = (ppt == 2 ? sizeof(tsb::LlSmem<tsb::LL_T, 2>) : sizeof(tsb::LlSmem<tsb::LL_T, 3>)) + 128;
+                : var == 2 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 3>
+                : var == 3 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 2, 2>
+                           : tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 3, 2>;
+  static_assert(2 * sizeof(tsb::LlSmem<tsb::LL_T, 3>) + 128 <= 227 * 1024, "two halves' shared memory in one CTA");
+  const size_t smem = halves * (ppt == 2 ? sizeof(tsb::LlSmem<tsb::LL_T, 2>) : sizeof(tsb::LlSmem<tsb::LL_T, 3>)) + 128;
   int rc = h->configure(kernel, smem);
   if (rc != TSB_OK) return rc;
   void* args[] = {const_cast<tsb::LlMultiParams*>(&prm)};
-  // cooperative: all CTAs of all pools co-resident (two per SM when there are two pools), or the launch fails
-  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid, pools), dim3(tsb::LL_T + 32), args, smem, s));
+  // cooperative: all CTAs of all pools co-resident (two per SM when there are two or three pools), or the launch fails
+  TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid, pools / halves),
+                                       dim3(halves * (tsb::LL_T + 32)), args, smem, s));
   h->launches++;
   return TSB_OK;
 }
@@ -1168,13 +1174,17 @@ int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, 
           fertile += st.cta_fertile[c];
           wide += st.cta_wide[c];
         }
+        // why the pool left: its round budget, fewer than m nodes, a relaunch (layer table or tag window), arena room
+        static const char* const why[] = {"dry", "budget", "space", "abort", "relaunch"};
         std::fprintf(stderr, "[tsb200] LL pace (pool %d of %d, handle %d): start +%.2f us, wall %.2f us, %llu rounds, "
                      "%.4f us per round, stagger %.2f us, parents %llu, children %llu, parents with children %llu, "
-                     "CTA rounds over one window %llu\n", a, n_act, map[a],
+                     "CTA rounds over one window %llu, exit %s, globaltimer %llu..%llu ns\n", a, n_act, map[a],
                      1e-3 * static_cast<double>(st.t_start - t0), wall, static_cast<unsigned long long>(st.rounds),
                      wall / static_cast<double>(std::max<unsigned long long>(1, st.rounds)),
                      1e-3 * static_cast<double>(t1 - st.t_exit), static_cast<unsigned long long>(st.parents),
-                     static_cast<unsigned long long>(st.children), fertile, wide);
+                     static_cast<unsigned long long>(st.children), fertile, wide,
+                     st.exit_code >= 0 && st.exit_code <= tsb::RND_EXIT_RELAUNCH ? why[st.exit_code] : "?", st.t_start,
+                     st.t_exit);
       }
       // residency: which pools' CTAs share an SM, and which of them started there first
       int row_of[2][tsb::LL_MAX_SMS * 2], n_on[tsb::LL_MAX_SMS * 2] = {};

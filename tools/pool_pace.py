@@ -12,8 +12,10 @@ their CTAs' share of the SMs after they leave.  Per pool (runs after the first, 
                 same work issued more slowly
   fertile parents   share of the pool's parents that had at least one child (all CTAs)
   wide CTA rounds   rounds of a CTA whose children took more than one staging window (LL_CAP), summed over CTAs
-  phases        CTA 0's cycles per round in each phase (TSB200_ROUNDS_PROF), averaged over the pool's rounds
-and which pools' CTAs share an SM (%smid), with the pool whose CTA started first there."""
+  phases        the cycles per round in each phase of the pool's CTA 0 (of its half of CTA 0 with four pools, which
+                share a CTA two by two: nq_rounds_ll_kernel's HALVES), averaged over the pool's rounds
+and which pools share an SM (%smid): two CTAs of different pools with two or three pools per launch, with the pool
+whose CTA started first there; the two halves of one CTA with four."""
 import argparse
 import collections
 import os
