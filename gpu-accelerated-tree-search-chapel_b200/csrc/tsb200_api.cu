@@ -616,13 +616,13 @@ struct Base {
   }
 };
 
-// f(std::integral_constant<int, N>) for the board size N = 1..TSB_MAX_QUEENS
-template <int N = 1, class F>
+// f(std::integral_constant<int, N>) for the board size N = 1..MAXN
+template <int N = 1, int MAXN = TSB_MAX_QUEENS, class F>
 int with_queens(int n, F&& f) {
-  if constexpr (N > TSB_MAX_QUEENS)
+  if constexpr (N > MAXN)
     return TSB_EINVAL;
   else
-    return n == N ? f(std::integral_constant<int, N>{}) : with_queens<N + 1>(n, f);
+    return n == N ? f(std::integral_constant<int, N>{}) : with_queens<N + 1, MAXN>(n, f);
 }
 // f(std::integral_constant<int, M>) for the template machine count mt = 5, 10 or 20
 template <class F>
@@ -843,6 +843,7 @@ void enable_peer(int a, int b) {
 struct tsb_nq : Base {
   tsb_nq* sibling[3] = {nullptr, nullptr, nullptr};  // further pools on the same device, owned by this handle (tsb_nq_sibling)
   int N = 0, g = 1;
+  bool wide = false;  // MAX_QUEENS = 24 build (tsb_nq_create_wide): 25-byte tsb_nq_node24 records, no persistent kernel
   int tile_threads = 0;  // env TSB200_NQ_TILE_THREADS = 128: always the TMA-pipelined kernel (tests force it on small chunks)
   tsb::FatNode* d_fat = nullptr;  // the pool in the self-validating 32-byte format, while the LL kernel owns it
   long long fat_cap = 0;
@@ -871,19 +872,27 @@ struct tsb_pfsp : Base {
 namespace {
 
 // ============================================================================ N-Queens
+// f(std::integral_constant<int, N>, std::integral_constant<int, R>) for the handle's board size N and record width R
+template <class F>
+int with_board(const tsb_nq* h, F&& f) {
+  if (h->wide)
+    return with_queens<1, TSB_MAX_QUEENS_WIDE>(h->N, [&](auto n) { return f(n, std::integral_constant<int, tsb::NQ_REC24>{}); });
+  return with_queens(h->N, [&](auto n) { return f(n, std::integral_constant<int, tsb::NQ_REC>{}); });
+}
+
 // small chunks (fewer than two 512-parent tiles per SM — the reference's default --M 50000 is 97 tiles) take the
 // one-parent-per-thread kernel, everything else the TMA-pipelined one
-template <int N>
+template <int N, int R>
 int launch_nq_n(tsb_nq* h, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
   if (count < 2LL * h->di.sms * tsb::NQ_TILE && h->tile_threads != 128) {
     const int grid = static_cast<int>((count + tsb::NQ_SMALL - 1) / tsb::NQ_SMALL);
-    tsb::nq_evaluate_small_kernel<N><<<grid, tsb::NQ_SMALL, 0, s>>>(in, out, static_cast<int>(count));
+    tsb::NqKernels<N, R>::evaluate_small<<<grid, tsb::NQ_SMALL, 0, s>>>(in, out, static_cast<int>(count));
     TSB_CUDA(cudaGetLastError());
     h->launches++;
     return TSB_OK;
   }
-  auto kernel = tsb::nq_evaluate_kernel<N>;
-  const size_t smem = sizeof(tsb::NqSmem<N>) + 128;
+  auto kernel = tsb::NqKernels<N, R>::evaluate;
+  const size_t smem = sizeof(tsb::NqSmem<N, R>) + 128;
   int grid = 1;
   int rc = h->grid_for(kernel, tsb::NQ_THREADS, smem, count, tsb::NQ_TILE, &grid);
   if (rc != TSB_OK) return rc;
@@ -894,12 +903,12 @@ int launch_nq_n(tsb_nq* h, const uint8_t* in, uint8_t* out, long long count, cud
 }
 
 int launch_nq(tsb_nq* h, const uint8_t* in, uint8_t* out, long long count, cudaStream_t s) {
-  return with_queens(h->N, [&](auto n) { return launch_nq_n<decltype(n)::value>(h, in, out, count, s); });
+  return with_board(h, [&](auto n, auto r) { return launch_nq_n<decltype(n)::value, decltype(r)::value>(h, in, out, count, s); });
 }
 
 // one evaluate + generate_children round over `pieces` of `arena` (count, build); children packed at
 // `children_d`.  Synchronous: the counts come back through the host-mapped result record.
-template <int N>
+template <int N, int R>
 int nq_expand_n(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& pieces, uint8_t* children_d,
                 cudaStream_t s, unsigned long long* n_children, unsigned long long* n_solutions, bool early) {
   tsb::ExpandParams prm;
@@ -913,9 +922,9 @@ int nq_expand_n(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& 
   rc = ex.reserve(std::max<long long>(prm.n_tiles, h->M_max / tsb::NQ_TILE + 2 * tsb::EXP_MAX_PIECES),
                   static_cast<long long>(tsb::NQ_TILE) * N * 2, s);
   if (rc != TSB_OK) return rc;
-  auto k1 = tsb::nq_expand_count_kernel<N>;
-  auto k3 = tsb::nq_expand_build_kernel<N>;
-  const size_t smem1 = sizeof(tsb::NqCountSmem) + 128, smem3 = sizeof(tsb::NqBuildSmem) + 128;
+  auto k1 = tsb::NqKernels<N, R>::count;
+  auto k3 = tsb::NqKernels<N, R>::build;
+  const size_t smem1 = sizeof(tsb::NqCountSmem<R>) + 128, smem3 = sizeof(tsb::NqBuildSmem<R>) + 128;
   const long long recs = static_cast<long long>(prm.n_tiles) * tsb::NQ_TILE;
   int g1 = 1, g3 = 1;
   rc = h->grid_for(k1, tsb::NQ_THREADS, smem1, recs, tsb::NQ_TILE, &g1);
@@ -946,19 +955,20 @@ int nq_expand_n(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& 
 
 int nq_expand(tsb_nq* h, const uint8_t* arena, const std::vector<PoolExtent>& pieces, uint8_t* children_d,
               cudaStream_t s, unsigned long long* nc, unsigned long long* ns, bool early = false) {
-  return with_queens(h->N, [&](auto n) {
-    return nq_expand_n<decltype(n)::value>(h, arena, pieces, children_d, s, nc, ns, early);
+  return with_board(h, [&](auto n, auto r) {
+    return nq_expand_n<decltype(n)::value, decltype(r)::value>(h, arena, pieces, children_d, s, nc, ns, early);
   });
 }
 
 // what a pool may hold: depth <= N, board[0..N) < N, the bytes past N zero (every node the reference or this library
-// creates; the persistent kernel packs a node into 125 bits on these terms, nq_rounds_ll.cuh)
-bool nq_nodes_valid(int N, const tsb_nq_node* nodes, int64_t n) {
+// creates; the persistent kernel packs a node into 125 bits on these terms, nq_rounds_ll.cuh).  `rec`-byte records:
+// {depth, board[rec - 1]}.
+bool nq_nodes_valid(int N, size_t rec, const uint8_t* nodes, int64_t n) {
   for (int64_t i = 0; i < n; i++) {
-    const tsb_nq_node& x = nodes[i];
-    if (x.depth > N) return false;
-    for (int j = 0; j < TSB_MAX_QUEENS; j++)
-      if (x.board[j] >= (j < N ? N : 1)) return false;
+    const uint8_t* x = nodes + static_cast<size_t>(i) * rec;
+    if (x[0] > N) return false;
+    for (size_t j = 0; j + 1 < rec; j++)
+      if (x[1 + j] >= (static_cast<int>(j) < N ? N : 1)) return false;
   }
   return true;
 }
@@ -1050,7 +1060,8 @@ int nq_materialize(tsb_nq* h) {
 // the other way.
 // *ppt: parents per thread of the kernel variant to launch (2, or 3 when the pool's CTAs would not cover M with 2).
 int nq_ll_grid(const tsb_nq* h, int M, int pools, int* ppt = nullptr) {
-  if (!h->di.coop || env_no_rounds() || pools < 1 || pools > tsb::LL_MAX_POOLS) return 0;
+  // (a wide handle's 24-queen boards do not fit the 32-byte nodes of the persistent kernel: two-kernel rounds)
+  if (h->wide || !h->di.coop || env_no_rounds() || pools < 1 || pools > tsb::LL_MAX_POOLS) return 0;
   const int sms = std::min(h->di.sms, tsb::LL_MAX_SMS);
   const int most = tsb::ll_ctas_per_pool(sms, pools);  // (ll_tiers.h: the drivers size their warm-up by the same tiers)
   const int per = static_cast<long long>(most) * tsb::ll_slice(2) >= M ? 2 : 3;
@@ -1762,16 +1773,18 @@ int tsb_debug_flag_exchange(int device, int rounds, int variant, int ctas, doubl
 }
 
 // ---------------------------------------------------------------- N-Queens
-int tsb_nq_create(tsb_nq** out, int device, int N, int g, int M_max) {
-  if (!out || N < 1 || N > TSB_MAX_QUEENS || g < 1 || M_max < 1) return TSB_EINVAL;
+static int nq_create(tsb_nq** out, int device, bool wide, int N, int g, int M_max) {
+  if (!out || N < 1 || N > (wide ? TSB_MAX_QUEENS_WIDE : TSB_MAX_QUEENS) || g < 1 || M_max < 1) return TSB_EINVAL;
   tsb_nq* h = new (std::nothrow) tsb_nq();
   if (!h) return TSB_ENOMEM;
   h->N = N;
   h->g = g;
+  h->wide = wide;
   if (const char* v = std::getenv("TSB200_NQ_TILE_THREADS")) h->tile_threads = std::atoi(v);
+  const size_t rec = wide ? sizeof(tsb_nq_node24) : sizeof(tsb_nq_node);
   // (the arena starts with room for four worst-case rounds: every slot of every parent survives)
-  h->pool.set_format(sizeof(tsb_nq_node), tsb::NQ_TILE, 1, N, std::max<long long>(1LL << 22, 4LL * M_max * N));
-  int rc = h->init(device, M_max, sizeof(tsb_nq_node), static_cast<size_t>(N));
+  h->pool.set_format(rec, tsb::NQ_TILE, 1, N, std::max<long long>(1LL << 22, 4LL * M_max * N));
+  int rc = h->init(device, M_max, rec, static_cast<size_t>(N));
   if (rc != TSB_OK) {
     h->fini();
     delete h;
@@ -1779,6 +1792,11 @@ int tsb_nq_create(tsb_nq** out, int device, int N, int g, int M_max) {
   }
   *out = h;
   return TSB_OK;
+}
+int tsb_nq_create(tsb_nq** out, int device, int N, int g, int M_max) { return nq_create(out, device, false, N, g, M_max); }
+int tsb_nq_create_wide(tsb_nq** out, int device, int max_queens, int N, int g, int M_max) {
+  if (max_queens != TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
+  return nq_create(out, device, true, N, g, M_max);
 }
 
 void tsb_nq_destroy(tsb_nq* h) {
@@ -1824,7 +1842,7 @@ int tsb_nq_expand(tsb_nq* h, const void* parents, int count, void* children, uin
 
 int tsb_nq_pool_push(tsb_nq* h, const void* nodes, int64_t n) {
   if (!h || n < 0 || (n && !nodes)) return TSB_EINVAL;
-  if (!nq_nodes_valid(h->N, static_cast<const tsb_nq_node*>(nodes), n)) return TSB_EINVAL;
+  if (!nq_nodes_valid(h->N, h->pool.rec, static_cast<const uint8_t*>(nodes), n)) return TSB_EINVAL;
   return pool_push(*h, nodes, n, [h] { return nq_materialize(h); });
 }
 
@@ -1864,7 +1882,7 @@ int tsb_nq_pool_run(tsb_nq* h, int m, int M, int64_t max_rounds, uint64_t* n_rou
 int tsb_nq_sibling(tsb_nq* h, int index, tsb_nq** sibling) {
   if (!h || !sibling || index < 1 || index >= tsb::LL_MAX_POOLS) return TSB_EINVAL;
   if (!h->sibling[index - 1]) {
-    int rc = tsb_nq_create(&h->sibling[index - 1], h->device, h->N, h->g, h->M_max);
+    int rc = nq_create(&h->sibling[index - 1], h->device, h->wide, h->N, h->g, h->M_max);
     if (rc != TSB_OK) return rc;
   }
   *sibling = h->sibling[index - 1];
@@ -1882,7 +1900,8 @@ int tsb_nq_pool_run_multi(tsb_nq* const* handles, int n_pools, int m, int M, int
   if (!handles || n_pools < 1 || n_pools > tsb::LL_MAX_POOLS || m < 1 || M < 1 || max_rounds < 0 || !out) return TSB_EINVAL;
   for (int i = 0; i < n_pools; i++) {
     const tsb_nq* h = handles[i];
-    if (!h || M > h->M_max || h->device != handles[0]->device || h->N != handles[0]->N) return TSB_EINVAL;
+    if (!h || M > h->M_max || h->device != handles[0]->device || h->N != handles[0]->N || h->wide != handles[0]->wide)
+      return TSB_EINVAL;
     for (int j = 0; j < i; j++)
       if (handles[j] == h) return TSB_EINVAL;
   }
@@ -1899,7 +1918,8 @@ int tsb_nq_pool_run_multi(tsb_nq* const* handles, int n_pools, int m, int M, int
 }
 
 int tsb_nq_pool_steal(tsb_nq* victim, tsb_nq* thief, int m, int64_t* n_stolen) {
-  if (!victim || !thief || victim == thief || m < 1 || !n_stolen || victim->N != thief->N) return TSB_EINVAL;
+  if (!victim || !thief || victim == thief || m < 1 || !n_stolen || victim->N != thief->N || victim->wide != thief->wide)
+    return TSB_EINVAL;
   return pool_steal(*victim, *thief, m, n_stolen, [victim, thief] {
     const int rc = nq_materialize(victim);
     return rc == TSB_OK ? nq_materialize(thief) : rc;
@@ -1956,6 +1976,10 @@ uint64_t tsb_nq_kernel_launches(const tsb_nq* h) {
   return n;
 }
 void* tsb_nq_stream(const tsb_nq* h) { return h ? static_cast<void*>(h->stream) : nullptr; }
+int tsb_nq_max_queens(const tsb_nq* h) {
+  if (!h) return TSB_EINVAL;
+  return h->wide ? TSB_MAX_QUEENS_WIDE : TSB_MAX_QUEENS;
+}
 
 // ---------------------------------------------------------------- PFSP
 int tsb_pfsp_create(tsb_pfsp** out, int device, int jobs, int machines, int M_max, const int32_t* p_times,

@@ -19,6 +19,7 @@
 #include <condition_variable>
 #include <mutex>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "ll_tiers.h"
@@ -91,15 +92,25 @@ struct Pool {
 };
 
 // ------------------------------------------------------------------ N-Queens CPU twin
+// Node: tsb_nq_node (N <= 20, tsb_nq_create handles) or tsb_nq_node24 (a MAX_QUEENS = 24 build, tsb_nq_create_wide)
+template <class Node>
+int nq_create_for(tsb_nq** h, int device, int N, int g, int M) {
+  if constexpr (std::is_same_v<Node, tsb_nq_node24>)
+    return tsb_nq_create_wide(h, device, TSB_MAX_QUEENS_WIDE, N, g, M);
+  else
+    return tsb_nq_create(h, device, N, g, M);
+}
 // isSafe / decompose of the drivers' CPU steps 1 and 3 (nqueens_gpu_chpl.chpl:51-89)
-inline bool nq_safe(const tsb_nq_node& p, int depth, int row_pos) {
+template <class Node>
+inline bool nq_safe(const Node& p, int depth, int row_pos) {
   for (int i = 0; i < depth; i++) {
     const int d = depth - i, o = p.board[i];
     if (o == row_pos - d || o == row_pos + d) return false;
   }
   return true;
 }
-void nq_decompose(int N, const tsb_nq_node& parent, uint64_t& tree, uint64_t& sol, Pool<tsb_nq_node>& pool) {
+template <class Node>
+void nq_decompose(int N, const Node& parent, uint64_t& tree, uint64_t& sol, Pool<Node>& pool) {
   const int depth = parent.depth;
   if (depth == N) {
     ++sol;
@@ -107,7 +118,7 @@ void nq_decompose(int N, const tsb_nq_node& parent, uint64_t& tree, uint64_t& so
   }
   for (int j = depth; j < N; j++)
     if (nq_safe(parent, depth, parent.board[j])) {
-      tsb_nq_node c = parent;
+      Node c = parent;
       c.depth = static_cast<uint8_t>(depth + 1);
       std::swap(c.board[depth], c.board[j]);
       pool.pushBack(c);
@@ -115,10 +126,11 @@ void nq_decompose(int N, const tsb_nq_node& parent, uint64_t& tree, uint64_t& so
     }
 }
 // nqueens_gpu_chpl.chpl:126-149
-void nq_generate_children(int N, const tsb_nq_node* parents, int size, const uint8_t* labels, uint64_t& tree,
-                          uint64_t& sol, Pool<tsb_nq_node>& pool) {
+template <class Node>
+void nq_generate_children(int N, const Node* parents, int size, const uint8_t* labels, uint64_t& tree, uint64_t& sol,
+                          Pool<Node>& pool) {
   for (int i = 0; i < size; i++) {
-    const tsb_nq_node& parent = parents[i];
+    const Node& parent = parents[i];
     const int depth = parent.depth;
     if (depth == N) {
       ++sol;
@@ -127,7 +139,7 @@ void nq_generate_children(int N, const tsb_nq_node* parents, int size, const uin
     const uint8_t* lab = labels + static_cast<size_t>(i) * N;
     for (int j = depth; j < N; j++)
       if (lab[j] == 1) {
-        tsb_nq_node c = parent;
+        Node c = parent;
         c.depth = static_cast<uint8_t>(depth + 1);
         std::swap(c.board[depth], c.board[j]);
         pool.pushBack(c);
@@ -147,14 +159,15 @@ inline void bind_task(int device, bool multi) {  // one host thread per GPU: nex
   if (multi && !std::getenv("TSB200_NO_NUMA")) (void)tsb_bind_thread_to_device(device);
 }
 
-void nq_gpu_task(int device, int N, int g, int m, int M, Pool<tsb_nq_node>& pool, GpuTaskResult& r) {
+template <class Node>
+void nq_gpu_task(int device, int N, int g, int m, int M, Pool<Node>& pool, GpuTaskResult& r) {
   tsb_nq* h = nullptr;
-  r.rc = tsb_nq_create(&h, device, N, g, M);
+  r.rc = nq_create_for<Node>(&h, device, N, g, M);
   if (r.rc != TSB_OK) return;
-  std::vector<tsb_nq_node> parents(M);
+  std::vector<Node> parents(M);
   std::vector<uint8_t> labels(static_cast<size_t>(M) * N);
   // the chunk arrays live for the whole step 2 (nqueens_gpu_chpl.chpl:191-192): page-lock them once
-  tsb_nq_register_host(h, parents.data(), parents.size() * sizeof(tsb_nq_node));
+  tsb_nq_register_host(h, parents.data(), parents.size() * sizeof(Node));
   tsb_nq_register_host(h, labels.data(), labels.size());
   for (;;) {
     const int n = pool.popBackBulk(m, M, parents.data());
@@ -394,8 +407,8 @@ void nq_devpool_multi_rounds(std::vector<tsb_nq*>& hs, int m, int M, StealBoard*
   if (r.rc != TSB_OK) board_abort(sb, me);
 }
 // pool -> device, all rounds, leftovers (fewer than m nodes) back to the host pool for step 3
-void nq_devpool_on(tsb_nq* h, int m, int M, Pool<tsb_nq_node>& pool, GpuTaskResult& r, StealBoard* sb = nullptr,
-                   int me = 0) {
+template <class Node>
+void nq_devpool_on(tsb_nq* h, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb = nullptr, int me = 0) {
   const uint64_t l0 = tsb_nq_kernel_launches(h);
   if (const int P = nq_pools_of(h, M); P > 1) {
     std::vector<tsb_nq*> hs{h};
@@ -404,7 +417,7 @@ void nq_devpool_on(tsb_nq* h, int m, int M, Pool<tsb_nq_node>& pool, GpuTaskResu
       r.rc = tsb_nq_sibling(h, i, &sib);
       hs.push_back(sib);
     }
-    std::vector<Pool<tsb_nq_node>> part;
+    std::vector<Pool<Node>> part;
     if (r.rc == TSB_OK) static_split(pool, P, part);
     long long most = 0;
     for (int i = 0; i < P && r.rc == TSB_OK; i++) {
@@ -432,18 +445,21 @@ void nq_devpool_on(tsb_nq* h, int m, int M, Pool<tsb_nq_node>& pool, GpuTaskResu
 // pools, arenas and fat arenas is ~1.4 GB of cudaMalloc / cudaFree per GPU, which at 8 GPUs cost more than the N = 17
 // search itself.  (The Chapel drivers declare their device arrays once, outside the search loop, as well.)
 // At most two idle handles are kept per device; tsb_release_cached_handles frees them all.
+// (rec: the node width of the handle, 21 or 25 bytes)
 struct NqHandleCache {
   struct Entry {
     int device, N, g, M;
+    size_t rec;
     tsb_nq* h;
   };
   std::mutex mu;
   std::vector<Entry> idle;
+  template <class Node>
   tsb_nq* acquire(int device, int N, int g, int M, int* rc) {
     {
       std::lock_guard<std::mutex> lk(mu);
       for (size_t i = 0; i < idle.size(); i++)
-        if (idle[i].device == device && idle[i].N == N && idle[i].g == g && idle[i].M == M) {
+        if (idle[i].device == device && idle[i].N == N && idle[i].g == g && idle[i].M == M && idle[i].rec == sizeof(Node)) {
           tsb_nq* h = idle[i].h;
           idle.erase(idle.begin() + static_cast<long>(i));
           *rc = TSB_OK;
@@ -451,10 +467,10 @@ struct NqHandleCache {
         }
     }
     tsb_nq* h = nullptr;
-    *rc = tsb_nq_create(&h, device, N, g, M);
+    *rc = nq_create_for<Node>(&h, device, N, g, M);
     return *rc == TSB_OK ? h : nullptr;
   }
-  void release(tsb_nq* h, int device, int N, int g, int M, bool healthy) {
+  void release(tsb_nq* h, int device, int N, int g, int M, size_t rec, bool healthy) {
     if (!h) return;
     if (!healthy || std::getenv("TSB200_NO_HANDLE_CACHE")) {
       tsb_nq_destroy(h);
@@ -464,7 +480,7 @@ struct NqHandleCache {
     tsb_nq* evict = nullptr;
     {
       std::lock_guard<std::mutex> lk(mu);
-      idle.push_back({device, N, g, M, h});
+      idle.push_back({device, N, g, M, rec, h});
       int on_device = 0;
       for (const Entry& e : idle) on_device += e.device == device;
       if (on_device > 2)
@@ -488,12 +504,13 @@ NqHandleCache& nq_handle_cache() {
   return *c;
 }
 
-void nq_devpool_task(int device, int N, int g, int m, int M, Pool<tsb_nq_node>& pool, GpuTaskResult& r,
+template <class Node>
+void nq_devpool_task(int device, int N, int g, int m, int M, Pool<Node>& pool, GpuTaskResult& r,
                      StealBoard* sb = nullptr, int me = 0) {
   tsb_nq* h = nullptr;
   const bool trace = std::getenv("TSB200_TRACE") != nullptr;
   const double tt0 = now_s();
-  h = nq_handle_cache().acquire(device, N, g, M, &r.rc);
+  h = nq_handle_cache().acquire<Node>(device, N, g, M, &r.rc);
   if (r.rc != TSB_OK) {
     if (sb) sb->publish_handle(me, nullptr, 0);
     return;
@@ -501,7 +518,7 @@ void nq_devpool_task(int device, int N, int g, int m, int M, Pool<tsb_nq_node>& 
   const double tt1 = now_s();
   nq_devpool_on(h, m, M, pool, r, sb, me);
   const double tt2 = now_s();
-  nq_handle_cache().release(h, device, N, g, M, r.rc == TSB_OK);
+  nq_handle_cache().release(h, device, N, g, M, sizeof(Node), r.rc == TSB_OK);
   if (trace) std::fprintf(stderr, "[tsb200] device %d: create %.1f ms, %llu rounds in %.1f ms, destroy %.1f ms\n", device,
                           (tt1 - tt0) * 1e3, static_cast<unsigned long long>(r.offloads), (tt2 - tt1) * 1e3,
                           (now_s() - tt2) * 1e3);
@@ -923,16 +940,20 @@ int tsb_pfsp_create_from_tables(tsb_pfsp** h, int device, int M_max, const tsb_p
                          t->pairs, t->johnson, t->lags, t->mp0, t->mp1, t->mp_order);
 }
 
-int tsb_nq_search(int N, int g, int m, int M, int D, tsb_search_stats* out) {
-  if (!out || N < 1 || N > TSB_MAX_QUEENS || g < 1 || m < 1 || M < 1 || D < 1 || D > 8) return TSB_EINVAL;
+}  // extern "C"
+namespace {
+template <class Node>
+int nq_search_host(int N, int g, int m, int M, int D, tsb_search_stats* out) {
+  const int max_n = std::is_same_v<Node, tsb_nq_node24> ? TSB_MAX_QUEENS_WIDE : TSB_MAX_QUEENS;
+  if (!out || N < 1 || N > max_n || g < 1 || m < 1 || M < 1 || D < 1 || D > 8) return TSB_EINVAL;
   std::memset(out, 0, sizeof(*out));
   if (int rc = tsb_init_devices(D); rc != TSB_OK) return rc;  // contexts exist before the timers start
-  Pool<tsb_nq_node> pool;
-  tsb_nq_node root{};
+  Pool<Node> pool;
+  Node root{};
   for (int i = 0; i < N; i++) root.board[i] = static_cast<uint8_t>(i);
   pool.pushBack(root);
   uint64_t tree = 0, sol = 0;
-  tsb_nq_node parent;
+  Node parent;
   double t0 = now_s();
   while (pool.size < static_cast<size_t>(D) * m) {  // step 1 (nqueens_multigpu_chpl.chpl:173-179)
     if (!pool.popFront(parent)) break;
@@ -947,7 +968,7 @@ int tsb_nq_search(int N, int g, int m, int M, int D, tsb_search_stats* out) {
   if (D == 1) {
     nq_gpu_task(0, N, g, m, M, pool, res[0]);
   } else {
-    std::vector<Pool<tsb_nq_node>> multi;
+    std::vector<Pool<Node>> multi;
     static_split(pool, D, multi);
     std::vector<std::thread> th;
     for (int gid = 0; gid < D; gid++)
@@ -981,21 +1002,25 @@ int tsb_nq_search(int N, int g, int m, int M, int D, tsb_search_stats* out) {
 // process-per-GPU launch): the step-1 tree is credited to part 0 and every part drains its own leftovers, so the
 // per-part counts add up to the whole search's.  `on` != nullptr: D = 1 on a handle the caller created (set-up
 // outside the search's timers, as the Chapel drivers' `on device var` declarations are).
-static int nq_search_device_impl(int N, int g, int m, int M, int D, int part, int device, tsb_nq* on,
-                                 tsb_search_stats* out) {
-  if (!out || N < 1 || N > TSB_MAX_QUEENS || g < 1 || m < 1 || M < 1 || D < 1 || D > 8 || part >= D) return TSB_EINVAL;
+template <class Node>
+int nq_search_device_impl(int N, int g, int m, int M, int D, int part, int device, tsb_nq* on, tsb_search_stats* out) {
+  constexpr bool wide = std::is_same_v<Node, tsb_nq_node24>;
+  if (!out || N < 1 || N > (wide ? TSB_MAX_QUEENS_WIDE : TSB_MAX_QUEENS) || g < 1 || m < 1 || M < 1 || D < 1 || D > 8 ||
+      part >= D)
+    return TSB_EINVAL;
   std::memset(out, 0, sizeof(*out));
   if (!on)
     if (int rc = tsb_init_devices(part < 0 ? D : device + 1); rc != TSB_OK) return rc;
-  Pool<tsb_nq_node> pool;
-  tsb_nq_node root{};
+  Pool<Node> pool;
+  Node root{};
   for (int i = 0; i < N; i++) root.board[i] = static_cast<uint8_t>(i);
   pool.pushBack(root);
   uint64_t tree = 0, sol = 0;
-  tsb_nq_node parent;
+  Node parent;
   double t0 = now_s();
-  // step 1 on the CPU, as in the reference: m nodes for every pool (two per task in pair mode, see nq_pair_mode)
-  while (pool.size < static_cast<size_t>(D) * m * nq_pools_wanted(M)) {
+  // step 1 on the CPU, as in the reference: m nodes for every pool (one pool per task on wide handles, which do not
+  // share launches of the persistent kernel)
+  while (pool.size < static_cast<size_t>(D) * m * (wide ? 1 : nq_pools_wanted(M))) {
     if (!pool.popFront(parent)) break;
     nq_decompose(N, parent, tree, sol, pool);
   }
@@ -1009,7 +1034,7 @@ static int nq_search_device_impl(int N, int g, int m, int M, int D, int part, in
     nq_devpool_on(on, m, M, pool, res[0]);
   } else if (part >= 0) {
     if (part != 0) tree = sol = 0;  // step 1 is credited to part 0
-    std::vector<Pool<tsb_nq_node>> multi;
+    std::vector<Pool<Node>> multi;
     if (D == 1) {
       multi.resize(1);
       std::swap(multi[0], pool);
@@ -1021,7 +1046,7 @@ static int nq_search_device_impl(int N, int g, int m, int M, int D, int part, in
   } else if (D == 1) {
     nq_devpool_task(0, N, g, m, M, pool, res[0]);
   } else {
-    std::vector<Pool<tsb_nq_node>> multi;
+    std::vector<Pool<Node>> multi;
     static_split(pool, D, multi);
     StealBoard board(D);
     StealBoard* sb = std::getenv("TSB200_NO_STEAL") ? nullptr : &board;
@@ -1052,6 +1077,17 @@ static int nq_search_device_impl(int N, int g, int m, int M, int D, int part, in
   out->explored_tree = tree;
   out->explored_sol = sol;
   return TSB_OK;
+}
+}  // namespace
+extern "C" {
+
+int tsb_nq_search(int N, int g, int m, int M, int D, tsb_search_stats* out) {
+  return N > TSB_MAX_QUEENS ? nq_search_host<tsb_nq_node24>(N, g, m, M, D, out)
+                            : nq_search_host<tsb_nq_node>(N, g, m, M, D, out);
+}
+int tsb_nq_search_wide(int max_queens, int N, int g, int m, int M, int D, tsb_search_stats* out) {
+  if (max_queens != TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
+  return nq_search_host<tsb_nq_node24>(N, g, m, M, D, out);
 }
 
 // pools > 1 (device pools only): every task's share split once more into `pools` device pools (pfsp_devpool_on)
@@ -1152,10 +1188,13 @@ static int pfsp_search_impl(int inst, int lb_kind, int ub, int m, int M, int D, 
 // min_size nodes; the pool, in order, and what was explored on the way
 void tsb_release_cached_handles(void) { nq_handle_cache().clear(); }
 
-int tsb_nq_warmup(int N, int min_size, void* nodes, int64_t capacity, int64_t* n, uint64_t* tree, uint64_t* sol) {
-  if (N < 1 || N > TSB_MAX_QUEENS || min_size < 1 || !n || !tree || !sol || (capacity && !nodes)) return TSB_EINVAL;
-  Pool<tsb_nq_node> pool;
-  tsb_nq_node root{}, parent;
+}  // extern "C"
+namespace {
+template <class Node>
+int nq_warmup(int N, int min_size, void* nodes, int64_t capacity, int64_t* n, uint64_t* tree, uint64_t* sol) {
+  if (min_size < 1 || !n || !tree || !sol || (capacity && !nodes)) return TSB_EINVAL;
+  Pool<Node> pool;
+  Node root{}, parent;
   for (int i = 0; i < N; i++) root.board[i] = static_cast<uint8_t>(i);
   pool.pushBack(root);
   *tree = *sol = 0;
@@ -1165,20 +1204,44 @@ int tsb_nq_warmup(int N, int min_size, void* nodes, int64_t capacity, int64_t* n
   }
   *n = static_cast<int64_t>(pool.size);
   if (*n > capacity) return TSB_ENOMEM;
-  if (pool.size) std::memcpy(nodes, &pool.el[pool.front], pool.size * sizeof(tsb_nq_node));
+  if (pool.size) std::memcpy(nodes, &pool.el[pool.front], pool.size * sizeof(Node));
   return TSB_OK;
+}
+// the search's node type for N (whole searches: the wide records only where the narrow ones cannot hold the board)
+template <class F>
+int with_nq_node(bool wide, F&& f) {
+  return wide ? f(tsb_nq_node24{}) : f(tsb_nq_node{});
+}
+}  // namespace
+extern "C" {
+
+int tsb_nq_warmup(int N, int min_size, void* nodes, int64_t capacity, int64_t* n, uint64_t* tree, uint64_t* sol) {
+  if (N < 1 || N > TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
+  return with_nq_node(N > TSB_MAX_QUEENS, [&](auto node) {
+    return nq_warmup<decltype(node)>(N, min_size, nodes, capacity, n, tree, sol);
+  });
 }
 
 int tsb_nq_search_device(int N, int g, int m, int M, int D, tsb_search_stats* out) {
-  return nq_search_device_impl(N, g, m, M, D, -1, 0, nullptr, out);
+  return with_nq_node(N > TSB_MAX_QUEENS, [&](auto node) {
+    return nq_search_device_impl<decltype(node)>(N, g, m, M, D, -1, 0, nullptr, out);
+  });
+}
+int tsb_nq_search_device_wide(int max_queens, int N, int g, int m, int M, int D, tsb_search_stats* out) {
+  if (max_queens != TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
+  return nq_search_device_impl<tsb_nq_node24>(N, g, m, M, D, -1, 0, nullptr, out);
 }
 int tsb_nq_search_device_part(int N, int g, int m, int M, int D, int part, int device, tsb_search_stats* out) {
   if (part < 0) return TSB_EINVAL;
-  return nq_search_device_impl(N, g, m, M, D, part, device, nullptr, out);
+  return with_nq_node(N > TSB_MAX_QUEENS, [&](auto node) {
+    return nq_search_device_impl<decltype(node)>(N, g, m, M, D, part, device, nullptr, out);
+  });
 }
 int tsb_nq_search_on(tsb_nq* h, int N, int m, int M, tsb_search_stats* out) {
   if (!h) return TSB_EINVAL;
-  return nq_search_device_impl(N, 1, m, M, 1, -1, 0, h, out);
+  return with_nq_node(tsb_nq_max_queens(h) == TSB_MAX_QUEENS_WIDE, [&](auto node) {
+    return nq_search_device_impl<decltype(node)>(N, 1, m, M, 1, -1, 0, h, out);
+  });
 }
 int tsb_pfsp_search(int inst, int lb_kind, int ub, int m, int M, int D, tsb_search_stats* out) {
   return pfsp_search_impl(inst, lb_kind, ub, m, M, D, false, -1, 0, nullptr, out);

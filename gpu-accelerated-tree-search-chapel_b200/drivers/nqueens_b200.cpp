@@ -31,6 +31,10 @@ int main(int argc, char** argv) {
     std::fprintf(stderr, "All parameters must be positive integers.\n");
     return 2;
   }
+  if (N > TSB_MAX_QUEENS_WIDE) {  // (N = 21..24 run as a `-sMAX_QUEENS=24` build would: 25-byte nodes)
+    std::fprintf(stderr, "--N %d: boards of at most %d queens are supported.\n", N, TSB_MAX_QUEENS_WIDE);
+    return 2;
+  }
   std::printf("\n=================================================\n%s H100 (tsb200)\n\n"
               "Resolution of the %d-Queens instance\n  with %d safety check(s) per evaluation\n"
               "=================================================\n", D > 1 ? "Multi-GPU" : "Single-GPU", N, g);

@@ -9,6 +9,7 @@ PKG_DIR = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB_PATH = os.environ.get("TSB200_LIB") or os.path.join(PKG_DIR, "libtsb200.so")  # (TSB200_LIB: A/B builds)
 
 MAX_JOBS = 20
+MAX_QUEENS, MAX_QUEENS_WIDE = 20, 24
 MAX_MACHINES = 20
 MAX_PAIRS = 190
 
@@ -75,6 +76,8 @@ SYMBOLS = {
     "tsb_bind_thread_to_device": (_i, [_i]),
     "tsb_version": (C.c_char_p, []),
     "tsb_nq_create": (_i, [C.POINTER(_vp), _i, _i, _i, _i]),
+    "tsb_nq_create_wide": (_i, [C.POINTER(_vp), _i, _i, _i, _i, _i]),
+    "tsb_nq_max_queens": (_i, [_vp]),
     "tsb_nq_destroy": (None, [_vp]),
     "tsb_nq_evaluate": (_i, [_vp, _vp, _i, _vp]),
     "tsb_nq_evaluate_device": (_i, [_vp, _vp, _i, _vp, _vp]),
@@ -133,6 +136,8 @@ SYMBOLS = {
     "tsb_pfsp_stream": (_vp, [_vp]),
     "tsb_nq_search": (_i, [_i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
     "tsb_nq_search_device": (_i, [_i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
+    "tsb_nq_search_wide": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
+    "tsb_nq_search_device_wide": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
     "tsb_pfsp_search": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
     "tsb_pfsp_search_device": (_i, [_i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
     "tsb_nq_search_on": (_i, [_vp, _i, _i, _i, C.POINTER(SearchStats)]),

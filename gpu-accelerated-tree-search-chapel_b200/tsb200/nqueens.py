@@ -5,20 +5,39 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import SearchStats, check, lib
+from ._lib import MAX_QUEENS, MAX_QUEENS_WIDE, SearchStats, check, lib
 
 # lib/nqueens/NQueens_node.chpl:9-11
-NQ_NODE_DTYPE = np.dtype([("depth", np.uint8), ("board", np.uint8, (20,))])
+NQ_NODE_DTYPE = np.dtype([("depth", np.uint8), ("board", np.uint8, (MAX_QUEENS,))])
 assert NQ_NODE_DTYPE.itemsize == 21
+# the same record of a build of the reference with MAX_QUEENS = 24 (boards of 21 to 24 queens)
+NQ_NODE24_DTYPE = np.dtype([("depth", np.uint8), ("board", np.uint8, (MAX_QUEENS_WIDE,))])
+assert NQ_NODE24_DTYPE.itemsize == 25
+
+
+def nq_node_dtype(N: int) -> np.dtype:
+    """the node record of the searches for N queens: 21 bytes up to N = 20, else 25 bytes"""
+    return NQ_NODE_DTYPE if N <= MAX_QUEENS else NQ_NODE24_DTYPE
 
 
 class NQueensEvaluator:
-    """Owns what `on device var parents_d, labels_d` owns in the reference (nqueens_gpu_chpl.chpl:194-195)."""
+    """Owns what `on device var parents_d, labels_d` owns in the reference (nqueens_gpu_chpl.chpl:194-195).
+    N > 20, or max_queens=24 for any N, creates a MAX_QUEENS = 24 handle (tsb_nq_create_wide): its nodes are
+    NQ_NODE24_DTYPE records (`node_dtype`), and its device pools run two-kernel rounds."""
 
-    def __init__(self, N: int, g: int = 1, M: int = 50000, device: int = 0):
+    wide, node_dtype = False, NQ_NODE_DTYPE  # (an object that wraps a tsb_nq_create handle)
+
+    def __init__(self, N: int, g: int = 1, M: int = 50000, device: int = 0, max_queens: int | None = None):
         self.N, self.g, self.M, self.device = N, g, M, device
         self._h = C.c_void_p()
-        check(lib().tsb_nq_create(C.byref(self._h), device, N, g, M), "tsb_nq_create")
+        if max_queens is None:
+            max_queens = MAX_QUEENS if N <= MAX_QUEENS else MAX_QUEENS_WIDE
+        self.wide = max_queens != MAX_QUEENS
+        self.node_dtype = NQ_NODE24_DTYPE if self.wide else NQ_NODE_DTYPE
+        if self.wide:
+            check(lib().tsb_nq_create_wide(C.byref(self._h), device, max_queens, N, g, M), "tsb_nq_create_wide")
+        else:
+            check(lib().tsb_nq_create(C.byref(self._h), device, N, g, M), "tsb_nq_create")
 
     def close(self):
         if self._h:
@@ -63,7 +82,7 @@ class NQueensEvaluator:
     def evaluate_gpu(self, parents: np.ndarray, size: int, labels: np.ndarray) -> None:
         """evaluate_gpu(parents_d, size, labels_d) of nqueens_gpu_chpl.chpl:97-123 including the copies of
         :203/:205; `size` = N * poolSize as in the reference call (:201-204)."""
-        assert parents.dtype == NQ_NODE_DTYPE and parents.flags.c_contiguous
+        assert parents.dtype == self.node_dtype and parents.flags.c_contiguous
         assert labels.dtype == np.uint8 and labels.flags.c_contiguous
         if size % self.N:
             raise ValueError("size must be N * poolSize")
@@ -80,9 +99,9 @@ class NQueensEvaluator:
     def expand(self, parents: np.ndarray):
         """children of the chunk (packed, reference order) and the number of depth == N parents:
         evaluate_gpu (nqueens_gpu_chpl.chpl:97-123) + generate_children (:126-149) in one device pass"""
-        assert parents.dtype == NQ_NODE_DTYPE and parents.flags.c_contiguous
+        assert parents.dtype == self.node_dtype and parents.flags.c_contiguous
         cap = parents.shape[0] * self.N
-        out = np.empty(max(cap, 1), dtype=NQ_NODE_DTYPE)
+        out = np.empty(max(cap, 1), dtype=self.node_dtype)
         nc, ns = C.c_uint64(0), C.c_uint64(0)
         check(lib().tsb_nq_expand(self._h, parents.ctypes.data, parents.shape[0], out.ctypes.data, cap,
                                   C.byref(nc), C.byref(ns)), "tsb_nq_expand")
@@ -95,7 +114,7 @@ class NQueensEvaluator:
         return int(nc.value), int(ns.value)
 
     def pool_push(self, nodes: np.ndarray) -> None:
-        assert nodes.dtype == NQ_NODE_DTYPE and nodes.flags.c_contiguous
+        assert nodes.dtype == self.node_dtype and nodes.flags.c_contiguous
         check(lib().tsb_nq_pool_push(self._h, nodes.ctypes.data, nodes.shape[0]), "tsb_nq_pool_push")
 
     @property
@@ -133,7 +152,7 @@ class NQueensEvaluator:
 
     def pool_drain(self) -> np.ndarray:
         n = self.pool_size
-        out = np.empty(max(n, 1), dtype=NQ_NODE_DTYPE)
+        out = np.empty(max(n, 1), dtype=self.node_dtype)
         got = C.c_int64(0)
         check(lib().tsb_nq_pool_drain(self._h, out.ctypes.data, n, C.byref(got)), "tsb_nq_pool_drain")
         return out[: got.value].copy()
@@ -154,26 +173,36 @@ def nqueens_pool_run_multi(evaluators, m: int, M: int, max_rounds: int = 2**62):
 
 
 def nqueens_warmup(N: int, min_size: int = 25):
-    """step 1 of the drivers (nqueens_gpu_chpl.chpl:169-175): (pool nodes, explored tree, solutions)"""
+    """step 1 of the drivers (nqueens_gpu_chpl.chpl:169-175): (pool nodes, explored tree, solutions); the nodes are
+    nq_node_dtype(N) records"""
     cap = max(1024, 32 * min_size)
-    out = np.zeros(cap, dtype=NQ_NODE_DTYPE)
+    out = np.zeros(cap, dtype=nq_node_dtype(N))
     n, tree, sol = C.c_int64(0), C.c_uint64(0), C.c_uint64(0)
     check(lib().tsb_nq_warmup(N, min_size, out.ctypes.data, cap, C.byref(n), C.byref(tree), C.byref(sol)), "tsb_nq_warmup")
     return out[: n.value].copy(), int(tree.value), int(sol.value)
 
 
-def nqueens_search(N: int = 14, g: int = 1, m: int = 25, M: int = 50000, D: int = 1) -> SearchStats:
+def nqueens_search(N: int = 14, g: int = 1, m: int = 25, M: int = 50000, D: int = 1,
+                   max_queens: int | None = None) -> SearchStats:
     """the 3-step search of nqueens_gpu_chpl.chpl:152-248 (D = 1) / nqueens_multigpu_chpl.chpl:158-352
-    (static split, D GPUs), run by the C++ emulation driver inside libtsb200.so"""
+    (static split, D GPUs), run by the C++ emulation driver inside libtsb200.so.  N in 1..24 (N > 20 with 25-byte
+    nodes); max_queens=24: every N as a MAX_QUEENS = 24 build runs it (tsb_nq_search_wide)"""
     st = SearchStats()
-    check(lib().tsb_nq_search(N, g, m, M, D, C.byref(st)), "tsb_nq_search")
+    if max_queens is None:
+        check(lib().tsb_nq_search(N, g, m, M, D, C.byref(st)), "tsb_nq_search")
+    else:
+        check(lib().tsb_nq_search_wide(max_queens, N, g, m, M, D, C.byref(st)), "tsb_nq_search_wide")
     return st
 
 
-def nqueens_search_device(N: int = 14, g: int = 1, m: int = 25, M: int = 50000, D: int = 1) -> SearchStats:
+def nqueens_search_device(N: int = 14, g: int = 1, m: int = 25, M: int = 50000, D: int = 1,
+                          max_queens: int | None = None) -> SearchStats:
     """same 3-step search, the pool(s) of step 2 resident on the device(s) (tsb_nq_pool_*)"""
     st = SearchStats()
-    check(lib().tsb_nq_search_device(N, g, m, M, D, C.byref(st)), "tsb_nq_search_device")
+    if max_queens is None:
+        check(lib().tsb_nq_search_device(N, g, m, M, D, C.byref(st)), "tsb_nq_search_device")
+    else:
+        check(lib().tsb_nq_search_device_wide(max_queens, N, g, m, M, D, C.byref(st)), "tsb_nq_search_device_wide")
     return st
 
 

@@ -19,6 +19,7 @@
  *
  * Node wire formats (must match the Chapel records bit for bit):
  *   N-Queens  lib/nqueens/NQueens_node.chpl:9-11   { uint8 depth; uint8 board[20]; }   21 B, align 1
+ *             a `chpl -sMAX_QUEENS=24` build            { uint8 depth; uint8 board[24]; }   25 B (tsb_nq_create_wide)
  *   PFSP      lib/pfsp/PFSP_node.chpl:9-12         { int32 depth; int32 limit1; int32 prmu[20]; } 88 B
  *
  * Output contract (same as the reference kernels): only slots k >= depth (N-Queens) /
@@ -38,6 +39,7 @@ extern "C" {
 #endif
 
 #define TSB_MAX_QUEENS 20
+#define TSB_MAX_QUEENS_WIDE 24 /* the reference built with `-sMAX_QUEENS=24` (lib/nqueens/NQueens_node.chpl:7): N <= 24 */
 #define TSB_MAX_JOBS 20
 #define TSB_MAX_MACHINES 20
 #define TSB_MAX_PAIRS 190
@@ -47,6 +49,11 @@ typedef struct {
   uint8_t depth;
   uint8_t board[TSB_MAX_QUEENS];
 } tsb_nq_node; /* 21 bytes */
+
+typedef struct {
+  uint8_t depth;
+  uint8_t board[TSB_MAX_QUEENS_WIDE];
+} tsb_nq_node24; /* 25 bytes: N-Queens Node of a MAX_QUEENS = 24 build */
 
 typedef struct {
   int32_t depth;
@@ -62,7 +69,7 @@ typedef struct {
 
 enum {
   TSB_OK = 0,
-  TSB_EINVAL = -1,   /* bad argument (NULL handle, N out of 1..20, count > M_max, unknown lb_kind ...) */
+  TSB_EINVAL = -1,   /* bad argument (NULL handle, N out of 1..20 (1..24 wide), count > M_max, unknown lb_kind ...) */
   TSB_ECUDA = -2,    /* a CUDA runtime call failed; tsb_last_cuda_error() has the text */
   TSB_ENOMEM = -3,   /* host or device allocation failed */
   TSB_ENODEV = -4,   /* no such CUDA device / no CUDA driver */
@@ -114,11 +121,22 @@ typedef struct tsb_nq tsb_nq;
  * on g: the reference's inner `for _g` loop ANDs the same boolean g times, :115-118),
  * M_max = the driver's --M (largest chunk). */
 int tsb_nq_create(tsb_nq** h, int device, int N, int g, int M_max);
+/* The reference built with MAX_QUEENS = max_queens; only 24 is accepted (TSB_EINVAL otherwise).  N in 1..24 (a
+ * `-sMAX_QUEENS=24` program may still run --N 14).  Every N-Queens entry point below works on such a handle with
+ * 25-byte tsb_nq_node24 records (parents, children and pool nodes) and N label bytes per parent; the push check
+ * reads board[N..24) == 0.  Differences from a tsb_nq_create handle:
+ *   - the persistent kernel is not used (its 32-byte nodes do not hold a 24-queen board): tsb_nq_pool_run is the
+ *     tsb_nq_pool_step loop, tsb_nq_pools_per_launch returns 1, tsb_nq_pool_run_multi runs the pools one after the
+ *     other;
+ *   - tsb_nq_pool_steal and tsb_nq_pool_run_multi take wide handles only together (TSB_EINVAL for a mix). */
+int tsb_nq_create_wide(tsb_nq** h, int device, int max_queens, int N, int g, int M_max);
+/* the MAX_QUEENS of the build a handle serves: 20 (tsb_nq_create) or 24 (tsb_nq_create_wide); TSB_EINVAL for NULL */
+int tsb_nq_max_queens(const tsb_nq* h);
 void tsb_nq_destroy(tsb_nq* h);
 
 /* Replaces the three statements of one offload round, nqueens_gpu_chpl.chpl:203-205
  *   parents_d = parents;  on device do evaluate_gpu(parents_d, N*count, labels_d);  labels = labels_d;
- * parents: count x 21 B host records; labels: count x N host bytes, labels[p*N + k] = 1 iff the
+ * parents: count x 21 B host records (25 B on a tsb_nq_create_wide handle); labels: count x N host bytes, labels[p*N + k] = 1 iff the
  * queen board[k] can be placed on row `depth` (evaluate_gpu, nqueens_gpu_chpl.chpl:97-123).
  * Synchronous; count == 0 is a no-op; only the live prefix moves (unlike Chapel's whole-array copy). */
 int tsb_nq_evaluate(tsb_nq* h, const void* parents, int count, uint8_t* labels);
@@ -147,7 +165,7 @@ int tsb_nq_expand_device(tsb_nq* h, const void* parents_d /*16-B aligned*/, int 
  * nodes, order preserved, read in place), evaluate, generate_children appended to the pool; drain = move what
  * is left to the host (logical order).  The pool's logical content after every round is byte-identical to
  * the reference's host pool.
- * push admits only nodes the search can create: depth <= N, board[0..N) < N and board[N..20) == 0.  Any other
+ * push admits only nodes the search can create: depth <= N, board[0..N) < N and board[N..20) == 0 (board[N..24) wide).  Any other
  * node makes it return TSB_EINVAL with the pool unchanged (the pool is packed to 125 bits per node on these terms). */
 int tsb_nq_pool_push(tsb_nq* h, const void* nodes, int64_t n);
 int64_t tsb_nq_pool_size(const tsb_nq* h);
@@ -369,10 +387,16 @@ typedef struct {
 } tsb_search_stats;
 
 /* step 1 of the drivers alone (nqueens_gpu_chpl.chpl:169-175): breadth-first from the root until the pool holds
- * min_size nodes; returns that pool (in order) and the nodes / solutions counted on the way */
+ * min_size nodes; returns that pool (in order) and the nodes / solutions counted on the way.  N in 1..24: the nodes
+ * are tsb_nq_node records for N <= 20, tsb_nq_node24 records for N = 21..24 */
 int tsb_nq_warmup(int N, int min_size, void* nodes, int64_t capacity_nodes, int64_t* n, uint64_t* tree, uint64_t* sol);
 /* nqueens_gpu_chpl.chpl:152-248 / nqueens_multigpu_chpl.chpl:158-352 */
+/* N in 1..24: N <= 20 runs on tsb_nq_create handles exactly as before, N = 21..24 on tsb_nq_create_wide handles (the
+ * same searches, with 25-byte nodes; the device pools of tsb_nq_search_device[_part] then run two-kernel rounds) */
 int tsb_nq_search(int N, int g, int m, int M, int D, tsb_search_stats* out);
+/* the same search as a MAX_QUEENS = max_queens build runs it (only 24: TSB_EINVAL otherwise): 25-byte nodes and
+ * tsb_nq_create_wide handles for every N in 1..24 (tsb_nq_search_device_wide: the device-pool search) */
+int tsb_nq_search_wide(int max_queens, int N, int g, int m, int M, int D, tsb_search_stats* out);
 /* tsb_nq_search_device[_part] keep their handles (device pools, arenas) per (device, N, g, M) between calls; this
  * frees them.  TSB200_NO_HANDLE_CACHE=1: create and destroy per search. */
 void tsb_release_cached_handles(void);
@@ -385,8 +409,10 @@ void tsb_release_cached_handles(void);
  * pool peer-to-peer (the reference's intra-node work stealing, nqueens_multigpu_chpl.chpl:255-312, moved to the
  * device pools; env TSB200_NO_STEAL=1 = the static split alone). */
 int tsb_nq_search_device(int N, int g, int m, int M, int D, tsb_search_stats* out);
-/* the D = 1 search on a handle the caller created (N and M_max >= M must match): set-up stays outside the
- * search's timers, as the `on device var` declarations of the Chapel drivers do */
+int tsb_nq_search_device_wide(int max_queens, int N, int g, int m, int M, int D, tsb_search_stats* out);
+/* the D = 1 search on a handle the caller created (N and M_max >= M must match; a tsb_nq_create_wide handle runs
+ * it with 25-byte nodes): set-up stays outside the search's timers, as the `on device var` declarations of the
+ * Chapel drivers do */
 int tsb_nq_search_on(tsb_nq* h, int N, int m, int M, tsb_search_stats* out);
 /* one task of that D-way split, on `device` — for process-per-GPU launches (one rank = one part): step 1 is
  * credited to part 0 and each part drains its own leftovers, so the parts' counts add up to the whole search */
