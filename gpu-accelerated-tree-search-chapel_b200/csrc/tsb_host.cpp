@@ -17,6 +17,7 @@
 #include <cstring>
 #include <atomic>
 #include <condition_variable>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <type_traits>
@@ -154,32 +155,8 @@ struct GpuTaskResult {
   int rc = 0;
 };
 
-// one GPU task's offload loop (nqueens_gpu_chpl.chpl:197-215; nqueens_multigpu_chpl.chpl:234-253)
-inline void bind_task(int device, bool multi) {  // one host thread per GPU: next to its GPU (env TSB200_NO_NUMA=1: no)
-  if (multi && !std::getenv("TSB200_NO_NUMA")) (void)tsb_bind_thread_to_device(device);
-}
-
-template <class Node>
-void nq_gpu_task(int device, int N, int g, int m, int M, Pool<Node>& pool, GpuTaskResult& r) {
-  tsb_nq* h = nullptr;
-  r.rc = nq_create_for<Node>(&h, device, N, g, M);
-  if (r.rc != TSB_OK) return;
-  std::vector<Node> parents(M);
-  std::vector<uint8_t> labels(static_cast<size_t>(M) * N);
-  // the chunk arrays live for the whole step 2 (nqueens_gpu_chpl.chpl:191-192): page-lock them once
-  tsb_nq_register_host(h, parents.data(), parents.size() * sizeof(Node));
-  tsb_nq_register_host(h, labels.data(), labels.size());
-  for (;;) {
-    const int n = pool.popBackBulk(m, M, parents.data());
-    if (n <= 0) break;
-    r.rc = tsb_nq_evaluate(h, parents.data(), n, labels.data());
-    if (r.rc != TSB_OK) break;
-    ++r.offloads;
-    r.parents += static_cast<uint64_t>(n);
-    nq_generate_children(N, parents.data(), n, labels.data(), r.tree, r.sol, pool);
-  }
-  r.launches = tsb_nq_kernel_launches(h);
-  tsb_nq_destroy(h);
+inline void bind_task(int device) {  // one host thread per GPU: next to its GPU (env TSB200_NO_NUMA=1: no)
+  if (!std::getenv("TSB200_NO_NUMA")) (void)tsb_bind_thread_to_device(device);
 }
 
 // ---- intra-node work stealing between the tasks' DEVICE pools (the reference steals between its per-GPU host
@@ -302,99 +279,90 @@ inline void board_abort(StealBoard* sb, int me) {
   sb->cv.notify_all();
 }
 
+// static strided split of the warm-up pool (nqueens_multigpu_chpl.chpl:199-226)
 template <class Node>
-void static_split(Pool<Node>& pool, int D, std::vector<Pool<Node>>& multi);
+void static_split(Pool<Node>& pool, int D, std::vector<Pool<Node>>& multi) {
+  const size_t poolSize = pool.size, c = poolSize / D, l = poolSize - (D - 1) * c, f = pool.front;
+  multi.resize(D);
+  for (int g = 0; g < D; g++) {
+    for (size_t i = 0; i < c; i++) multi[g].pushBack(pool.el[g + f + i * D]);
+    if (g == D - 1)
+      for (size_t i = 0; i < l - c; i++) multi[g].pushBack(pool.el[D * c + f + i]);
+  }
+  pool.front = 0;
+  pool.size = 0;
+}
 
 // rounds per library call when nodes may move between pools (a victim serves requests between calls)
 inline int64_t rounds_per_call(bool moves, int M) { return !moves ? INT64_MAX : small_chunks(M) ? 256 : 4; }
 
-// drain a device pool and push what it held back onto the host pool
+// (env set: nodes never move between the device pools of a search, the static split alone)
+inline bool steal_allowed() { return !std::getenv("TSB200_NO_STEAL"); }
+
+// ---- the device pools of one task, for either handle type: the library's pool calls, overloaded on the handle
+inline int64_t pool_size(const tsb_nq* h) { return tsb_nq_pool_size(h); }
+inline int64_t pool_size(const tsb_pfsp* h) { return tsb_pfsp_pool_size(h); }
+inline int pool_push(tsb_nq* h, const void* nodes, int64_t n) { return tsb_nq_pool_push(h, nodes, n); }
+inline int pool_push(tsb_pfsp* h, const void* nodes, int64_t n) { return tsb_pfsp_pool_push(h, nodes, n); }
+inline int pool_drain(tsb_nq* h, void* nodes, int64_t cap, int64_t* n) { return tsb_nq_pool_drain(h, nodes, cap, n); }
+inline int pool_drain(tsb_pfsp* h, void* nodes, int64_t cap, int64_t* n) { return tsb_pfsp_pool_drain(h, nodes, cap, n); }
+inline int pool_steal(tsb_nq* v, tsb_nq* t, int m, int64_t* got) { return tsb_nq_pool_steal(v, t, m, got); }
+inline int pool_steal(tsb_pfsp* v, tsb_pfsp* t, int m, int64_t* got) { return tsb_pfsp_pool_steal(v, t, m, got); }
+inline int pool_sibling(tsb_nq* h, int i, tsb_nq** sib) { return tsb_nq_sibling(h, i, sib); }
+inline int pool_sibling(tsb_pfsp* h, int i, tsb_pfsp** sib) { return tsb_pfsp_sibling(h, i, sib); }
+inline uint64_t kernel_launches(const tsb_nq* h) { return tsb_nq_kernel_launches(h); }
+inline uint64_t kernel_launches(const tsb_pfsp* h) { return tsb_pfsp_kernel_launches(h); }
+
+// drain a device pool and push what it held onto a host pool
 template <class H, class Node>
-int drain_to_host(H* h, Pool<Node>& pool, int64_t (*size)(const H*), int (*drain)(H*, void*, int64_t, int64_t*)) {
-  const int64_t left = size(h);
+int drain_to_host(H* h, Pool<Node>& pool) {
+  const int64_t left = pool_size(h);
   std::vector<Node> rest(static_cast<size_t>(left) + 1);
   int64_t n = 0;
-  const int rc = drain(h, rest.data(), left, &n);
+  const int rc = pool_drain(h, rest.data(), left, &n);
   for (int64_t i = 0; i < n && rc == TSB_OK; i++) pool.pushBack(rest[i]);
   return rc;
 }
 
-// the offload loop with the task's pool resident on the device (tsb_nq_pool_*): all rounds of step 2 inside the
-// library (one persistent kernel for small M, two kernels per round otherwise); the host only reads counters
-void nq_devpool_rounds(tsb_nq* h, int m, int M, StealBoard* sb, int me, GpuTaskResult& r) {
-  const auto steal = [m](void* v, void* t, int64_t* got) {
-    return tsb_nq_pool_steal(static_cast<tsb_nq*>(v), static_cast<tsb_nq*>(t), m, got);
-  };
-  while (r.rc == TSB_OK) {
-    uint64_t nr = 0, np = 0, nc = 0, ns = 0;
-    r.rc = tsb_nq_pool_run(h, m, M, rounds_per_call(sb, M), &nr, &np, &nc, &ns);
-    if (r.rc != TSB_OK) break;
-    r.tree += nc;
-    r.sol += ns;
-    r.offloads += nr;
-    r.parents += np;
-    const long long size = tsb_nq_pool_size(h);
-    if (size >= m) {
-      r.rc = board_service(sb, me, size, steal_floor(m, M), steal);
-      continue;
-    }
-    if (!board_acquire(sb, me, size, steal_floor(m, M))) break;
-  }
-  if (r.rc != TSB_OK) board_abort(sb, me);
-}
-// Several pools per task (TSB200_POOLS=1 turns it off, =2 caps it at two): for chunks that fit the persistent kernel a
-// round is a chain of L2 round trips with little work in between, so the task's share of the warm-up pool is split
-// once more — the reference's own strided split (static_split) — into P device pools (P = tsb_nq_pools_per_launch: 4
-// on an H100 for M <= 50688) whose rounds run in ONE launch (tsb_nq_pool_run_multi), two CTAs of different pools on
-// every SM filling each other's waits.  Each pool follows the reference's rule on its own nodes: for D tasks the
-// chunk sequence is that of a 2-level split into P D pools, the totals are split-invariant.  A pool of the group
-// that runs dry takes the oldest half of the fullest one (as between tasks).
-inline int nq_pools_wanted(int M) {  // (decides the warm-up size, before any handle exists)
-  int cap = 4;
-  if (const char* v = std::getenv("TSB200_POOLS")) cap = std::max(1, std::min(4, std::atoi(v)));
-  // the persistent kernel's tiers (ll_tiers.h) on device 0's SM count: the GPUs of one node are one model
-  return std::min(cap, tsb::ll_pools_for(tsb_device_sm_count(0), M));
-}
-inline int nq_pools_of(tsb_nq* h, int M) { return std::min(nq_pools_wanted(M), tsb_nq_pools_per_launch(h, M)); }
-void nq_devpool_multi_rounds(std::vector<tsb_nq*>& hs, int m, int M, StealBoard* sb, int me, GpuTaskResult& r) {
-  const bool no_steal = [] {
-    const char* v = std::getenv("TSB200_NO_STEAL");
-    return v && *v && *v != '0';
-  }();
+// The offload loop of one task whose P >= 1 pools (a handle and its siblings) are resident on the device: all rounds
+// of step 2 inside the library (one persistent kernel for small M, two kernels per round otherwise; the pools' rounds
+// share its launches, S::run_multi = tsb_*_pool_run_multi), `rounds` rounds per call; the host only reads counters.
+// `balance`: a pool of the group that runs dry takes the oldest half of the fullest one (as between tasks).  Between
+// two calls a thief task is served from the fullest pool of the group.  best[i]: pool i's incumbent.
+template <class S, class H>
+void devpool_rounds(const S& s, const std::vector<H*>& hs, int m, int M, int64_t rounds, bool balance, StealBoard* sb,
+                    int me, int64_t* best, GpuTaskResult& r) {
   const int P = static_cast<int>(hs.size());
   const auto fullest = [&] {
     int v = 0;
     for (int i = 1; i < P; i++)
-      if (tsb_nq_pool_size(hs[i]) > tsb_nq_pool_size(hs[v])) v = i;
+      if (pool_size(hs[i]) > pool_size(hs[v])) v = i;
     return v;
   };
-  // a thief task is served from the fullest pool of the group
-  const auto steal = [&](void*, void* t, int64_t* got) {
-    return tsb_nq_pool_steal(hs[fullest()], static_cast<tsb_nq*>(t), m, got);
-  };
+  const auto steal = [&](void*, void* t, int64_t* got) { return pool_steal(hs[fullest()], static_cast<H*>(t), m, got); };
   const long long floor_ = steal_floor(m, M);
   std::vector<uint64_t> out(4 * P);
   while (r.rc == TSB_OK) {
-    if (!no_steal) {  // balance inside the group: every dry pool takes half of the fullest one
+    if (balance) {
       for (int i = 0; i < P && r.rc == TSB_OK; i++) {
-        if (tsb_nq_pool_size(hs[i]) >= m) continue;
+        if (pool_size(hs[i]) >= m) continue;
         const int v = fullest();
-        if (v == i || tsb_nq_pool_size(hs[v]) < floor_) break;
+        if (v == i || pool_size(hs[v]) < floor_) break;
         int64_t got = 0;
-        r.rc = tsb_nq_pool_steal(hs[v], hs[i], m, &got);
+        r.rc = pool_steal(hs[v], hs[i], m, &got);
       }
       if (r.rc != TSB_OK) break;
     }
     long long most = 0, total = 0;
-    for (tsb_nq* x : hs) {
-      most = std::max<long long>(most, tsb_nq_pool_size(x));
-      total += tsb_nq_pool_size(x);
+    for (H* x : hs) {
+      most = std::max<long long>(most, pool_size(x));
+      total += pool_size(x);
     }
     if (most < m) {
       if (!board_acquire(sb, me, total, floor_)) break;
       continue;
     }
-    r.rc = tsb_nq_pool_run_multi(hs.data(), P, m, M, sb ? rounds_per_call(sb, M) : 2048, out.data());
+    r.rc = s.run_multi(hs.data(), P, m, M, rounds, best, out.data());
     if (r.rc != TSB_OK) break;
     for (int i = 0; i < P; i++) {
       r.offloads += out[4 * i];
@@ -402,45 +370,60 @@ void nq_devpool_multi_rounds(std::vector<tsb_nq*>& hs, int m, int M, StealBoard*
       r.tree += out[4 * i + 2];
       r.sol += out[4 * i + 3];
     }
-    r.rc = board_service(sb, me, tsb_nq_pool_size(hs[fullest()]), floor_, steal);
+    r.rc = board_service(sb, me, pool_size(hs[fullest()]), floor_, steal);
   }
   if (r.rc != TSB_OK) board_abort(sb, me);
 }
-// pool -> device, all rounds, leftovers (fewer than m nodes) back to the host pool for step 3
-template <class Node>
-void nq_devpool_on(tsb_nq* h, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb = nullptr, int me = 0) {
-  const uint64_t l0 = tsb_nq_kernel_launches(h);
-  if (const int P = nq_pools_of(h, M); P > 1) {
-    std::vector<tsb_nq*> hs{h};
-    for (int i = 1; i < P && r.rc == TSB_OK; i++) {
-      tsb_nq* sib = nullptr;
-      r.rc = tsb_nq_sibling(h, i, &sib);
-      hs.push_back(sib);
-    }
-    std::vector<Pool<Node>> part;
-    if (r.rc == TSB_OK) static_split(pool, P, part);
-    long long most = 0;
-    for (int i = 0; i < P && r.rc == TSB_OK; i++) {
-      r.rc = tsb_nq_pool_push(hs[i], &part[i].el[part[i].front], static_cast<int64_t>(part[i].size));
-      most = std::max<long long>(most, tsb_nq_pool_size(hs[i]));
-    }
-    if (sb) sb->publish_handle(me, r.rc == TSB_OK ? h : nullptr, most);
-    if (r.rc == TSB_OK) nq_devpool_multi_rounds(hs, m, M, sb, me, r);
-    for (tsb_nq* x : hs) {
-      if (r.rc != TSB_OK) break;
-      r.rc = drain_to_host(x, pool, tsb_nq_pool_size, tsb_nq_pool_drain);
-    }
-    r.launches = tsb_nq_kernel_launches(h) - l0;
-    return;
+
+// One task's step 2 on device pools: its pool -> the P = S::pools_on(h, M) device pools of h and its siblings (for
+// P > 1 split once more, by the reference's own strided split), all rounds, and the leftovers (fewer than m nodes per
+// pool) back to the task's pool.  Each of several pools is one reference task with its own incumbent
+// (pfsp_multigpu_chpl.chpl:384), min-reduced here, and hands its leftovers back as a reference task does (popBack).
+template <class S, class H, class Node>
+void devpool_on(const S& s, H* h, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me) {
+  const uint64_t l0 = kernel_launches(h);
+  const int P = s.pools_on(h, M);
+  std::vector<H*> hs{h};
+  for (int i = 1; i < P && r.rc == TSB_OK; i++) {
+    H* sib = nullptr;
+    r.rc = pool_sibling(h, i, &sib);
+    hs.push_back(sib);
   }
-  r.rc = tsb_nq_pool_push(h, &pool.el[pool.front], static_cast<int64_t>(pool.size));
-  pool.front = 0;
-  pool.size = 0;
-  if (sb) sb->publish_handle(me, r.rc == TSB_OK ? h : nullptr, tsb_nq_pool_size(h));
-  if (r.rc == TSB_OK) nq_devpool_rounds(h, m, M, sb, me, r);
-  if (r.rc == TSB_OK) r.rc = drain_to_host(h, pool, tsb_nq_pool_size, tsb_nq_pool_drain);
-  r.launches = tsb_nq_kernel_launches(h) - l0;
+  std::vector<Pool<Node>> part;
+  if (r.rc == TSB_OK) static_split(pool, P, part);
+  long long most = 0;
+  for (int i = 0; i < P && r.rc == TSB_OK; i++) {
+    r.rc = pool_push(hs[i], &part[i].el[part[i].front], static_cast<int64_t>(part[i].size));
+    most = std::max<long long>(most, pool_size(hs[i]));
+  }
+  if (sb) sb->publish_handle(me, r.rc == TSB_OK ? h : nullptr, most);
+  std::unique_ptr<int64_t[]> best(new int64_t[P]);
+  std::fill(best.get(), best.get() + P, r.best);
+  if (r.rc == TSB_OK) devpool_rounds(s, hs, m, M, s.rounds(P, sb != nullptr, M), s.balance, sb, me, best.get(), r);
+  r.best = *std::min_element(best.get(), best.get() + P);
+  for (H* x : hs) {
+    if (r.rc != TSB_OK) break;
+    Pool<Node> rest;
+    r.rc = drain_to_host(x, P == 1 ? pool : rest);
+    for (Node n; rest.popBack(n);) pool.pushBack(n);
+  }
+  r.launches = kernel_launches(h) - l0;
 }
+
+// Several pools per task (TSB200_POOLS=1 turns it off, =2 caps it at two): for chunks that fit the persistent kernel a
+// round is a chain of L2 round trips with little work in between, so the task's share of the warm-up pool is split
+// once more — the reference's own strided split (static_split) — into P device pools (P = tsb_nq_pools_per_launch: 4
+// on an H100 for M <= 50688) whose rounds run in ONE launch (tsb_nq_pool_run_multi), two CTAs of different pools on
+// every SM filling each other's waits.  Each pool follows the reference's rule on its own nodes: for D tasks the
+// chunk sequence is that of a 2-level split into P D pools, the totals are split-invariant.
+inline int nq_pools_wanted(int M) {  // (decides the warm-up size, before any handle exists)
+  int cap = 4;
+  if (const char* v = std::getenv("TSB200_POOLS")) cap = std::max(1, std::min(4, std::atoi(v)));
+  // the persistent kernel's tiers (ll_tiers.h) on device 0's SM count: the GPUs of one node are one model
+  return std::min(cap, tsb::ll_pools_for(tsb_device_sm_count(0), M));
+}
+inline int nq_pools_of(tsb_nq* h, int M) { return std::min(nq_pools_wanted(M), tsb_nq_pools_per_launch(h, M)); }
+
 // Handles of the device-pool drivers are kept between searches (per device, N, g, M): a handle with its sibling
 // pools, arenas and fat arenas is ~1.4 GB of cudaMalloc / cudaFree per GPU, which at 8 GPUs cost more than the N = 17
 // search itself.  (The Chapel drivers declare their device arrays once, outside the search loop, as well.)
@@ -502,40 +485,6 @@ struct NqHandleCache {
 NqHandleCache& nq_handle_cache() {
   static NqHandleCache* c = new NqHandleCache();  // (never destroyed: no CUDA calls at process exit)
   return *c;
-}
-
-template <class Node>
-void nq_devpool_task(int device, int N, int g, int m, int M, Pool<Node>& pool, GpuTaskResult& r,
-                     StealBoard* sb = nullptr, int me = 0) {
-  tsb_nq* h = nullptr;
-  const bool trace = std::getenv("TSB200_TRACE") != nullptr;
-  const double tt0 = now_s();
-  h = nq_handle_cache().acquire<Node>(device, N, g, M, &r.rc);
-  if (r.rc != TSB_OK) {
-    if (sb) sb->publish_handle(me, nullptr, 0);
-    return;
-  }
-  const double tt1 = now_s();
-  nq_devpool_on(h, m, M, pool, r, sb, me);
-  const double tt2 = now_s();
-  nq_handle_cache().release(h, device, N, g, M, sizeof(Node), r.rc == TSB_OK);
-  if (trace) std::fprintf(stderr, "[tsb200] device %d: create %.1f ms, %llu rounds in %.1f ms, destroy %.1f ms\n", device,
-                          (tt1 - tt0) * 1e3, static_cast<unsigned long long>(r.offloads), (tt2 - tt1) * 1e3,
-                          (now_s() - tt2) * 1e3);
-}
-
-// static strided split of the warm-up pool (nqueens_multigpu_chpl.chpl:199-226)
-template <class Node>
-void static_split(Pool<Node>& pool, int D, std::vector<Pool<Node>>& multi) {
-  const size_t poolSize = pool.size, c = poolSize / D, l = poolSize - (D - 1) * c, f = pool.front;
-  multi.resize(D);
-  for (int g = 0; g < D; g++) {
-    for (size_t i = 0; i < c; i++) multi[g].pushBack(pool.el[g + f + i * D]);
-    if (g == D - 1)
-      for (size_t i = 0; i < l - c; i++) multi[g].pushBack(pool.el[D * c + f + i]);
-  }
-  pool.front = 0;
-  pool.size = 0;
 }
 
 // ------------------------------------------------------------------ PFSP CPU twin
@@ -674,177 +623,6 @@ void pfsp_generate_children(int jobs, const tsb_pfsp_node* parents, int size, co
   }
 }
 
-void pfsp_gpu_task(int device, const tsb_pfsp_tables& t, int lb_kind, int m, int M, Pool<tsb_pfsp_node>& pool,
-                   GpuTaskResult& r) {
-  tsb_pfsp* h = nullptr;
-  r.rc = tsb_pfsp_create_from_tables(&h, device, M, &t);
-  if (r.rc != TSB_OK) return;
-  const int jobs = t.jobs;
-  std::vector<tsb_pfsp_node> parents(M);
-  std::vector<int32_t> bounds(static_cast<size_t>(M) * jobs);
-  // the chunk arrays live for the whole step 2 (pfsp_gpu_chpl.chpl:355-356): page-lock them once
-  tsb_pfsp_register_host(h, parents.data(), parents.size() * sizeof(tsb_pfsp_node));
-  tsb_pfsp_register_host(h, bounds.data(), bounds.size() * sizeof(int32_t));
-  for (;;) {
-    const int n = pool.popBackBulk(m, M, parents.data());
-    if (n <= 0) break;
-    r.rc = tsb_pfsp_evaluate(h, lb_kind, parents.data(), n, r.best, bounds.data());
-    if (r.rc != TSB_OK) break;
-    ++r.offloads;
-    r.parents += static_cast<uint64_t>(n);
-    pfsp_generate_children(jobs, parents.data(), n, bounds.data(), r.tree, r.sol, r.best, pool);
-  }
-  r.launches = tsb_pfsp_kernel_launches(h);
-  tsb_pfsp_destroy(h);
-}
-
-// Several device pools per task, as many as the caller asks for (tsb_pfsp_search_device_pools): the PFSP twin of
-// nq_devpool_multi_rounds.  Every pool is one reference task with its own incumbent best[i]
-// (pfsp_multigpu_chpl.chpl:384); the pools' rounds share the launches of the persistent kernel
-// (tsb_pfsp_pool_run_multi, which runs them one after the other where one launch cannot take them: same rounds).
-// `balance` (ub = 1 only: moves keep the counts only while best is constant): a pool of the group that runs dry takes
-// the oldest half of the fullest one, and a thief task is served from the fullest pool.
-void pfsp_devpool_multi_rounds(std::vector<tsb_pfsp*>& hs, int lb_kind, int m, int M, bool balance, StealBoard* sb,
-                               int me, std::vector<int64_t>& best, GpuTaskResult& r) {
-  const int P = static_cast<int>(hs.size());
-  const auto fullest = [&] {
-    int v = 0;
-    for (int i = 1; i < P; i++)
-      if (tsb_pfsp_pool_size(hs[i]) > tsb_pfsp_pool_size(hs[v])) v = i;
-    return v;
-  };
-  const auto steal = [&](void*, void* t, int64_t* got) {
-    return tsb_pfsp_pool_steal(hs[fullest()], static_cast<tsb_pfsp*>(t), m, got);
-  };
-  const long long floor_ = steal_floor(m, M);
-  std::vector<uint64_t> out(4 * P);
-  while (r.rc == TSB_OK) {
-    if (balance) {
-      for (int i = 0; i < P && r.rc == TSB_OK; i++) {
-        if (tsb_pfsp_pool_size(hs[i]) >= m) continue;
-        const int v = fullest();
-        if (v == i || tsb_pfsp_pool_size(hs[v]) < floor_) break;
-        int64_t got = 0;
-        r.rc = tsb_pfsp_pool_steal(hs[v], hs[i], m, &got);
-      }
-      if (r.rc != TSB_OK) break;
-    }
-    long long most = 0, total = 0;
-    for (tsb_pfsp* x : hs) {
-      most = std::max<long long>(most, tsb_pfsp_pool_size(x));
-      total += tsb_pfsp_pool_size(x);
-    }
-    if (most < m) {
-      if (!board_acquire(sb, me, total, floor_)) break;
-      continue;
-    }
-    r.rc = tsb_pfsp_pool_run_multi(hs.data(), P, lb_kind, m, M, rounds_per_call(balance || sb, M), best.data(),
-                                   out.data());
-    if (r.rc != TSB_OK) break;
-    for (int i = 0; i < P; i++) {
-      r.offloads += out[4 * i];
-      r.parents += out[4 * i + 1];
-      r.tree += out[4 * i + 2];
-      r.sol += out[4 * i + 3];
-    }
-    r.rc = board_service(sb, me, tsb_pfsp_pool_size(hs[fullest()]), floor_, steal);
-  }
-  if (r.rc != TSB_OK) board_abort(sb, me);
-}
-
-// the same loop with the task's pool resident on the device (tsb_pfsp_pool_*)
-void pfsp_devpool_on(tsb_pfsp* h, int lb_kind, int m, int M, Pool<tsb_pfsp_node>& pool, GpuTaskResult& r,
-                     StealBoard* sb = nullptr, int me = 0, int pools = 1, bool balance = false) {
-  const uint64_t l0 = tsb_pfsp_kernel_launches(h);
-  if (pools > 1) {  // the task's share split once more (the same strided split) into `pools` device pools
-    std::vector<tsb_pfsp*> hs{h};
-    for (int i = 1; i < pools && r.rc == TSB_OK; i++) {
-      tsb_pfsp* sib = nullptr;
-      r.rc = tsb_pfsp_sibling(h, i, &sib);
-      hs.push_back(sib);
-    }
-    std::vector<Pool<tsb_pfsp_node>> part;
-    if (r.rc == TSB_OK) static_split(pool, pools, part);
-    long long most = 0;
-    for (int i = 0; i < pools && r.rc == TSB_OK; i++) {
-      r.rc = tsb_pfsp_pool_push(hs[i], &part[i].el[part[i].front], static_cast<int64_t>(part[i].size));
-      most = std::max<long long>(most, tsb_pfsp_pool_size(hs[i]));
-    }
-    if (sb) sb->publish_handle(me, r.rc == TSB_OK ? h : nullptr, most);
-    std::vector<int64_t> best(pools, r.best);
-    if (r.rc == TSB_OK) pfsp_devpool_multi_rounds(hs, lb_kind, m, M, balance, sb, me, best, r);
-    r.best = *std::min_element(best.begin(), best.end());
-    // leftovers pool by pool, each handed back as a reference task hands back its own (popBack onto the pool)
-    for (tsb_pfsp* x : hs) {
-      if (r.rc != TSB_OK) break;
-      Pool<tsb_pfsp_node> rest;
-      r.rc = drain_to_host(x, rest, tsb_pfsp_pool_size, tsb_pfsp_pool_drain);
-      for (tsb_pfsp_node n; rest.popBack(n);) pool.pushBack(n);
-    }
-    r.launches = tsb_pfsp_kernel_launches(h) - l0;
-    return;
-  }
-  r.rc = tsb_pfsp_pool_push(h, &pool.el[pool.front], static_cast<int64_t>(pool.size));
-  pool.front = 0;
-  pool.size = 0;
-  if (sb) sb->publish_handle(me, r.rc == TSB_OK ? h : nullptr, tsb_pfsp_pool_size(h));
-  const auto steal = [m](void* v, void* t, int64_t* got) {
-    return tsb_pfsp_pool_steal(static_cast<tsb_pfsp*>(v), static_cast<tsb_pfsp*>(t), m, got);
-  };
-  // all rounds of step 2 inside the library (one persistent kernel for lb1 / lb1_d and small M, two kernels per
-  // round otherwise); thieves are served between calls
-  while (r.rc == TSB_OK) {
-    uint64_t nr = 0, np = 0, nc = 0, ns = 0;
-    r.rc = tsb_pfsp_pool_run(h, lb_kind, m, M, rounds_per_call(sb, M), &r.best, &nr, &np, &nc, &ns);
-    if (r.rc != TSB_OK) break;
-    r.tree += nc;
-    r.sol += ns;
-    r.offloads += nr;
-    r.parents += np;
-    const long long size = tsb_pfsp_pool_size(h);
-    if (size >= m) {
-      r.rc = board_service(sb, me, size, steal_floor(m, M), steal);
-      continue;
-    }
-    if (!board_acquire(sb, me, size, steal_floor(m, M))) break;
-  }
-  if (r.rc != TSB_OK) board_abort(sb, me);
-  if (r.rc == TSB_OK) r.rc = drain_to_host(h, pool, tsb_pfsp_pool_size, tsb_pfsp_pool_drain);
-  r.launches = tsb_pfsp_kernel_launches(h) - l0;
-}
-void pfsp_devpool_task(int device, const tsb_pfsp_tables& t, int lb_kind, int m, int M, Pool<tsb_pfsp_node>& pool,
-                       GpuTaskResult& r, StealBoard* sb = nullptr, int me = 0, int pools = 1, bool balance = false) {
-  tsb_pfsp* h = nullptr;
-  r.rc = tsb_pfsp_create_from_tables(&h, device, M, &t);
-  if (r.rc != TSB_OK) {
-    if (sb) sb->publish_handle(me, nullptr, 0);
-    return;
-  }
-  pfsp_devpool_on(h, lb_kind, m, M, pool, r, sb, me, pools, balance);
-  tsb_pfsp_destroy(h);
-}
-void pfsp_gpu_task_nosteal(int device, const tsb_pfsp_tables& t, int lb_kind, int m, int M, Pool<tsb_pfsp_node>& pool,
-                           GpuTaskResult& r, StealBoard*, int, int, bool) {
-  pfsp_gpu_task(device, t, lb_kind, m, M, pool, r);
-}
-
-}  // namespace
-
-// ====================================================================== exported
-extern "C" {
-
-int tsb_taillard_nb_jobs(int id) {
-  return id > 110 ? 500 : id > 90 ? 200 : id > 60 ? 100 : id > 30 ? 50 : 20;
-}
-int tsb_taillard_nb_machines(int id) {
-  static const int m[12] = {5, 10, 20, 5, 10, 20, 5, 10, 20, 10, 20, 20};  // per group of ten instances
-  if (id < 1 || id > 120) return -1;
-  return m[(id - 1) / 10];
-}
-int64_t tsb_taillard_best_ub(int id) { return (id < 1 || id > 120) ? -1 : kBestUb[id - 1]; }
-
-}  // extern "C"
-namespace {
 // lbound1 / lbound2 of a Taillard instance (pfsp_gpu_chpl.chpl:325-332) into either table struct
 template <class T, int MAXJ>
 int build_tables(T* t, int inst, int variant) {
@@ -918,247 +696,209 @@ int build_tables(T* t, int inst, int variant) {
   }
   return TSB_OK;
 }
-}  // namespace
-extern "C" {
 
-int tsb_pfsp_tables_build(tsb_pfsp_tables* t, int inst) { return tsb_pfsp_tables_build_variant(t, inst, TSB_LB2_FULL); }
-int tsb_pfsp_tables_build_variant(tsb_pfsp_tables* t, int inst, int variant) {
-  return build_tables<tsb_pfsp_tables, TSB_MAX_JOBS>(t, inst, variant);
-}
-int tsb_pfsp_tables50_build(tsb_pfsp_tables50* t, int inst, int variant) {
-  return build_tables<tsb_pfsp_tables50, TSB_MAX_JOBS_WIDE>(t, inst, variant);
-}
-int tsb_pfsp_create50_from_tables(tsb_pfsp** h, int device, int M_max, const tsb_pfsp_tables50* t) {
-  if (!t) return TSB_EINVAL;
-  return tsb_pfsp_create_wide(h, device, TSB_MAX_JOBS_WIDE, t->jobs, t->machines, M_max, t->p_times, t->min_heads,
-                              t->min_tails, t->pairs, t->johnson, t->lags, t->mp0, t->mp1, t->mp_order);
-}
+// ------------------------------------------------------------------ the 3-step search
+// The problems of the search.  Each gives the root node and decompose, the incumbent the search starts from (N-Queens:
+// 0), the task of one device on its host pool (host_task) or on device pools (device_task), `pools` (device pools per
+// task: step 1 warms up D·m·pools nodes), whether device-pool tasks `steal` from each other, and for the device pools
+// of one task (devpool_on): how many a handle takes, the rounds per library call, `balance` and run_multi.
 
-int tsb_pfsp_create_from_tables(tsb_pfsp** h, int device, int M_max, const tsb_pfsp_tables* t) {
-  if (!t) return TSB_EINVAL;
-  return tsb_pfsp_create(h, device, t->jobs, t->machines, M_max, t->p_times, t->min_heads, t->min_tails,
-                         t->pairs, t->johnson, t->lags, t->mp0, t->mp1, t->mp_order);
-}
-
-}  // extern "C"
-namespace {
-template <class Node>
-int nq_search_host(int N, int g, int m, int M, int D, tsb_search_stats* out) {
-  const int max_n = std::is_same_v<Node, tsb_nq_node24> ? TSB_MAX_QUEENS_WIDE : TSB_MAX_QUEENS;
-  if (!out || N < 1 || N > max_n || g < 1 || m < 1 || M < 1 || D < 1 || D > 8) return TSB_EINVAL;
-  std::memset(out, 0, sizeof(*out));
-  if (int rc = tsb_init_devices(D); rc != TSB_OK) return rc;  // contexts exist before the timers start
-  Pool<Node> pool;
-  Node root{};
-  for (int i = 0; i < N; i++) root.board[i] = static_cast<uint8_t>(i);
-  pool.pushBack(root);
-  uint64_t tree = 0, sol = 0;
-  Node parent;
-  double t0 = now_s();
-  while (pool.size < static_cast<size_t>(D) * m) {  // step 1 (nqueens_multigpu_chpl.chpl:173-179)
-    if (!pool.popFront(parent)) break;
+// N-Queens on boards of up to 20 queens (tsb_nq_node) or, on wide handles, 24 (tsb_nq_node24)
+template <class NodeT>
+struct NqSearch {
+  using Node = NodeT;
+  using Handle = tsb_nq;
+  static constexpr bool wide = std::is_same_v<Node, tsb_nq_node24>;
+  int N, g;
+  bool devpool;
+  int pools;  // (one on wide handles, which do not share launches of the persistent kernel)
+  bool steal, balance;
+  int64_t initial_best = 0;
+  NqSearch(int N_, int g_, int M, bool devpool_)
+      : N(N_), g(g_), devpool(devpool_), pools(devpool_ && !wide ? nq_pools_wanted(M) : 1),
+        steal(devpool_ && steal_allowed()), balance(steal) {}
+  Node root() const {
+    Node root{};
+    for (int i = 0; i < N; i++) root.board[i] = static_cast<uint8_t>(i);
+    return root;
+  }
+  void decompose(const Node& parent, uint64_t& tree, uint64_t& sol, int64_t&, Pool<Node>& pool) const {
     nq_decompose(N, parent, tree, sol, pool);
   }
-  double t1 = now_s();
-  out->t_step1 = t1 - t0;
-  std::vector<GpuTaskResult> res(D);  // step 2
-  // task g drives GPU g; with fewer than D GPUs present the tasks wrap around (g % ndev): the
-  // per-task pools stay independent, so counts are unchanged — used to test D > 1 on one GPU
-  const int ndev = std::max(1, tsb_device_count());
-  if (D == 1) {
-    nq_gpu_task(0, N, g, m, M, pool, res[0]);
-  } else {
-    std::vector<Pool<Node>> multi;
-    static_split(pool, D, multi);
-    std::vector<std::thread> th;
-    for (int gid = 0; gid < D; gid++)
-      th.emplace_back([&, gid] {
-        bind_task(gid % ndev, true);
-        nq_gpu_task(gid % ndev, N, g, m, M, multi[gid], res[gid]);
-      });
-    for (auto& x : th) x.join();
-    for (int gid = 0; gid < D; gid++)  // leftovers back to the global pool (:315-320)
-      while (multi[gid].popBack(parent)) pool.pushBack(parent);
-  }
-  for (int gid = 0; gid < D; gid++) {
-    if (res[gid].rc != TSB_OK) return res[gid].rc;
-    tree += res[gid].tree;
-    sol += res[gid].sol;
-    out->offloads += res[gid].offloads;
-    out->offloaded_parents += res[gid].parents;
-    out->kernel_launches += res[gid].launches;
-    out->per_gpu_tree[gid] = res[gid].tree;
-  }
-  double t2 = now_s();
-  out->t_step2 = t2 - t1;
-  while (pool.popBack(parent)) nq_decompose(N, parent, tree, sol, pool);  // step 3
-  out->t_step3 = now_s() - t2;
-  out->explored_tree = tree;
-  out->explored_sol = sol;
-  return TSB_OK;
-}
-
-// part < 0: the whole search.  part >= 0: only task `part` of the D-way static split, on `device` (one rank of a
-// process-per-GPU launch): the step-1 tree is credited to part 0 and every part drains its own leftovers, so the
-// per-part counts add up to the whole search's.  `on` != nullptr: D = 1 on a handle the caller created (set-up
-// outside the search's timers, as the Chapel drivers' `on device var` declarations are).
-template <class Node>
-int nq_search_device_impl(int N, int g, int m, int M, int D, int part, int device, tsb_nq* on, tsb_search_stats* out) {
-  constexpr bool wide = std::is_same_v<Node, tsb_nq_node24>;
-  if (!out || N < 1 || N > (wide ? TSB_MAX_QUEENS_WIDE : TSB_MAX_QUEENS) || g < 1 || m < 1 || M < 1 || D < 1 || D > 8 ||
-      part >= D)
-    return TSB_EINVAL;
-  std::memset(out, 0, sizeof(*out));
-  if (!on)
-    if (int rc = tsb_init_devices(part < 0 ? D : device + 1); rc != TSB_OK) return rc;
-  Pool<Node> pool;
-  Node root{};
-  for (int i = 0; i < N; i++) root.board[i] = static_cast<uint8_t>(i);
-  pool.pushBack(root);
-  uint64_t tree = 0, sol = 0;
-  Node parent;
-  double t0 = now_s();
-  // step 1 on the CPU, as in the reference: m nodes for every pool (one pool per task on wide handles, which do not
-  // share launches of the persistent kernel)
-  while (pool.size < static_cast<size_t>(D) * m * (wide ? 1 : nq_pools_wanted(M))) {
-    if (!pool.popFront(parent)) break;
-    nq_decompose(N, parent, tree, sol, pool);
-  }
-  double t1 = now_s();
-  out->t_step1 = t1 - t0;
-  // step 2: every task's pool moves to its device and stays there (same static split as tsb_nq_search); tasks
-  // that run dry steal from the fullest device pool peer-to-peer
-  std::vector<GpuTaskResult> res(D);
-  const int ndev = std::max(1, tsb_device_count());
-  if (on) {
-    nq_devpool_on(on, m, M, pool, res[0]);
-  } else if (part >= 0) {
-    if (part != 0) tree = sol = 0;  // step 1 is credited to part 0
-    std::vector<Pool<Node>> multi;
-    if (D == 1) {
-      multi.resize(1);
-      std::swap(multi[0], pool);
-    } else {
-      static_split(pool, D, multi);
+  // one GPU task's offload loop (nqueens_gpu_chpl.chpl:197-215; nqueens_multigpu_chpl.chpl:234-253)
+  void host_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r) const {
+    tsb_nq* h = nullptr;
+    r.rc = nq_create_for<Node>(&h, device, N, g, M);
+    if (r.rc != TSB_OK) return;
+    std::vector<Node> parents(M);
+    std::vector<uint8_t> labels(static_cast<size_t>(M) * N);
+    // the chunk arrays live for the whole step 2 (nqueens_gpu_chpl.chpl:191-192): page-lock them once
+    tsb_nq_register_host(h, parents.data(), parents.size() * sizeof(Node));
+    tsb_nq_register_host(h, labels.data(), labels.size());
+    for (;;) {
+      const int n = pool.popBackBulk(m, M, parents.data());
+      if (n <= 0) break;
+      r.rc = tsb_nq_evaluate(h, parents.data(), n, labels.data());
+      if (r.rc != TSB_OK) break;
+      ++r.offloads;
+      r.parents += static_cast<uint64_t>(n);
+      nq_generate_children(N, parents.data(), n, labels.data(), r.tree, r.sol, pool);
     }
-    nq_devpool_task(device, N, g, m, M, multi[part], res[part]);
-    while (multi[part].popBack(parent)) pool.pushBack(parent);
-  } else if (D == 1) {
-    nq_devpool_task(0, N, g, m, M, pool, res[0]);
-  } else {
-    std::vector<Pool<Node>> multi;
-    static_split(pool, D, multi);
-    StealBoard board(D);
-    StealBoard* sb = std::getenv("TSB200_NO_STEAL") ? nullptr : &board;
-    std::vector<std::thread> th;
-    for (int gid = 0; gid < D; gid++)
-      th.emplace_back([&, gid] {
-        bind_task(gid % ndev, true);
-        nq_devpool_task(gid % ndev, N, g, m, M, multi[gid], res[gid], sb, gid);
-      });
-    for (auto& x : th) x.join();
-    for (int gid = 0; gid < D; gid++)
-      while (multi[gid].popBack(parent)) pool.pushBack(parent);
-    out->steals = board.steals;
+    r.launches = tsb_nq_kernel_launches(h);
+    tsb_nq_destroy(h);
   }
-  for (int gid = 0; gid < D; gid++) {
-    if (res[gid].rc != TSB_OK) return res[gid].rc;
-    tree += res[gid].tree;
-    sol += res[gid].sol;
-    out->offloads += res[gid].offloads;
-    out->offloaded_parents += res[gid].parents;
-    out->kernel_launches += res[gid].launches;
-    out->per_gpu_tree[gid] = res[gid].tree;
+  void device_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me) const {
+    const double tt0 = now_s();
+    tsb_nq* h = nq_handle_cache().acquire<Node>(device, N, g, M, &r.rc);
+    if (r.rc != TSB_OK) {
+      if (sb) sb->publish_handle(me, nullptr, 0);
+      return;
+    }
+    const double tt1 = now_s();
+    devpool_on(*this, h, m, M, pool, r, sb, me);
+    const double tt2 = now_s();
+    nq_handle_cache().release(h, device, N, g, M, sizeof(Node), r.rc == TSB_OK);
+    if (std::getenv("TSB200_TRACE"))
+      std::fprintf(stderr, "[tsb200] device %d: create %.1f ms, %llu rounds in %.1f ms, destroy %.1f ms\n", device,
+                   (tt1 - tt0) * 1e3, static_cast<unsigned long long>(r.offloads), (tt2 - tt1) * 1e3,
+                   (now_s() - tt2) * 1e3);
   }
-  double t2 = now_s();
-  out->t_step2 = t2 - t1;
-  while (pool.popBack(parent)) nq_decompose(N, parent, tree, sol, pool);  // step 3
-  out->t_step3 = now_s() - t2;
-  out->explored_tree = tree;
-  out->explored_sol = sol;
-  return TSB_OK;
-}
-}  // namespace
-extern "C" {
+  int pools_on(tsb_nq* h, int M) const { return nq_pools_of(h, M); }
+  // (with no thief to serve, the dry pools of a group rebalance every 2048 rounds)
+  int64_t rounds(int P, bool sb, int M) const { return P == 1 || sb ? rounds_per_call(sb, M) : 2048; }
+  int run_multi(tsb_nq* const* hs, int P, int m, int M, int64_t rounds, int64_t*, uint64_t* out) const {
+    return tsb_nq_pool_run_multi(hs, P, m, M, rounds, out);
+  }
+};
 
-int tsb_nq_search(int N, int g, int m, int M, int D, tsb_search_stats* out) {
-  return N > TSB_MAX_QUEENS ? nq_search_host<tsb_nq_node24>(N, g, m, M, D, out)
-                            : nq_search_host<tsb_nq_node>(N, g, m, M, D, out);
-}
-int tsb_nq_search_wide(int max_queens, int N, int g, int m, int M, int D, tsb_search_stats* out) {
-  if (max_queens != TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
-  return nq_search_host<tsb_nq_node24>(N, g, m, M, D, out);
-}
-
-// pools > 1 (device pools only): every task's share split once more into `pools` device pools (pfsp_devpool_on)
-static int pfsp_search_impl(int inst, int lb_kind, int ub, int m, int M, int D, bool devpool, int part, int device,
-                            tsb_pfsp* on, tsb_search_stats* out, int pools = 1) {
-  if (!out || lb_kind < 0 || lb_kind > 2 || (ub != 0 && ub != 1) || m < 1 || M < 1 || D < 1 || D > 8 || part >= D ||
-      pools < 1 || pools > 4)
-    return TSB_EINVAL;
-  std::memset(out, 0, sizeof(*out));
-  std::vector<tsb_pfsp_tables> tv(1);
-  tsb_pfsp_tables& t = tv[0];
-  int rc = tsb_pfsp_tables_build(&t, inst);
-  if (rc != TSB_OK) return rc;
-  if (!on)
-    if (rc = tsb_init_devices(part < 0 ? D : device + 1); rc != TSB_OK) return rc;  // contexts exist before the timers start
-  HostBounds hb(t);
-  int64_t best = ub == 1 ? tsb_taillard_best_ub(inst) : INT64_MAX;  // pfsp_gpu_chpl.chpl:37
-  Pool<tsb_pfsp_node> pool;
-  tsb_pfsp_node root{};
-  root.limit1 = -1;
-  for (int i = 0; i < t.jobs; i++) root.prmu[i] = i;
-  pool.pushBack(root);
-  uint64_t tree = 0, sol = 0;
-  tsb_pfsp_node parent;
-  double t0 = now_s();
-  while (pool.size < static_cast<size_t>(D) * m * pools) {  // m nodes for every pool
-    if (!pool.popFront(parent)) break;
+// PFSP on the tables of a Taillard instance; `pools` device pools per task, as many as the caller asks for
+struct PfspSearch {
+  using Node = tsb_pfsp_node;
+  using Handle = tsb_pfsp;
+  HostBounds hb;
+  int lb_kind;
+  bool devpool;
+  int pools;
+  // moves between pools keep the counts only while best is constant: --ub 1 (SURVEY A.6)
+  bool steal, balance;
+  int64_t initial_best;
+  PfspSearch(const tsb_pfsp_tables& t, int inst, int lb_kind_, int ub, bool devpool_, int pools_)
+      : hb(t), lb_kind(lb_kind_), devpool(devpool_), pools(pools_), steal(devpool_ && ub == 1 && steal_allowed()),
+        balance(pools_ > 1 && ub == 1 && steal_allowed()),
+        initial_best(ub == 1 ? tsb_taillard_best_ub(inst) : INT64_MAX) {}  // pfsp_gpu_chpl.chpl:37
+  Node root() const {
+    Node root{};
+    root.limit1 = -1;
+    for (int i = 0; i < hb.t.jobs; i++) root.prmu[i] = i;
+    return root;
+  }
+  void decompose(const Node& parent, uint64_t& tree, uint64_t& sol, int64_t& best, Pool<Node>& pool) const {
     pfsp_decompose(hb, lb_kind, parent, tree, sol, best, pool);
   }
+  void host_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r) const {
+    tsb_pfsp* h = nullptr;
+    r.rc = tsb_pfsp_create_from_tables(&h, device, M, &hb.t);
+    if (r.rc != TSB_OK) return;
+    const int jobs = hb.t.jobs;
+    std::vector<tsb_pfsp_node> parents(M);
+    std::vector<int32_t> bounds(static_cast<size_t>(M) * jobs);
+    // the chunk arrays live for the whole step 2 (pfsp_gpu_chpl.chpl:355-356): page-lock them once
+    tsb_pfsp_register_host(h, parents.data(), parents.size() * sizeof(tsb_pfsp_node));
+    tsb_pfsp_register_host(h, bounds.data(), bounds.size() * sizeof(int32_t));
+    for (;;) {
+      const int n = pool.popBackBulk(m, M, parents.data());
+      if (n <= 0) break;
+      r.rc = tsb_pfsp_evaluate(h, lb_kind, parents.data(), n, r.best, bounds.data());
+      if (r.rc != TSB_OK) break;
+      ++r.offloads;
+      r.parents += static_cast<uint64_t>(n);
+      pfsp_generate_children(jobs, parents.data(), n, bounds.data(), r.tree, r.sol, r.best, pool);
+    }
+    r.launches = tsb_pfsp_kernel_launches(h);
+    tsb_pfsp_destroy(h);
+  }
+  void device_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me) const {
+    tsb_pfsp* h = nullptr;
+    r.rc = tsb_pfsp_create_from_tables(&h, device, M, &hb.t);
+    if (r.rc != TSB_OK) {
+      if (sb) sb->publish_handle(me, nullptr, 0);
+      return;
+    }
+    devpool_on(*this, h, m, M, pool, r, sb, me);
+    tsb_pfsp_destroy(h);
+  }
+  int pools_on(tsb_pfsp*, int) const { return pools; }
+  int64_t rounds(int, bool sb, int M) const { return rounds_per_call(balance || sb, M); }
+  int run_multi(tsb_pfsp* const* hs, int P, int m, int M, int64_t rounds, int64_t* best, uint64_t* out) const {
+    return tsb_pfsp_pool_run_multi(hs, P, lb_kind, m, M, rounds, best, out);
+  }
+};
+
+// The drivers' search (nqueens_multigpu_chpl.chpl, pfsp_multigpu_chpl.chpl; D = 1: nqueens_gpu_chpl.chpl,
+// pfsp_gpu_chpl.chpl) with the same Pool contract: step 1 on the CPU, step 2 on D tasks, step 3 on the CPU.
+// part < 0: the whole search.  part >= 0: only task `part` of the D-way static split, on `device` (one rank of a
+// process-per-GPU launch): the step-1 tree is credited to part 0 and every part drains its own leftovers, so the
+// per-part counts add up to the whole search's.  `on` != nullptr: D = 1 on device pools of a handle the caller created
+// (set-up outside the search's timers, as the Chapel drivers' `on device var` declarations are).
+template <class S>
+int three_step_search(const S& s, int m, int M, int D, int part, int device, typename S::Handle* on,
+                      tsb_search_stats* out) {
+  using Node = typename S::Node;
+  if (!on)
+    if (int rc = tsb_init_devices(part < 0 ? D : device + 1); rc != TSB_OK) return rc;  // contexts exist before the timers start
+  int64_t best = s.initial_best;
+  Pool<Node> pool;
+  pool.pushBack(s.root());
+  uint64_t tree = 0, sol = 0;
+  Node parent;
+  double t0 = now_s();
+  while (pool.size < static_cast<size_t>(D) * m * s.pools) {  // step 1 (nqueens_multigpu_chpl.chpl:173-179)
+    if (!pool.popFront(parent)) break;
+    s.decompose(parent, tree, sol, best, pool);
+  }
   double t1 = now_s();
   out->t_step1 = t1 - t0;
+  // step 2: on device pools, every task's pool moves to its device and stays there; tasks that run dry steal from
+  // the fullest device pool peer-to-peer
   std::vector<GpuTaskResult> res(D);
-  const int ndev = std::max(1, tsb_device_count());
   for (auto& r : res) r.best = best;  // per-task best_l = best (pfsp_multigpu_chpl.chpl:384)
-  auto task = devpool ? pfsp_devpool_task : pfsp_gpu_task_nosteal;
-  // moves between the pools of one task, as between tasks: only where they keep the counts (ub = 1)
-  const bool balance = pools > 1 && ub == 1 && !std::getenv("TSB200_NO_STEAL");
-  // a task's leftovers back to the global pool (:315-320); several pools per task already handed theirs back to
-  // the task's pool one by one, as the reference's tasks do, so that order stays
-  const auto hand_back = [&](Pool<tsb_pfsp_node>& from) {
-    if (pools > 1)
+  const auto task = [&](int dev, Pool<Node>& from, GpuTaskResult& r, StealBoard* sb, int me) {
+    if (s.devpool)
+      s.device_task(dev, m, M, from, r, sb, me);
+    else
+      s.host_task(dev, m, M, from, r);
+  };
+  // a task's leftovers back to the global pool (:315-320); several pools per task already handed theirs back to the
+  // task's pool one by one, as the reference's tasks do, so that order stays
+  const auto hand_back = [&](Pool<Node>& from) {
+    if (s.pools > 1)
       for (size_t i = 0; i < from.size; i++) pool.pushBack(from.el[from.front + i]);
     else
       while (from.popBack(parent)) pool.pushBack(parent);
   };
+  // task g drives GPU g; with fewer than D GPUs present the tasks wrap around (g % ndev): the
+  // per-task pools stay independent, so counts are unchanged — used to test D > 1 on one GPU
+  const int ndev = std::max(1, tsb_device_count());
   if (on) {
-    pfsp_devpool_on(on, lb_kind, m, M, pool, res[0], nullptr, 0, pools, balance);
-  } else if (part >= 0) {  // one task of the split (see nq_search_device_impl)
-    if (part != 0) tree = sol = 0;
-    std::vector<Pool<tsb_pfsp_node>> multi;
-    if (D == 1) {
-      multi.resize(1);
-      std::swap(multi[0], pool);
-    } else {
-      static_split(pool, D, multi);
-    }
-    task(device, t, lb_kind, m, M, multi[part], res[part], nullptr, 0, pools, balance);
+    devpool_on(s, on, m, M, pool, res[0], nullptr, 0);
+  } else if (part >= 0) {
+    if (part != 0) tree = sol = 0;  // step 1 is credited to part 0
+    std::vector<Pool<Node>> multi;
+    static_split(pool, D, multi);
+    task(device, multi[part], res[part], nullptr, 0);
     hand_back(multi[part]);
   } else if (D == 1) {
-    task(0, t, lb_kind, m, M, pool, res[0], nullptr, 0, pools, balance);
+    task(0, pool, res[0], nullptr, 0);
   } else {
-    std::vector<Pool<tsb_pfsp_node>> multi;
+    std::vector<Pool<Node>> multi;
     static_split(pool, D, multi);
     StealBoard board(D);
-    // (stealing keeps the counts only when `best` is constant: --ub 1, SURVEY A.6)
-    StealBoard* sb = (devpool && ub == 1 && !std::getenv("TSB200_NO_STEAL")) ? &board : nullptr;
+    StealBoard* sb = s.steal ? &board : nullptr;
     std::vector<std::thread> th;
     for (int gid = 0; gid < D; gid++)
       th.emplace_back([&, gid] {
-        bind_task(gid % ndev, true);
-        task(gid % ndev, t, lb_kind, m, M, multi[gid], res[gid], sb, gid, pools, balance);
+        bind_task(gid % ndev);
+        task(gid % ndev, multi[gid], res[gid], sb, gid);
       });
     for (auto& x : th) x.join();
     for (int gid = 0; gid < D; gid++) hand_back(multi[gid]);
@@ -1176,7 +916,7 @@ static int pfsp_search_impl(int inst, int lb_kind, int ub, int m, int M, int D, 
   }
   double t2 = now_s();
   out->t_step2 = t2 - t1;
-  while (pool.popBack(parent)) pfsp_decompose(hb, lb_kind, parent, tree, sol, best, pool);
+  while (pool.popBack(parent)) s.decompose(parent, tree, sol, best, pool);  // step 3
   out->t_step3 = now_s() - t2;
   out->explored_tree = tree;
   out->explored_sol = sol;
@@ -1184,12 +924,29 @@ static int pfsp_search_impl(int inst, int lb_kind, int ub, int m, int M, int D, 
   return TSB_OK;
 }
 
-// step 1 of the drivers alone (nqueens_gpu_chpl.chpl:169-175): breadth-first from the root until the pool holds
-// min_size nodes; the pool, in order, and what was explored on the way
-void tsb_release_cached_handles(void) { nq_handle_cache().clear(); }
+template <class Node>
+int nq_search(int N, int g, int m, int M, int D, bool devpool, int part, int device, tsb_nq* on,
+              tsb_search_stats* out) {
+  constexpr bool wide = std::is_same_v<Node, tsb_nq_node24>;
+  if (!out || N < 1 || N > (wide ? TSB_MAX_QUEENS_WIDE : TSB_MAX_QUEENS) || g < 1 || m < 1 || M < 1 || D < 1 || D > 8 ||
+      part >= D)
+    return TSB_EINVAL;
+  std::memset(out, 0, sizeof(*out));
+  return three_step_search(NqSearch<Node>(N, g, M, devpool), m, M, D, part, device, on, out);
+}
 
-}  // extern "C"
-namespace {
+// pools > 1 (device pools only): every task's share split once more into `pools` device pools (devpool_on)
+int pfsp_search(int inst, int lb_kind, int ub, int m, int M, int D, bool devpool, int part, int device, tsb_pfsp* on,
+                tsb_search_stats* out, int pools = 1) {
+  if (!out || lb_kind < 0 || lb_kind > 2 || (ub != 0 && ub != 1) || m < 1 || M < 1 || D < 1 || D > 8 || part >= D ||
+      pools < 1 || pools > 4)
+    return TSB_EINVAL;
+  std::memset(out, 0, sizeof(*out));
+  std::vector<tsb_pfsp_tables> tv(1);
+  if (int rc = tsb_pfsp_tables_build(&tv[0], inst); rc != TSB_OK) return rc;
+  return three_step_search(PfspSearch(tv[0], inst, lb_kind, ub, devpool, pools), m, M, D, part, device, on, out);
+}
+
 template <class Node>
 int nq_warmup(int N, int min_size, void* nodes, int64_t capacity, int64_t* n, uint64_t* tree, uint64_t* sol) {
   if (min_size < 1 || !n || !tree || !sol || (capacity && !nodes)) return TSB_EINVAL;
@@ -1213,8 +970,43 @@ int with_nq_node(bool wide, F&& f) {
   return wide ? f(tsb_nq_node24{}) : f(tsb_nq_node{});
 }
 }  // namespace
+
+// ====================================================================== exported
 extern "C" {
 
+int tsb_taillard_nb_jobs(int id) {
+  return id > 110 ? 500 : id > 90 ? 200 : id > 60 ? 100 : id > 30 ? 50 : 20;
+}
+int tsb_taillard_nb_machines(int id) {
+  static const int m[12] = {5, 10, 20, 5, 10, 20, 5, 10, 20, 10, 20, 20};  // per group of ten instances
+  if (id < 1 || id > 120) return -1;
+  return m[(id - 1) / 10];
+}
+int64_t tsb_taillard_best_ub(int id) { return (id < 1 || id > 120) ? -1 : kBestUb[id - 1]; }
+
+int tsb_pfsp_tables_build(tsb_pfsp_tables* t, int inst) { return tsb_pfsp_tables_build_variant(t, inst, TSB_LB2_FULL); }
+int tsb_pfsp_tables_build_variant(tsb_pfsp_tables* t, int inst, int variant) {
+  return build_tables<tsb_pfsp_tables, TSB_MAX_JOBS>(t, inst, variant);
+}
+int tsb_pfsp_tables50_build(tsb_pfsp_tables50* t, int inst, int variant) {
+  return build_tables<tsb_pfsp_tables50, TSB_MAX_JOBS_WIDE>(t, inst, variant);
+}
+int tsb_pfsp_create50_from_tables(tsb_pfsp** h, int device, int M_max, const tsb_pfsp_tables50* t) {
+  if (!t) return TSB_EINVAL;
+  return tsb_pfsp_create_wide(h, device, TSB_MAX_JOBS_WIDE, t->jobs, t->machines, M_max, t->p_times, t->min_heads,
+                              t->min_tails, t->pairs, t->johnson, t->lags, t->mp0, t->mp1, t->mp_order);
+}
+
+int tsb_pfsp_create_from_tables(tsb_pfsp** h, int device, int M_max, const tsb_pfsp_tables* t) {
+  if (!t) return TSB_EINVAL;
+  return tsb_pfsp_create(h, device, t->jobs, t->machines, M_max, t->p_times, t->min_heads, t->min_tails,
+                         t->pairs, t->johnson, t->lags, t->mp0, t->mp1, t->mp_order);
+}
+
+void tsb_release_cached_handles(void) { nq_handle_cache().clear(); }
+
+// step 1 of the drivers alone (nqueens_gpu_chpl.chpl:169-175): breadth-first from the root until the pool holds
+// min_size nodes; the pool, in order, and what was explored on the way
 int tsb_nq_warmup(int N, int min_size, void* nodes, int64_t capacity, int64_t* n, uint64_t* tree, uint64_t* sol) {
   if (N < 1 || N > TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
   return with_nq_node(N > TSB_MAX_QUEENS, [&](auto node) {
@@ -1222,54 +1014,63 @@ int tsb_nq_warmup(int N, int min_size, void* nodes, int64_t capacity, int64_t* n
   });
 }
 
+int tsb_nq_search(int N, int g, int m, int M, int D, tsb_search_stats* out) {
+  return with_nq_node(N > TSB_MAX_QUEENS, [&](auto node) {
+    return nq_search<decltype(node)>(N, g, m, M, D, false, -1, 0, nullptr, out);
+  });
+}
+int tsb_nq_search_wide(int max_queens, int N, int g, int m, int M, int D, tsb_search_stats* out) {
+  if (max_queens != TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
+  return nq_search<tsb_nq_node24>(N, g, m, M, D, false, -1, 0, nullptr, out);
+}
 int tsb_nq_search_device(int N, int g, int m, int M, int D, tsb_search_stats* out) {
   return with_nq_node(N > TSB_MAX_QUEENS, [&](auto node) {
-    return nq_search_device_impl<decltype(node)>(N, g, m, M, D, -1, 0, nullptr, out);
+    return nq_search<decltype(node)>(N, g, m, M, D, true, -1, 0, nullptr, out);
   });
 }
 int tsb_nq_search_device_wide(int max_queens, int N, int g, int m, int M, int D, tsb_search_stats* out) {
   if (max_queens != TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
-  return nq_search_device_impl<tsb_nq_node24>(N, g, m, M, D, -1, 0, nullptr, out);
+  return nq_search<tsb_nq_node24>(N, g, m, M, D, true, -1, 0, nullptr, out);
 }
 int tsb_nq_search_device_part(int N, int g, int m, int M, int D, int part, int device, tsb_search_stats* out) {
   if (part < 0) return TSB_EINVAL;
   return with_nq_node(N > TSB_MAX_QUEENS, [&](auto node) {
-    return nq_search_device_impl<decltype(node)>(N, g, m, M, D, part, device, nullptr, out);
+    return nq_search<decltype(node)>(N, g, m, M, D, true, part, device, nullptr, out);
   });
 }
 int tsb_nq_search_on(tsb_nq* h, int N, int m, int M, tsb_search_stats* out) {
   if (!h) return TSB_EINVAL;
   return with_nq_node(tsb_nq_max_queens(h) == TSB_MAX_QUEENS_WIDE, [&](auto node) {
-    return nq_search_device_impl<decltype(node)>(N, 1, m, M, 1, -1, 0, h, out);
+    return nq_search<decltype(node)>(N, 1, m, M, 1, true, -1, 0, h, out);
   });
 }
 int tsb_pfsp_search(int inst, int lb_kind, int ub, int m, int M, int D, tsb_search_stats* out) {
-  return pfsp_search_impl(inst, lb_kind, ub, m, M, D, false, -1, 0, nullptr, out);
+  return pfsp_search(inst, lb_kind, ub, m, M, D, false, -1, 0, nullptr, out);
 }
 int tsb_pfsp_search_device(int inst, int lb_kind, int ub, int m, int M, int D, tsb_search_stats* out) {
-  return pfsp_search_impl(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out);
+  return pfsp_search(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out);
 }
 int tsb_pfsp_search_device_part(int inst, int lb_kind, int ub, int m, int M, int D, int part, int device,
                                 tsb_search_stats* out) {
   if (part < 0) return TSB_EINVAL;
-  return pfsp_search_impl(inst, lb_kind, ub, m, M, D, true, part, device, nullptr, out);
+  return pfsp_search(inst, lb_kind, ub, m, M, D, true, part, device, nullptr, out);
 }
 int tsb_pfsp_search_on(tsb_pfsp* h, int inst, int lb_kind, int ub, int m, int M, tsb_search_stats* out) {
   if (!h) return TSB_EINVAL;
-  return pfsp_search_impl(inst, lb_kind, ub, m, M, 1, true, -1, 0, h, out);
+  return pfsp_search(inst, lb_kind, ub, m, M, 1, true, -1, 0, h, out);
 }
 int tsb_pfsp_search_device_pools(int inst, int lb_kind, int ub, int m, int M, int D, int pools, tsb_search_stats* out) {
-  return pfsp_search_impl(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out, pools);
+  return pfsp_search(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out, pools);
 }
 int tsb_pfsp_search_device_pools_part(int inst, int lb_kind, int ub, int m, int M, int D, int pools, int part,
                                       int device, tsb_search_stats* out) {
   if (part < 0) return TSB_EINVAL;
-  return pfsp_search_impl(inst, lb_kind, ub, m, M, D, true, part, device, nullptr, out, pools);
+  return pfsp_search(inst, lb_kind, ub, m, M, D, true, part, device, nullptr, out, pools);
 }
 int tsb_pfsp_search_on_pools(tsb_pfsp* h, int inst, int lb_kind, int ub, int m, int M, int pools,
                              tsb_search_stats* out) {
   if (!h) return TSB_EINVAL;
-  return pfsp_search_impl(inst, lb_kind, ub, m, M, 1, true, -1, 0, h, out, pools);
+  return pfsp_search(inst, lb_kind, ub, m, M, 1, true, -1, 0, h, out, pools);
 }
 
 }  // extern "C"
