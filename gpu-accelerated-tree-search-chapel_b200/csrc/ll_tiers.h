@@ -22,7 +22,8 @@ constexpr long long ll_pool_capacity(int sms, int pools) {
 // pools per launch the drivers use for chunks of up to M parents: 4, 3, 2 (up to the one-pool capacity), or 1
 // (beyond it: two-kernel rounds).  On an H100 (132 SMs): 4 up to 50 688, 3 up to 67 584, then 1.
 // (tsb_nq_pools_per_launch answers a different question, the most pools one launch can take: 4, 3, 2 up to
-// ll_pool_capacity(sms, 2) = 101 376 on an H100, then 1.  The drivers cap it by this function and TSB200_POOLS, so
+// ll_pool_capacity(sms, 2) = 101 376 on an H100, then 1.  Above the one-pool capacity, a pool that such a launch
+// leaves running alone finishes in two-kernel rounds.  The drivers cap it by this function and TSB200_POOLS, so
 // beyond the one-pool capacity they run one pool in two-kernel rounds.)
 constexpr int ll_pools_for(int sms, long long M) {
   return M <= ll_pool_capacity(sms, 4) ? 4 : M <= ll_pool_capacity(sms, 3) ? 3 : M <= ll_pool_capacity(sms, 1) ? 2 : 1;

@@ -15,7 +15,8 @@ constexpr int pf_ctas_per_pool(int sms, int pools) {
   return most < PFR_MAX_CTAS ? most : PFR_MAX_CTAS;
 }
 // largest chunk (parents) of each pool.  On a 132-SM H100: one pool or two: 50 688 (covers the reference's default
-// --M 50000), three: 33 792, four: 25 344
+// --M 50000), three: 33 792, four: 25 344.  One pool alone takes the kernel only up to PFR_MAX_M as well, so above
+// it a pool that a shared launch leaves running alone finishes in two-kernel rounds.
 constexpr long long pf_pool_capacity(int sms, int pools) {
   return static_cast<long long>(pf_ctas_per_pool(sms, pools)) * PFR_SLICE;
 }

@@ -752,6 +752,126 @@ int step_loop(int64_t max_rounds, uint64_t* out, Step&& step) {
   return TSB_OK;
 }
 
+// ---- the persistent kernel's host loop, over a problem type R (NqRounds, PfspRounds) that supplies the handle, sync
+// and parameter types and: grid(h0, M, pools, &variant) (CTAs per pool, 0: the launch does not take M);
+// prepare(h, i, left, need, &prm, &queued) (pool i's arena ready for a next round of up to `need` nodes, prm's own
+// fields; queued: work on h's stream the launch must follow); launch(h0, params, grid, pools, variant) on h0's stream;
+// resume(h, i, st, m, M, &left, out, &again) (what pool i does after its exit code); step (one two-kernel round of
+// pool i); report (the TSB200_ROUNDS_PROF lines of a launch); of_pool(i) (pool i's problem on its own).
+
+// Up to max_rounds rounds of EACH of the K pools hs[0..K) (handles on one device) in launches of R's persistent kernel
+// that serve every pool that still has work: grid (G, pools).  out[4 i ..] += {rounds, parents, children, solutions}
+// of pool i.  A pool leaves a launch on its own: when it holds fewer than m nodes, after its round budget, when its
+// next round's worst case does not fit its arena (it grows and goes again), or for a reason of R's (R::resume).  The
+// launch ends when every pool has left; the grid follows the number of pools that still run.
+template <class R>
+int rounds_run(const R& r, typename R::Handle* const* hs, int K, int m, int M, int64_t max_rounds, uint64_t* out) {
+  int64_t left[R::kMaxPools];
+  bool active[R::kMaxPools];
+  for (int i = 0; i < K; i++) {
+    left[i] = max_rounds;
+    active[i] = true;
+  }
+  const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
+  for (;;) {
+    int map[R::kMaxPools], n_act = 0;
+    for (int i = 0; i < K; i++) {
+      active[i] = active[i] && hs[i]->pool.size >= m && left[i] > 0;
+      if (active[i]) map[n_act++] = i;
+    }
+    if (n_act == 0) return TSB_OK;
+    typename R::Handle* h0 = hs[map[0]];
+    int variant = 0;
+    const int grid = r.grid(h0, M, n_act, &variant);
+    if (grid == 0) {
+      // A launch that takes K >= 2 pools takes any 2..K of them (the callers check K), but one pool alone may not be
+      // taken at the same M: the one-pool kernel has a smaller capacity (ll_tiers.h) or a lower limit (PFR_MAX_M).
+      // The last pool then finishes in two-kernel rounds, as pool_run runs it.
+      if (n_act > 1) return TSB_EINVAL;
+      const int i = map[0];
+      return step_loop(left[i], &out[4 * i], [&](int64_t* np, uint64_t* nc, uint64_t* ns) {
+        return r.step(h0, i, m, M, np, nc, ns);
+      });
+    }
+    typename R::Params mp;
+    std::memset(&mp, 0, sizeof(mp));
+    long long need[R::kMaxPools];
+    for (int a = 0; a < n_act; a++) {
+      const int i = map[a];
+      typename R::Handle* h = hs[i];
+      const long long n = std::min<long long>(h->pool.size, M);
+      need[a] = h->pool.size - n + n * h->pool.fanout;  // the worst case of the next round
+      bool queued = !h->rounds.d_sync;  // (a new handle's flags are cleared on its stream)
+      int rc = h->rounds.template ensure<typename R::Sync>(h->stream);
+      if (rc == TSB_OK) rc = r.prepare(h, i, left[i], need[a], &mp.pool[a], &queued);
+      if (rc != TSB_OK) return rc;
+      if (queued && a > 0) TSB_CUDA(cudaStreamSynchronize(h->stream));  // (the launch goes on the first pool's stream)
+      auto& prm = mp.pool[a];
+      prm.size0 = h->pool.size;
+      prm.epoch0 = h->rounds.epoch;
+      prm.m = m;
+      prm.M = M;
+      prm.max_rounds = left[i];
+      prm.prof = prof;
+      prm.sync = h->rounds.template sync<typename R::Sync>();
+      prm.state = h->rounds.d_state;
+      h->rounds.h_state->exit_code = -1;
+    }
+    int rc = r.launch(h0, mp, grid, n_act, variant);
+    if (rc != TSB_OK) return rc;
+    TSB_CUDA(cudaStreamSynchronize(h0->stream));
+    tsb::RoundsState st[R::kMaxPools];
+    for (int a = 0; a < n_act; a++) {
+      const int i = map[a];
+      typename R::Handle* h = hs[i];
+      rc = h->finish_launch(R::kKernel, R::kStuck, &st[a], &out[4 * i]);
+      if (rc != TSB_OK) return rc;
+      left[i] -= static_cast<int64_t>(st[a].rounds);
+      if (st[a].exit_code == tsb::RND_EXIT_SPACE && st[a].rounds == 0 && need[a] <= h->pool.cap)
+        return TSB_ENOMEM;  // (cannot happen: the arena was grown for `need`)
+      rc = r.resume(h, i, st[a], m, M, &left[i], &out[4 * i], &active[i]);
+      if (rc != TSB_OK) return rc;
+    }
+    if (prof) r.report(st, map, n_act, grid);
+  }
+}
+
+// one pool: the persistent kernel when it takes M, else two-kernel rounds
+template <class R>
+int pool_run(const R& r, typename R::Handle* h, int m, int M, int64_t max_rounds, uint64_t* n_rounds,
+             uint64_t* n_parents, uint64_t* n_children, uint64_t* n_solutions) {
+  *n_rounds = *n_parents = *n_children = *n_solutions = 0;
+  TSB_CUDA(cudaSetDevice(h->device));
+  uint64_t out[4] = {0, 0, 0, 0};
+  const int rc = rounds_run(r, &h, 1, m, M, max_rounds, out);
+  *n_rounds = out[0];
+  *n_parents = out[1];
+  *n_children = out[2];
+  *n_solutions = out[3];
+  return rc;
+}
+
+// K pools in shared launches, or one pool after the other when one launch does not take K pools at this M
+template <class R>
+int pool_run_multi(const R& r, typename R::Handle* const* hs, int K, int m, int M, int64_t max_rounds, uint64_t* out) {
+  std::memset(out, 0, sizeof(uint64_t) * 4 * K);
+  TSB_CUDA(cudaSetDevice(hs[0]->device));
+  if (r.grid(hs[0], M, K, nullptr) > 0) return rounds_run(r, hs, K, m, M, max_rounds, out);
+  for (int i = 0; i < K; i++) {
+    const int rc = rounds_run(r.of_pool(i), &hs[i], 1, m, M, max_rounds, &out[4 * i]);
+    if (rc != TSB_OK) return rc;
+  }
+  return TSB_OK;
+}
+
+// the most pools one launch takes with chunks of up to M parents (1: not several)
+template <class R, class H>
+int pools_per_launch(const R& r, H* h, int M) {
+  for (int pools = R::kMaxPools; pools > 1; pools--)
+    if (r.grid(h, M, pools, nullptr) > 0) return pools;
+  return 1;
+}
+
 // expand of host arrays: the parents through d_in, the children through d_children (room for M_max parents' worst
 // case)
 template <class Expand>
@@ -1071,164 +1191,121 @@ int nq_ll_grid(const tsb_nq* h, int M, int pools, int* ppt = nullptr) {
   if (ppt) *ppt = per;
   return static_cast<long long>(M) <= static_cast<long long>(grid) * slice && (pools > 1 || per == 2) ? grid : 0;
 }
-// Up to `max_rounds` rounds of EACH of the K pools (handles on one device, same N) in launches of the persistent
-// kernel that serve all pools that still have work: grid (grid, pools).  out[4 i ..] += {rounds, parents, children,
-// solutions} of pool i.  A pool leaves the launch on its own (done, round budget, arena full, layer table full); the
-// launch ends when every pool has left, the pools that stopped for room grow and go again.
-int nq_ll_run_multi(tsb_nq* const* hs, int K, int m, int M, int64_t max_rounds, uint64_t* out) {
-  int64_t left[tsb::LL_MAX_POOLS];
-  bool active[tsb::LL_MAX_POOLS];
-  for (int i = 0; i < K; i++) {
-    left[i] = max_rounds;
-    active[i] = true;
-    int rc = hs[i]->rounds.ensure<tsb::LlSync>(hs[i]->stream);
+// The N-Queens side of rounds_run: launches of nq_rounds_ll_kernel on the pools' fat arenas
+struct NqRounds {
+  using Handle = tsb_nq;
+  using Sync = tsb::LlSync;
+  using Params = tsb::LlMultiParams;
+  static constexpr int kMaxPools = tsb::LL_MAX_POOLS;
+  static constexpr const char* kKernel = "nq_rounds_ll_kernel";
+  static constexpr const char* kStuck = "a flag exchange or a node poll did not complete";
+
+  // (*ppt: the variant's parents per thread; a lone survivor gets the one-pool kernel)
+  int grid(const tsb_nq* h0, int M, int pools, int* ppt) const { return nq_ll_grid(h0, M, pools, ppt); }
+  int prepare(tsb_nq* h, int, int64_t left, long long need, tsb::LlParams* prm, bool* queued) const {
+    DevicePool& p = h->pool;
+    int rc = TSB_OK;
+    if (h->in_fat && need > p.cap) rc = nq_materialize(h);  // (grows below and imports again)
     if (rc != TSB_OK) return rc;
+    if (!h->in_fat) {
+      // room for the worst case of the next round
+      rc = p.make_stack(h->stream, need);
+      if (rc == TSB_OK) rc = nq_ensure_fat(h, p.cap);
+      if (rc == TSB_OK) rc = with_queens(h->N, [h](auto q) { return nq_fat_import<decltype(q)::value>(h); });
+      if (rc != TSB_OK) return rc;
+      h->in_fat = true;
+      *queued = true;
+    }
+    prm->fat = h->d_fat;
+    prm->cap = std::min(p.cap, h->fat_cap);
+    return nq_fat_tag_window(h, left, &prm->epoch_last, queued);
   }
-  const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
-  std::vector<tsb::RoundsState> pace(prof ? tsb::LL_MAX_POOLS : 0);  // (each pool's record of the last launch)
-  for (;;) {
-    tsb::LlMultiParams mp;
-    std::memset(&mp, 0, sizeof(mp));
-    int map[tsb::LL_MAX_POOLS], n_act = 0;
-    long long need_of[tsb::LL_MAX_POOLS];
-    for (int i = 0; i < K; i++) {
-      tsb_nq* h = hs[i];
-      DevicePool& p = h->pool;
-      if (!active[i] || p.size < m || left[i] <= 0) {
-        active[i] = false;
-        continue;
-      }
-      const long long n = std::min<long long>(p.size, M);
-      const long long need = p.size - n + n * h->N;
-      int rc = TSB_OK;
-      if (h->in_fat && need > p.cap) rc = nq_materialize(h);  // (grows below and imports again)
-      if (rc != TSB_OK) return rc;
-      bool queued = false;  // work on h's stream that the launch must follow
-      if (!h->in_fat) {
-        // room for the worst case of the next round
-        rc = p.make_stack(h->stream, need);
-        if (rc == TSB_OK) rc = nq_ensure_fat(h, p.cap);
-        if (rc == TSB_OK) rc = with_queens(h->N, [h](auto q) { return nq_fat_import<decltype(q)::value>(h); });
-        if (rc != TSB_OK) return rc;
-        h->in_fat = true;
-        queued = true;
-      }
-      tsb::LlParams& prm = mp.pool[n_act];
-      rc = nq_fat_tag_window(h, left[i], &prm.epoch_last, &queued);
-      if (rc != TSB_OK) return rc;
-      if (queued && n_act > 0) TSB_CUDA(cudaStreamSynchronize(h->stream));  // (the launch goes on the first pool's stream)
-      prm.fat = h->d_fat;
-      prm.cap = std::min(p.cap, h->fat_cap);
-      prm.size0 = p.size;
-      prm.epoch0 = h->rounds.epoch;
-      prm.m = m;
-      prm.M = M;
-      prm.max_rounds = left[i];
-      prm.prof = prof;
-      prm.sync = h->rounds.sync<tsb::LlSync>();
-      prm.state = h->rounds.d_state;
-      h->rounds.h_state->exit_code = -1;
-      need_of[n_act] = need;
-      map[n_act++] = i;
-    }
-    if (n_act == 0) break;
-    tsb_nq* h0 = hs[map[0]];
-    // (variant and grid follow the number of pools that still run: a lone survivor gets the one-pool kernel)
-    int ppt = 2;
-    const int grid = nq_ll_grid(h0, M, n_act, &ppt);
-    if (grid == 0) return TSB_EINVAL;  // (checked by the callers for K pools, and fewer pools fit a fortiori)
-    int rc = with_queens(h0->N, [&](auto q) {
-      return nq_ll_launch_n<decltype(q)::value>(h0, mp, grid, n_act, ppt, h0->stream);
-    });
-    if (rc != TSB_OK) return rc;
-    TSB_CUDA(cudaStreamSynchronize(h0->stream));
-    for (int a = 0; a < n_act; a++) {
-      const int i = map[a];
-      tsb_nq* h = hs[i];
-      tsb::RoundsState st;
-      rc = h->finish_launch("nq_rounds_ll_kernel", "a flag exchange or a node poll did not complete", &st, &out[4 * i]);
-      if (rc != TSB_OK) return rc;
-      h->tag_hi = std::max(h->tag_hi, st.size_hi);
-      if (prof) {
-        const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
-        std::fprintf(stderr, "[tsb200] LL rounds kernel (pool %d of %d): %llu rounds; CTA 0 cycles per round: workers: set-up %.0f "
-                     "poll-nodes %.0f scan+items %.0f build %.0f handoff-wait %.0f store %.0f | exchange warp: "
-                     "scan-wait %.0f publish+plan-ahead %.0f gather-wait %.0f sums+plan %.0f handoff-wait %.0f\n", a, n_act,
-                     static_cast<unsigned long long>(st.rounds), st.prof[tsb::LL_PROF_SETUP] / r, st.prof[tsb::LL_PROF_POLL] / r,
-                     st.prof[tsb::LL_PROF_SCAN] / r, st.prof[tsb::LL_PROF_BUILD] / r, st.prof[tsb::LL_PROF_HAND] / r,
-                     st.prof[tsb::LL_PROF_STORE] / r, st.prof[tsb::LL_PROF_X_SCAN] / r, st.prof[tsb::LL_PROF_X_AHEAD] / r,
-                     st.prof[tsb::LL_PROF_X_GATHER] / r, st.prof[tsb::LL_PROF_X_TAIL] / r, st.prof[tsb::LL_PROF_X_HAND] / r);
-        pace[a] = st;
-      }
-      left[i] -= static_cast<int64_t>(st.rounds);
-      if (st.exit_code == tsb::RND_EXIT_SPACE) {
-        if (st.rounds == 0 && need_of[a] <= h->pool.cap) return TSB_ENOMEM;  // (cannot happen)
-        rc = nq_materialize(h);  // back to the plain arena, which then grows
-        if (rc != TSB_OK) return rc;
-      } else if (st.exit_code != tsb::RND_EXIT_RELAUNCH) {  // (layer table full: a fresh launch trusts the whole pool)
-        active[i] = false;                                    // DONE or PAUSE
-      }
-    }
-    if (prof) {
-      // the pace of the launch: it ends when its last pool leaves, so a pool that leaves early idles its CTAs' SMs
-      // share for the rest of it
-      unsigned long long t0 = ~0ull, t1 = 0;
-      for (int a = 0; a < n_act; a++) {
-        t0 = std::min(t0, pace[a].t_start);
-        t1 = std::max(t1, pace[a].t_exit);
-      }
-      for (int a = 0; a < n_act; a++) {
-        const tsb::RoundsState& st = pace[a];
-        const double wall = 1e-3 * static_cast<double>(st.t_exit - st.t_start);
-        unsigned long long fertile = 0, wide = 0;  // (over the pool's CTAs)
-        for (int c = 0; c < grid; c++) {
-          fertile += st.cta_fertile[c];
-          wide += st.cta_wide[c];
-        }
-        // why the pool left: its round budget, fewer than m nodes, a relaunch (layer table or tag window), arena room
-        static const char* const why[] = {"dry", "budget", "space", "abort", "relaunch"};
-        std::fprintf(stderr, "[tsb200] LL pace (pool %d of %d, handle %d): start +%.2f us, wall %.2f us, %llu rounds, "
-                     "%.4f us per round, stagger %.2f us, parents %llu, children %llu, parents with children %llu, "
-                     "CTA rounds over one window %llu, exit %s, globaltimer %llu..%llu ns\n", a, n_act, map[a],
-                     1e-3 * static_cast<double>(st.t_start - t0), wall, static_cast<unsigned long long>(st.rounds),
-                     wall / static_cast<double>(std::max<unsigned long long>(1, st.rounds)),
-                     1e-3 * static_cast<double>(t1 - st.t_exit), static_cast<unsigned long long>(st.parents),
-                     static_cast<unsigned long long>(st.children), fertile, wide,
-                     st.exit_code >= 0 && st.exit_code <= tsb::RND_EXIT_RELAUNCH ? why[st.exit_code] : "?", st.t_start,
-                     st.t_exit);
-      }
-      // residency: which pools' CTAs share an SM, and which of them started there first
-      int row_of[2][tsb::LL_MAX_SMS * 2], n_on[tsb::LL_MAX_SMS * 2] = {};
-      unsigned t_of[2][tsb::LL_MAX_SMS * 2];
-      for (int a = 0; a < n_act; a++)
-        for (int c = 0; c < grid; c++) {
-          const unsigned s = pace[a].cta_sm[c] % (tsb::LL_MAX_SMS * 2);
-          if (n_on[s] < 2) {
-            row_of[n_on[s]][s] = a;
-            t_of[n_on[s]][s] = pace[a].cta_t0[c];
-          }
-          n_on[s]++;
-        }
-      int pairs[tsb::LL_MAX_POOLS][tsb::LL_MAX_POOLS] = {}, first[tsb::LL_MAX_POOLS] = {}, over = 0;
-      for (int s = 0; s < tsb::LL_MAX_SMS * 2; s++) {
-        if (n_on[s] > 2) over++;
-        if (n_on[s] < 2) continue;
-        const bool zero_first = static_cast<int>(t_of[1][s] - t_of[0][s]) >= 0;
-        const int lo = std::min(row_of[0][s], row_of[1][s]), hi = std::max(row_of[0][s], row_of[1][s]);
-        pairs[lo][hi]++;
-        first[zero_first ? row_of[0][s] : row_of[1][s]]++;
-      }
-      std::string sh;
-      for (int x = 0; x < n_act; x++)
-        for (int y = x; y < n_act; y++)
-          if (pairs[x][y]) sh += " " + std::to_string(x) + "+" + std::to_string(y) + ": " + std::to_string(pairs[x][y]);
-      std::string fs;
-      for (int x = 0; x < n_act; x++) fs += " " + std::to_string(x) + ": " + std::to_string(first[x]);
-      std::fprintf(stderr, "[tsb200] LL residency: SMs shared by pools%s | started first on a shared SM, by pool%s | SMs "
-                   "with more than two CTAs: %d\n", sh.c_str(), fs.c_str(), over);
-    }
+  int launch(tsb_nq* h0, const tsb::LlMultiParams& mp, int grid, int pools, int ppt) const {
+    return with_queens(h0->N, [&](auto q) { return nq_ll_launch_n<decltype(q)::value>(h0, mp, grid, pools, ppt, h0->stream); });
   }
-  return TSB_OK;
+  // SPACE: back to the plain arena, which grows before the next launch; RELAUNCH (layer table full, or the tag window
+  // used up): a fresh launch trusts the whole pool; DONE or PAUSE: the pool leaves
+  int resume(tsb_nq* h, int, const tsb::RoundsState& st, int, int, int64_t*, uint64_t*, bool* again) const {
+    h->tag_hi = std::max(h->tag_hi, st.size_hi);
+    *again = st.exit_code == tsb::RND_EXIT_SPACE || st.exit_code == tsb::RND_EXIT_RELAUNCH;
+    return st.exit_code == tsb::RND_EXIT_SPACE ? nq_materialize(h) : TSB_OK;
+  }
+  int step(tsb_nq* h, int, int m, int M, int64_t* np, uint64_t* nc, uint64_t* ns) const {
+    return tsb_nq_pool_step(h, m, M, np, nc, ns);
+  }
+  void report(const tsb::RoundsState* pace, const int* map, int n_act, int grid) const;
+  NqRounds of_pool(int) const { return *this; }
+};
+
+// TSB200_ROUNDS_PROF: CTA 0's phases of each pool, the pace of the launch and which pools shared an SM
+void NqRounds::report(const tsb::RoundsState* pace, const int* map, int n_act, int grid) const {
+  for (int a = 0; a < n_act; a++) {
+    const tsb::RoundsState& st = pace[a];
+    const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
+    std::fprintf(stderr, "[tsb200] LL rounds kernel (pool %d of %d): %llu rounds; CTA 0 cycles per round: workers: set-up %.0f "
+                 "poll-nodes %.0f scan+items %.0f build %.0f handoff-wait %.0f store %.0f | exchange warp: "
+                 "scan-wait %.0f publish+plan-ahead %.0f gather-wait %.0f sums+plan %.0f handoff-wait %.0f\n", a, n_act,
+                 static_cast<unsigned long long>(st.rounds), st.prof[tsb::LL_PROF_SETUP] / r, st.prof[tsb::LL_PROF_POLL] / r,
+                 st.prof[tsb::LL_PROF_SCAN] / r, st.prof[tsb::LL_PROF_BUILD] / r, st.prof[tsb::LL_PROF_HAND] / r,
+                 st.prof[tsb::LL_PROF_STORE] / r, st.prof[tsb::LL_PROF_X_SCAN] / r, st.prof[tsb::LL_PROF_X_AHEAD] / r,
+                 st.prof[tsb::LL_PROF_X_GATHER] / r, st.prof[tsb::LL_PROF_X_TAIL] / r, st.prof[tsb::LL_PROF_X_HAND] / r);
+  }
+  // the pace of the launch: it ends when its last pool leaves, so a pool that leaves early idles its CTAs' SMs
+  // share for the rest of it
+  unsigned long long t0 = ~0ull, t1 = 0;
+  for (int a = 0; a < n_act; a++) {
+    t0 = std::min(t0, pace[a].t_start);
+    t1 = std::max(t1, pace[a].t_exit);
+  }
+  for (int a = 0; a < n_act; a++) {
+    const tsb::RoundsState& st = pace[a];
+    const double wall = 1e-3 * static_cast<double>(st.t_exit - st.t_start);
+    unsigned long long fertile = 0, wide = 0;  // (over the pool's CTAs)
+    for (int c = 0; c < grid; c++) {
+      fertile += st.cta_fertile[c];
+      wide += st.cta_wide[c];
+    }
+    // why the pool left: its round budget, fewer than m nodes, a relaunch (layer table or tag window), arena room
+    static const char* const why[] = {"dry", "budget", "space", "abort", "relaunch"};
+    std::fprintf(stderr, "[tsb200] LL pace (pool %d of %d, handle %d): start +%.2f us, wall %.2f us, %llu rounds, "
+                 "%.4f us per round, stagger %.2f us, parents %llu, children %llu, parents with children %llu, "
+                 "CTA rounds over one window %llu, exit %s, globaltimer %llu..%llu ns\n", a, n_act, map[a],
+                 1e-3 * static_cast<double>(st.t_start - t0), wall, static_cast<unsigned long long>(st.rounds),
+                 wall / static_cast<double>(std::max<unsigned long long>(1, st.rounds)),
+                 1e-3 * static_cast<double>(t1 - st.t_exit), static_cast<unsigned long long>(st.parents),
+                 static_cast<unsigned long long>(st.children), fertile, wide,
+                 st.exit_code >= 0 && st.exit_code <= tsb::RND_EXIT_RELAUNCH ? why[st.exit_code] : "?", st.t_start,
+                 st.t_exit);
+  }
+  // residency: which pools' CTAs share an SM, and which of them started there first
+  int row_of[2][tsb::LL_MAX_SMS * 2], n_on[tsb::LL_MAX_SMS * 2] = {};
+  unsigned t_of[2][tsb::LL_MAX_SMS * 2];
+  for (int a = 0; a < n_act; a++)
+    for (int c = 0; c < grid; c++) {
+      const unsigned s = pace[a].cta_sm[c] % (tsb::LL_MAX_SMS * 2);
+      if (n_on[s] < 2) {
+        row_of[n_on[s]][s] = a;
+        t_of[n_on[s]][s] = pace[a].cta_t0[c];
+      }
+      n_on[s]++;
+    }
+  int pairs[tsb::LL_MAX_POOLS][tsb::LL_MAX_POOLS] = {}, first[tsb::LL_MAX_POOLS] = {}, over = 0;
+  for (int s = 0; s < tsb::LL_MAX_SMS * 2; s++) {
+    if (n_on[s] > 2) over++;
+    if (n_on[s] < 2) continue;
+    const bool zero_first = static_cast<int>(t_of[1][s] - t_of[0][s]) >= 0;
+    const int lo = std::min(row_of[0][s], row_of[1][s]), hi = std::max(row_of[0][s], row_of[1][s]);
+    pairs[lo][hi]++;
+    first[zero_first ? row_of[0][s] : row_of[1][s]]++;
+  }
+  std::string sh;
+  for (int x = 0; x < n_act; x++)
+    for (int y = x; y < n_act; y++)
+      if (pairs[x][y]) sh += " " + std::to_string(x) + "+" + std::to_string(y) + ": " + std::to_string(pairs[x][y]);
+  std::string fs;
+  for (int x = 0; x < n_act; x++) fs += " " + std::to_string(x) + ": " + std::to_string(first[x]);
+  std::fprintf(stderr, "[tsb200] LL residency: SMs shared by pools%s | started first on a shared SM, by pool%s | SMs "
+               "with more than two CTAs: %d\n", sh.c_str(), fs.c_str(), over);
 }
 
 // ============================================================================ PFSP
@@ -1475,114 +1552,60 @@ int pfsp_rounds_launch(tsb_pfsp* h, int lb_kind, const tsb::PfRoundsMultiParams&
     return TSB_OK;
   });
 }
-// Up to max_rounds rounds of EACH of the K pools (handles on one device, same route) in launches of the persistent
-// kernel that serve every pool that still has work: grid (G, pools).  out[4 i ..] += {rounds, parents, children,
-// solutions} of pool i, best[i] is pool i's incumbent.  A pool leaves a launch on its own: when it holds fewer than m
-// nodes, after its round budget, when its next round's worst case does not fit its arena (it grows and the pool goes
-// again) or when a leaf of its chunk improves best[i] (that round goes through tsb_pfsp_pool_step and its sequential
-// rule, then the pool goes again with the new incumbent).  The launch ends when every pool has left.  A pool that is
-// the only one left runs exactly as tsb_pfsp_pool_run runs it (pfsp_rounds_grid, or the loop of pool_step).
-int pfsp_rounds_run(tsb_pfsp* const* hs, int K, int lb_kind, int m, int M, int64_t max_rounds, int64_t* best, uint64_t* out) {
-  int64_t left[tsb::PFR_MAX_POOLS];
-  bool active[tsb::PFR_MAX_POOLS];
-  for (int i = 0; i < K; i++) {
-    left[i] = max_rounds;
-    active[i] = true;
-    int rc = hs[i]->rounds.ensure<tsb::PfRoundsSync>(hs[i]->stream);
-    if (rc != TSB_OK) return rc;
+// The PFSP side of rounds_run: launches of pfsp_rounds_kernel on the pools' plain arenas; best[i] is pool i's
+// incumbent
+struct PfspRounds {
+  using Handle = tsb_pfsp;
+  using Sync = tsb::PfRoundsSync;
+  using Params = tsb::PfRoundsMultiParams;
+  static constexpr int kMaxPools = tsb::PFR_MAX_POOLS;
+  static constexpr const char* kKernel = "pfsp_rounds_kernel";
+  static constexpr const char* kStuck = "a count or store exchange did not complete";
+  int lb_kind;
+  int64_t* best;
+
+  int grid(tsb_pfsp* h0, int M, int pools, int*) const {
+    return pools == 1 ? pfsp_rounds_grid(h0, lb_kind, M) : pfsp_multi_grid(h0, lb_kind, M, pools);
   }
-  const bool prof = std::getenv("TSB200_ROUNDS_PROF") != nullptr;
-  for (;;) {
-    tsb::PfRoundsMultiParams mp;
-    std::memset(&mp, 0, sizeof(mp));
-    int map[tsb::PFR_MAX_POOLS], n_act = 0;
-    long long need_of[tsb::PFR_MAX_POOLS];
-    for (int i = 0; i < K; i++) {
-      tsb_pfsp* h = hs[i];
-      DevicePool& p = h->pool;
-      if (!active[i] || p.size < m || left[i] <= 0) {
-        active[i] = false;
-        continue;
-      }
-      // room for the worst case of the next round
-      const long long n = std::min<long long>(p.size, M);
-      const long long need = p.size - n + n * h->jobs;
-      int rc = p.make_stack(h->stream, need);
-      if (rc != TSB_OK) return rc;
-      // (the launch goes on the first pool's stream: a pool_step round may still be storing on this one)
-      if (n_act > 0) TSB_CUDA(cudaStreamSynchronize(h->stream));
-      tsb::PfRoundsParams& prm = mp.pool[n_act];
-      prm.arena = p.arena[p.cur];
-      prm.tables = h->d_tab1;
-      prm.cap = p.cap;
-      prm.size0 = p.size;
-      prm.max_rounds = left[i];
-      prm.epoch0 = h->rounds.epoch;
-      prm.m = m;
-      prm.M = M;
-      prm.best = clamp_best(best[i]);
-      prm.prof = prof;
-      prm.sync = h->rounds.sync<tsb::PfRoundsSync>();
-      prm.state = h->rounds.d_state;
-      h->rounds.h_state->exit_code = -1;
-      need_of[n_act] = need;
-      map[n_act++] = i;
-    }
-    if (n_act == 0) break;
-    tsb_pfsp* h0 = hs[map[0]];
-    const int grid = n_act == 1 ? pfsp_rounds_grid(h0, lb_kind, M) : pfsp_multi_grid(h0, lb_kind, M, n_act);
-    if (grid == 0) {
-      if (n_act > 1) return TSB_EINVAL;  // (checked by the caller for K pools, and fewer pools fit a fortiori)
-      const int i = map[0];  // the last pool, at an M the persistent kernel leaves to two-kernel rounds
-      return step_loop(left[i], &out[4 * i], [&](int64_t* np, uint64_t* nc, uint64_t* ns) {
-        return tsb_pfsp_pool_step(h0, lb_kind, m, M, &best[i], np, nc, ns);
-      });
-    }
-    int rc = pfsp_rounds_launch(h0, lb_kind, mp, grid, n_act, h0->stream);
-    if (rc != TSB_OK) return rc;
-    TSB_CUDA(cudaStreamSynchronize(h0->stream));
+  int prepare(tsb_pfsp* h, int i, int64_t, long long need, tsb::PfRoundsParams* prm, bool* queued) const {
+    DevicePool& p = h->pool;
+    const int rc = p.make_stack(h->stream, need);  // room for the worst case of the next round
+    prm->arena = p.arena[p.cur];
+    prm->tables = h->d_tab1;
+    prm->cap = p.cap;
+    prm->best = clamp_best(best[i]);
+    *queued = true;  // (a pool_step round may still be storing on h's stream)
+    return rc;
+  }
+  int launch(tsb_pfsp* h0, const tsb::PfRoundsMultiParams& mp, int grid, int pools, int) const {
+    return pfsp_rounds_launch(h0, lb_kind, mp, grid, pools, h0->stream);
+  }
+  // SPACE: the arena grows before the next launch; IMPROVED: a leaf of the chunk improved best[i], so that round goes
+  // through tsb_pfsp_pool_step and its sequential rule and the pool goes again with the new incumbent; DONE or PAUSE:
+  // the pool leaves
+  int resume(tsb_pfsp* h, int i, const tsb::RoundsState& st, int m, int M, int64_t* left, uint64_t* out, bool* again) const {
+    *again = st.exit_code == tsb::RND_EXIT_SPACE || st.exit_code == tsb::PFR_EXIT_IMPROVED;
+    if (st.exit_code != tsb::PFR_EXIT_IMPROVED) return TSB_OK;
+    --*left;
+    return step_loop(1, out, [&](int64_t* np, uint64_t* nc, uint64_t* ns) { return step(h, i, m, M, np, nc, ns); });
+  }
+  int step(tsb_pfsp* h, int i, int m, int M, int64_t* np, uint64_t* nc, uint64_t* ns) const {
+    return tsb_pfsp_pool_step(h, lb_kind, m, M, &best[i], np, nc, ns);
+  }
+  // TSB200_ROUNDS_PROF: CTA 0's phases of each pool
+  void report(const tsb::RoundsState* pace, const int*, int n_act, int) const {
     for (int a = 0; a < n_act; a++) {
-      const int i = map[a];
-      tsb_pfsp* h = hs[i];
-      tsb::RoundsState st;
-      rc = h->finish_launch("pfsp_rounds_kernel", "a count or store exchange did not complete", &st, &out[4 * i]);
-      if (rc != TSB_OK) return rc;
-      if (prof) {
-        const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
-        std::fprintf(stderr, "[tsb200] PFSP rounds kernel (pool %d of %d): %llu rounds (exit %d); CTA 0 cycles per round: "
-                     "load %.0f bounds %.0f publish+items %.0f gather %.0f store %.0f store-exchange %.0f\n", a, n_act,
-                     static_cast<unsigned long long>(st.rounds), st.exit_code, st.prof[tsb::PFR_PROF_LOAD] / r,
-                     st.prof[tsb::PFR_PROF_BOUND] / r, st.prof[tsb::PFR_PROF_PUBLISH] / r, st.prof[tsb::PFR_PROF_GATHER] / r,
-                     st.prof[tsb::PFR_PROF_STORE] / r, st.prof[tsb::PFR_PROF_BARRIER] / r);
-      }
-      left[i] -= static_cast<int64_t>(st.rounds);
-      if (st.exit_code == tsb::RND_EXIT_SPACE) {
-        if (st.rounds == 0 && need_of[a] <= h->pool.cap) return TSB_ENOMEM;  // (cannot happen: the arena was grown for `need`)
-      } else if (st.exit_code == tsb::PFR_EXIT_IMPROVED) {
-        int64_t np = 0;
-        uint64_t nc = 0, ns = 0;
-        rc = tsb_pfsp_pool_step(h, lb_kind, m, M, &best[i], &np, &nc, &ns);
-        if (rc != TSB_OK) return rc;
-        out[4 * i] += 1;
-        out[4 * i + 1] += static_cast<uint64_t>(np);
-        out[4 * i + 2] += nc;
-        out[4 * i + 3] += ns;
-        --left[i];
-      } else {
-        active[i] = false;  // DONE or PAUSE
-      }
+      const tsb::RoundsState& st = pace[a];
+      const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
+      std::fprintf(stderr, "[tsb200] PFSP rounds kernel (pool %d of %d): %llu rounds (exit %d); CTA 0 cycles per round: "
+                   "load %.0f bounds %.0f publish+items %.0f gather %.0f store %.0f store-exchange %.0f\n", a, n_act,
+                   static_cast<unsigned long long>(st.rounds), st.exit_code, st.prof[tsb::PFR_PROF_LOAD] / r,
+                   st.prof[tsb::PFR_PROF_BOUND] / r, st.prof[tsb::PFR_PROF_PUBLISH] / r, st.prof[tsb::PFR_PROF_GATHER] / r,
+                   st.prof[tsb::PFR_PROF_STORE] / r, st.prof[tsb::PFR_PROF_BARRIER] / r);
     }
   }
-  return TSB_OK;
-}
-// tsb_pfsp_pool_run of one pool, out[] += {rounds, parents, children, solutions}
-int pfsp_pool_run_one(tsb_pfsp* h, int lb_kind, int m, int M, int64_t max_rounds, int64_t* best, uint64_t* out) {
-  if (pfsp_rounds_grid(h, lb_kind, M) > 0) return pfsp_rounds_run(&h, 1, lb_kind, m, M, max_rounds, best, out);
-  // lb2, large chunks: one round = two kernels (tsb_pfsp_pool_step)
-  return step_loop(max_rounds, out, [&](int64_t* np, uint64_t* nc, uint64_t* ns) {
-    return tsb_pfsp_pool_step(h, lb_kind, m, M, best, np, nc, ns);
-  });
-}
+  PfspRounds of_pool(int i) const { return {lb_kind, best + i}; }
+};
 
 // a handle with h's device, M_max and tables (its route included) and an empty pool; the device tables are copied
 // device to device, so none of the arrays h was created from is needed
@@ -1860,23 +1883,7 @@ int tsb_nq_pool_run(tsb_nq* h, int m, int M, int64_t max_rounds, uint64_t* n_rou
                     uint64_t* n_children, uint64_t* n_solutions) {
   if (!h || m < 1 || M < 1 || M > h->M_max || max_rounds < 0 || !n_rounds || !n_parents || !n_children || !n_solutions)
     return TSB_EINVAL;
-  *n_rounds = *n_parents = *n_children = *n_solutions = 0;
-  TSB_CUDA(cudaSetDevice(h->device));
-  uint64_t out[4] = {0, 0, 0, 0};
-  int rc;
-  if (nq_ll_grid(h, M, 1) > 0) {  // the whole loop in launches of the persistent kernel (nq_rounds_ll.cuh)
-    tsb_nq* one[1] = {h};
-    rc = nq_ll_run_multi(one, 1, m, M, max_rounds, out);
-  } else {  // large chunks: one round = two bandwidth-bound kernels (tsb_nq_pool_step)
-    rc = step_loop(max_rounds, out, [&](int64_t* np, uint64_t* nc, uint64_t* ns) {
-      return tsb_nq_pool_step(h, m, M, np, nc, ns);
-    });
-  }
-  *n_rounds = out[0];
-  *n_parents = out[1];
-  *n_children = out[2];
-  *n_solutions = out[3];
-  return rc;
+  return pool_run(NqRounds{}, h, m, M, max_rounds, n_rounds, n_parents, n_children, n_solutions);
 }
 
 int tsb_nq_sibling(tsb_nq* h, int index, tsb_nq** sibling) {
@@ -1891,9 +1898,7 @@ int tsb_nq_sibling(tsb_nq* h, int index, tsb_nq** sibling) {
 
 int tsb_nq_pools_per_launch(const tsb_nq* h, int M) {
   if (!h || M < 1 || M > h->M_max) return 1;
-  for (int pools = tsb::LL_MAX_POOLS; pools > 1; pools--)
-    if (nq_ll_grid(h, M, pools) > 0) return pools;
-  return 1;
+  return pools_per_launch(NqRounds{}, h, M);
 }
 
 int tsb_nq_pool_run_multi(tsb_nq* const* handles, int n_pools, int m, int M, int64_t max_rounds, uint64_t* out) {
@@ -1905,16 +1910,7 @@ int tsb_nq_pool_run_multi(tsb_nq* const* handles, int n_pools, int m, int M, int
     for (int j = 0; j < i; j++)
       if (handles[j] == h) return TSB_EINVAL;
   }
-  std::memset(out, 0, sizeof(uint64_t) * 4 * n_pools);
-  TSB_CUDA(cudaSetDevice(handles[0]->device));
-  if (nq_ll_grid(handles[0], M, n_pools) == 0) {  // chunks too large for the persistent kernel with this many pools: one pool after the other
-    for (int i = 0; i < n_pools; i++) {
-      int rc = tsb_nq_pool_run(handles[i], m, M, max_rounds, &out[4 * i], &out[4 * i + 1], &out[4 * i + 2], &out[4 * i + 3]);
-      if (rc != TSB_OK) return rc;
-    }
-    return TSB_OK;
-  }
-  return nq_ll_run_multi(handles, n_pools, m, M, max_rounds, out);
+  return pool_run_multi(NqRounds{}, handles, n_pools, m, M, max_rounds, out);
 }
 
 int tsb_nq_pool_steal(tsb_nq* victim, tsb_nq* thief, int m, int64_t* n_stolen) {
@@ -2334,15 +2330,7 @@ int tsb_pfsp_pool_run(tsb_pfsp* h, int lb_kind, int m, int M, int64_t max_rounds
       !n_parents || !n_children || !n_solutions)
     return TSB_EINVAL;
   if (lb_kind == TSB_LB2 && h->pairs == 0) return TSB_EINVAL;
-  *n_rounds = *n_parents = *n_children = *n_solutions = 0;
-  TSB_CUDA(cudaSetDevice(h->device));
-  uint64_t out[4] = {0, 0, 0, 0};
-  const int rc = pfsp_pool_run_one(h, lb_kind, m, M, max_rounds, best, out);
-  *n_rounds = out[0];
-  *n_parents = out[1];
-  *n_children = out[2];
-  *n_solutions = out[3];
-  return rc;
+  return pool_run(PfspRounds{lb_kind, best}, h, m, M, max_rounds, n_rounds, n_parents, n_children, n_solutions);
 }
 
 int tsb_pfsp_sibling(tsb_pfsp* h, int index, tsb_pfsp** sibling) {
@@ -2359,15 +2347,12 @@ int tsb_pfsp_sibling(tsb_pfsp* h, int index, tsb_pfsp** sibling) {
 
 int tsb_pfsp_pools_per_launch(const tsb_pfsp* h, int lb_kind, int M) {
   if (!h || h->wide || M < 1 || M > h->M_max) return 1;
-  // (const: what the occupancy query caches on the handle does not change what it computes)
-  tsb_pfsp* w = const_cast<tsb_pfsp*>(h);
   if (cudaSetDevice(h->device) != cudaSuccess) {
     (void)cudaGetLastError();
     return 1;
   }
-  for (int pools = tsb::PFR_MAX_POOLS; pools > 1; pools--)
-    if (pfsp_multi_grid(w, lb_kind, M, pools) > 0) return pools;
-  return 1;
+  // (const: what the occupancy query caches on the handle does not change what it computes)
+  return pools_per_launch(PfspRounds{lb_kind, nullptr}, const_cast<tsb_pfsp*>(h), M);
 }
 
 int tsb_pfsp_pool_run_multi(tsb_pfsp* const* handles, int n_pools, int lb_kind, int m, int M, int64_t max_rounds,
@@ -2387,16 +2372,7 @@ int tsb_pfsp_pool_run_multi(tsb_pfsp* const* handles, int n_pools, int lb_kind, 
       if (handles[j] == h) return TSB_EINVAL;
   }
   if (lb_kind == TSB_LB2 && h0->pairs == 0) return TSB_EINVAL;
-  std::memset(out, 0, sizeof(uint64_t) * 4 * n_pools);
-  TSB_CUDA(cudaSetDevice(h0->device));
-  if (n_pools == 1 || pfsp_multi_grid(handles[0], lb_kind, M, n_pools) == 0) {  // one pool after the other
-    for (int i = 0; i < n_pools; i++) {
-      int rc = pfsp_pool_run_one(handles[i], lb_kind, m, M, max_rounds, &best[i], &out[4 * i]);
-      if (rc != TSB_OK) return rc;
-    }
-    return TSB_OK;
-  }
-  return pfsp_rounds_run(handles, n_pools, lb_kind, m, M, max_rounds, best, out);
+  return pool_run_multi(PfspRounds{lb_kind, best}, handles, n_pools, m, M, max_rounds, out);
 }
 
 }  // extern "C"

@@ -342,7 +342,7 @@ def test_pool_run_multi(N, K, sms):
     starts, m, M, R = start_pools(N, K, 7600 + 10 * N + K)
     if K > 2:
         M = var2_M(sms, K)
-    # the launch takes the pools that hold at least m nodes (nq_ll_run_multi) and picks its variant by their number:
+    # the launch takes the pools that hold at least m nodes (rounds_run) and picks its variant by their number:
     # all K pools in the first launch (max_rounds = 1 below)
     assert sum(s.shape[0] >= m for s in starts) == K
     assert variant(sms, M, K) == (1 if K == 2 else 2)
@@ -359,6 +359,35 @@ def test_pool_run_multi(N, K, sms):
         assert all(o.size == 0 for o in oracles)
         if N >= 5:  # the pools left the shared launch at different rounds
             assert len({len(o.rounds) for o in oracles}) > 1
+
+
+@pytest.mark.parametrize("N", [12, 17])
+@pytest.mark.parametrize("case", ["below_m", "dry"])
+def test_pool_run_multi_lone_pool_above_the_one_pool_tier(N, case, sms):
+    """M = the one-pool capacity + 1: one launch takes two pools but not one.  A pool left running alone finishes its
+    calls in two-kernel rounds, as pool_run runs it: below_m: the other pool holds fewer than m nodes from the start;
+    dry: the other pool, a few deep nodes, shares the first call's launch and runs dry in it"""
+    M = pool_capacity(sms, 1) + 1
+    assert ll_grid(sms, M, 1)[0] == 0 and ll_grid(sms, M, 2)[0] > 0
+    m, R = 25, 24
+    rng = np.random.default_rng(7650 + N)
+    big = random_nodes(rng, N, M + 5000, depth_lo=2, depth_hi=N)
+    if case == "below_m":  # (the lone pool is the second handle)
+        starts, calls = [deep_nodes(rng, N, m - 1), big], (0, 1, 3, R - 4)
+    else:
+        starts, calls = [big, deep_nodes(rng, N, 40)], (2, 1, 3, R - 6)
+    oracles = [OraclePool(N, s) for s in starts]
+    with Handles(N, M, 2) as evs:
+        assert evs[0].pools_per_launch(M) == 2
+        for ev, s in zip(evs, starts):
+            ev.pool_push(s)
+        for k in calls:
+            run_and_check(evs, oracles, m, M, k)
+            if case == "dry":
+                assert 1 <= len(oracles[1].rounds) <= 2 and oracles[1].size < m
+    lone, other = (oracles[1], oracles[0]) if case == "below_m" else (oracles[0], oracles[1])
+    assert len(lone.rounds) == R and all(r["parents"] == M for r in lone.rounds)
+    assert other.size < m
 
 
 # ------------------------------------------------------------------------------------------ persistent-kernel edges

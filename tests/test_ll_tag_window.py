@@ -63,7 +63,7 @@ def test_window_edges(window):
 @pytest.mark.parametrize("seed", range(4))
 def test_launch_sequences_keep_the_window(window, seed):
     """random launches (round budgets from 1 to beyond the window, launches that stop early): the host's loop of
-    nq_ll_run_multi, one decision at a time"""
+    rounds_run (NqRounds::prepare), one decision at a time"""
     rng = np.random.default_rng(seed)
     epoch, clear, clears = 0, 0, 0
     for _ in range(3000):

@@ -6,7 +6,7 @@ python tools/step2_pace.py [--steps 3] [--launches]
 Replays bench.py's step2() on one GPU: the same warm-up split into P pools (the reference's strided split), the same
 calls of tsb_nq_pool_run_multi with 2048 rounds per pool, the same steal rule between calls (a pool with fewer than m
 nodes takes the oldest half of the fullest pool).  It runs with TSB200_ROUNDS_PROF=1 and reads the library's per-launch
-records from stderr (nq_ll_run_multi: "LL pace", "LL residency").  A launch ends when its last pool leaves; the other
+records from stderr (NqRounds::report: "LL pace", "LL residency").  A launch ends when its last pool leaves; the other
 pools idle their CTAs' share of the GPU for the rest of it.  After one step that warms up, per timed step:
   launches, steals, the time inside launches (first pool start to last pool exit, %globaltimer) against t_dev (CUDA
   events around the whole step), and the host time between launches (last exit of one launch to the first start of
