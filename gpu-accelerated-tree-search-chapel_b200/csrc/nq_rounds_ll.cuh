@@ -17,18 +17,22 @@
 //
 //   fat node = 4 x 8-byte words; word i = data32[i] | x16[i] << 32 | tag << 48   (32 B per node = one sector,
 //   32-byte aligned), read and written as two 16-byte pieces (words 0-1 and 2-3)
-//   data32[0..3] = the node packed in 125 bits (any N <= 20: every board value is below 32):
-//     board[i] in bits 5 (i % 6) .. +4 of data32[i / 6]            (six values per word; board[18], [19] in data32[3])
+//   data32[0..3] = the node packed in 125 bits (any N <= 24: every board value is below 32):
+//     board[i] in bits 5 (i % 6) .. +4 of data32[i / 6]            (six values per word)
 //     depth in the 2-bit tails (bits 30..31) of data32[0], [1], [2]: bits 0-1, 2-3 and 4 of the depth
-//     data32[3] bits 10..29: the node's child mask (slot k set <=> k >= depth and board[k] is not attacked: evaluate_gpu's
-//     label for slot k, nqueens_gpu_chpl.chpl:97-123), bit 30: leaf (depth == N)
+//     21-byte records (N <= 20): data32[3] holds board[18], [19] in bits 0..9, then bits 10..29: the node's child mask
+//     (slot k set <=> k >= depth and board[k] is not attacked: evaluate_gpu's label for slot k,
+//     nqueens_gpu_chpl.chpl:97-123), bit 30: leaf (depth == N)
+//     25-byte records (a wide handle, N <= 24): data32[3] holds board[18..23] in bits 0..29; neither the child mask
+//     nor the leaf flag is stored: a leaf is depth == N, and the child mask is evaluated when the node is read as a
+//     parent, from its board and its diagonal masks (ll_child_mask: a few slots, most parents lie at depth N-4..N-3)
 //   x16[0..3] = the node's diagonal masks, the values its next row attacks (N bits each):
 //     ld (rising diagonals) = x16[0] | x16[1] << 16, in piece 0; rd (falling diagonals) = x16[2] | x16[3] << 16, in piece 1
 //   tag = the 16-bit tag of the epoch the word was stored in (ll_tag; 0: no round's tag, see below)
-//   A child's masks follow from its parent's in O(1) and its child mask is evaluated from them when it is built
-//   (ll_build_child), so a round reads its parents' masks instead of recomputing them from the placed prefix.  (An
-//   earlier version stored the masks in a side word next to each 21-byte node: 64 bytes per node, twice the poll loads
-//   and store pieces of a round.)
+//   A child's masks follow from its parent's in O(1) and (21-byte records) its child mask is evaluated from them when it
+//   is built (ll_build_child), so a round reads its parents' masks instead of recomputing them from the placed prefix.
+//   (An earlier version stored the masks in a side word next to each 21-byte node: 64 bytes per node, twice the poll
+//   loads and store pieces of a round.)
 //
 // Every 8-byte word is written by one store (an element of a st.v2.u64) and is therefore seen whole or not at all;
 // a reader that expects the children of round r polls the words of its slice until all four carry r's tag.  No
@@ -66,7 +70,7 @@
 // stores, behind two CTA barriers; the exchange warp gathers while the workers build and does the bookkeeping before
 // the handoff, so the workers go from their stores straight into the next poll (6 % faster, DESIGN §5).
 //
-// The plain 21-byte arena is converted
+// The plain arena (21- or 25-byte records) is converted
 // to and from the fat arena by nq_fat_import / nq_fat_export (whole pool, only when the host needs the plain form:
 // drain, steal, pool_step, arena growth).
 //
@@ -74,7 +78,8 @@
 // a chain of L2 round trips with little work in between, and nothing inside one pool can fill the waits — another
 // pool's CTA on the same SM can: on the N = 17 search at M = 50000 three or four pools per launch (two pools per SM in
 // all, 768 parents per CTA) take little more than half the time of one pool.  Four pools run as grid (G, 2) of CTAs
-// that each hold two pools' CTAs as halves (HALVES, above nq_rounds_ll_kernel).
+// that each hold two pools' CTAs as halves (HALVES, above nq_rounds_ll_kernel).  Pools of 25-byte records run one per
+// launch (nq_rounds_ll_wide_kernel).
 //
 // A spin loop that waits longer than ~2 s raises a global abort flag and every CTA leaves (exit code ABORT): a logic
 // error must never hang the GPU.
@@ -161,8 +166,8 @@ __device__ __forceinline__ void ll_piece(uint32_t d0, uint32_t d1, uint32_t mask
   b = static_cast<unsigned long long>(__byte_perm(mask, tag, 0x5432)) << 32 | d1;
 }
 // the packed node (data32[0..3], see above)
-constexpr int LL_CM_SHIFT = 10;          // child mask: data32[3] bits 10..29
-constexpr uint32_t LL_LEAF = 1u << 30;   // leaf flag: data32[3] bit 30
+constexpr int LL_CM_SHIFT = 10;          // (21-byte records) child mask: data32[3] bits 10..29
+constexpr uint32_t LL_LEAF = 1u << 30;   // (21-byte records) leaf flag: data32[3] bit 30
 __host__ __device__ constexpr int ll_fw(int i) { return i / 6; }        // data word of board[i]
 __host__ __device__ constexpr int ll_fs(int i) { return 5 * (i % 6); }  // its first bit
 __device__ __forceinline__ uint32_t ll_depth(uint32_t d0, uint32_t d1, uint32_t d2) {
@@ -269,6 +274,29 @@ __global__ void nq_fat_import_kernel(const uint8_t* __restrict__ arena, FatNode*
   ll_piece(d[2], d[3], static_cast<uint32_t>(aux >> 20) & 0xFFFFFu, 0u, w[2], w[3]);
   for (int i = 0; i < LL_WORDS; i += 2) st_fat2(&fat[p].w[i], w[i], w[i + 1]);
 }
+// the same for 25-byte records: board[18..23] in data32[3], no child mask or leaf flag, the diagonal masks N <= 24
+// bits each.  (A kernel of its own: as a template over the record width the 21-byte kernel's SASS would not stay the
+// same.)
+template <int N>
+__global__ void nq_fat_import_wide_kernel(const uint8_t* __restrict__ arena, FatNode* __restrict__ fat, long long size) {
+  const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (p >= size) return;
+  const uint8_t* node = arena + p * NQ_REC24;
+  uint32_t d[LL_WORDS] = {0, 0, 0, 0};
+  for (int i = 0; i < NQ_REC24 - 1; i++) d[ll_fw(i)] |= static_cast<uint32_t>(node[1 + i]) << ll_fs(i);
+  ll_set_depth(d, node[0]);
+  const int depth = node[0];
+  uint32_t ld = 0, rd = 0;
+  for (int i = 0; i < depth && i < N; i++) {
+    const int b = node[1 + i], s = depth - i;
+    if (b + s < N) ld |= 1u << (b + s);
+    if (b - s >= 0) rd |= 1u << (b - s);
+  }
+  unsigned long long w[LL_WORDS];
+  ll_piece(d[0], d[1], ld, 0u, w[0], w[1]);
+  ll_piece(d[2], d[3], rd, 0u, w[2], w[3]);
+  for (int i = 0; i < LL_WORDS; i += 2) st_fat2(&fat[p].w[i], w[i], w[i + 1]);
+}
 // the clear: tag 0 on the `words` first words of the arena, data kept
 __global__ void nq_fat_clear_tags_kernel(FatNode* __restrict__ fat, long long words) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -277,14 +305,22 @@ __global__ void nq_fat_clear_tags_kernel(FatNode* __restrict__ fat, long long wo
     *w &= 0x0000FFFFFFFFFFFFull;
   }
 }
-__global__ void nq_fat_export_kernel(const FatNode* __restrict__ fat, uint8_t* __restrict__ arena, long long size) {
+// fat nodes -> R-byte records (nq_fat_export_kernel, nq_fat_export_wide_kernel)
+template <int R>
+__device__ __forceinline__ void nq_fat_export_body(const FatNode* __restrict__ fat, uint8_t* __restrict__ arena, long long size) {
   const long long p = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (p >= size) return;
-  uint8_t* node = arena + p * NQ_REC;
+  uint8_t* node = arena + p * R;
   uint32_t d[LL_WORDS];
   for (int i = 0; i < LL_WORDS; i++) d[i] = static_cast<uint32_t>(fat[p].w[i]);
   node[0] = static_cast<uint8_t>(ll_depth(d[0], d[1], d[2]));
-  for (int i = 0; i < NQ_REC - 1; i++) node[1 + i] = static_cast<uint8_t>(d[ll_fw(i)] >> ll_fs(i) & 31u);
+  for (int i = 0; i < R - 1; i++) node[1 + i] = static_cast<uint8_t>(d[ll_fw(i)] >> ll_fs(i) & 31u);
+}
+__global__ void nq_fat_export_kernel(const FatNode* __restrict__ fat, uint8_t* __restrict__ arena, long long size) {
+  nq_fat_export_body<NQ_REC>(fat, arena, size);
+}
+__global__ void nq_fat_export_wide_kernel(const FatNode* __restrict__ fat, uint8_t* __restrict__ arena, long long size) {
+  nq_fat_export_body<NQ_REC24>(fat, arena, size);
 }
 
 // The exchange warp's count gather: 2G slots {epoch << 32 | leaves << 20 | children}, lane l holds the slot pairs
@@ -355,7 +391,7 @@ __device__ __forceinline__ bool warp_gather_slots2(const unsigned long long* slo
     load();
   }
 }
-// The gathered children over all slots and over the slots before k0 / k1 (in every lane: at most 2G x 13 056, 32
+// The gathered children over all slots and over the slots before k0 / k1 (in every lane: at most 2G x 18 432, 32
 // bits), and this lane's share of the leaves
 __device__ __forceinline__ void warp_sum_slots2(const unsigned long long* slot, const unsigned long long (&v0)[LL_GB],
                                                 const unsigned long long (&v1)[LL_GB], int n, int k0, int k1,
@@ -409,13 +445,14 @@ enum {
   LL_PROF_N
 };
 static_assert(LL_PROF_N <= 12, "RoundsState::prof");
-template <int T, int PPT>
+// (R: the pool's record width; a parent has at most R - 1 children)
+template <int T, int PPT, int R = NQ_REC>
 struct LlSmem {
   alignas(16) uint4 parent[T * PPT];   // the slice: data32[0..3] of every parent
   alignas(8) uint2 diag[T * PPT];      // ... and its {ld, rd}
   alignas(16) uint4 stage[LL_CAP];     // the window's children: data32[0..3]
   alignas(8) uint2 stage_diag[LL_CAP]; // ... and their {ld, rd}
-  alignas(16) uint16_t item[T * PPT * 20];  // (record << 5) | slot, in child order
+  alignas(16) uint16_t item[T * PPT * (R - 1)];  // (record << 5) | slot, in child order
   unsigned long long warp_tot64[T / 32];
   LlPlan plan;
   int poll_abort;                  // a worker's poll gave up: the exchange warp leaves after the scan barrier
@@ -426,9 +463,29 @@ struct LlSmem {
   unsigned lay_tag[LL_LAYERS];     // ... and the tag its nodes were stored with (LL_TRUSTED: before the launch)
 };
 
-// child `item` of the slice -> its four data words (board[depth] and board[k] swapped, depth + 1, its child mask
-// evaluated here over the board words that hold a slot >= depth + 1) and *cdiag its diagonal masks, from its parent's
+// The child mask of a node with data words P at `depth` whose row `depth` has the safe values S = ~(ld | rd): slot i
+// set <=> i >= depth and bit board[i] of S is set (evaluate_gpu's label for slot i).  Only the data words that hold a
+// slot >= depth are read (word 0 is skipped from depth 6 on, word 1 from depth 12, word 2 from depth 18); the slots of
+// the words that are read are masked at the end (none for a leaf).  Bits of P above the board are ignored.
 template <int N>
+__device__ __forceinline__ uint32_t ll_child_mask(const uint32_t (&P)[4], uint32_t depth, uint32_t S) {
+  uint32_t cm = 0;
+#pragma unroll
+  for (int j = 0; j < 4; j++) {
+    if (6 * j >= N) break;
+    if (6 * j + 6 < N && depth >= static_cast<uint32_t>(6 * j + 6)) continue;
+#pragma unroll
+    for (int i = 6 * j; i < 6 * j + 6 && i < N; i++) {
+      const uint32_t x = shf_r_wrap(S, 0u, P[j] >> ll_fs(i)) & 1u;  // bit board[i] of S (the shift wraps mod 32)
+      asm("mad.lo.u32 %0, %1, %2, %0;" : "+r"(cm) : "r"(x), "r"(1u << i));  // cm |= x << i on the FMA pipe
+    }
+  }
+  return cm & shl_clamp(0xFFFFFFFFu, depth);
+}
+
+// child `item` of the slice -> its four data words (board[depth] and board[k] swapped, depth + 1; 21-byte records: its
+// child mask evaluated here, ll_child_mask) and *cdiag its diagonal masks, from its parent's
+template <int N, int R>
 __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2* diag, int item, uint2* cdiag) {
   const int r = item >> 5;
   const uint32_t k = static_cast<uint32_t>(item & 31);
@@ -436,7 +493,7 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
   uint32_t P[4] = {p.x, p.y, p.z, p.w};
   const uint32_t depth = ll_depth(p.x, p.y, p.z);
   // first bit of board[i] in the four data words read as one 128-bit value: 32 (i / 6) + 5 (i % 6) = 5 i + 2 (i / 6),
-  // with i / 6 = (43 i) >> 8 for every i < 20 (no division)
+  // with i / 6 = (43 i) >> 8 for every i < 24 (no division; it holds up to i = 127)
   const uint32_t bd = 5u * depth + 2u * (depth * 43u >> 8), bk = 5u * k + 2u * (k * 43u >> 8);
   // (a clamped right shift by b - 32 j is the field at bit b in word j and 0 in every other word)
   const auto field = [&](uint32_t b) {
@@ -453,22 +510,11 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
   const uint32_t bit = 1u << v;
   const uint32_t cld = ((pd.x | bit) << 1) & ((1u << N) - 1u), crd = (pd.y | bit) >> 1;
   *cdiag = make_uint2(cld, crd);
-  const uint32_t S = ~(cld | crd);  // safe values of row cd
-  uint32_t cm = 0;
-  // only slots i >= cd exist (none for a leaf): a data word whose six slots all lie below cd is skipped (word 0 for
-  // children of depth 6 and more, word 1 from depth 12); the slots of the words that are read are masked below
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    if (6 * j >= N) break;
-    if (6 * j + 6 < N && cd >= static_cast<uint32_t>(6 * j + 6)) continue;
-#pragma unroll
-    for (int i = 6 * j; i < 6 * j + 6 && i < N; i++) {
-      const uint32_t x = shf_r_wrap(S, 0u, P[j] >> ll_fs(i)) & 1u;  // bit board[i] of S (the shift wraps mod 32)
-      asm("mad.lo.u32 %0, %1, %2, %0;" : "+r"(cm) : "r"(x), "r"(1u << i));  // cm |= x << i on the FMA pipe
-    }
+  if constexpr (R == NQ_REC) {
+    const uint32_t cm = ll_child_mask<N>(P, cd, ~(cld | crd));  // (the safe values of row cd)
+    P[3] = (P[3] & 0x3FFu) | cm << LL_CM_SHIFT | (cd == static_cast<uint32_t>(N) ? LL_LEAF : 0u);
   }
-  cm &= shl_clamp(0xFFFFFFFFu, cd);  // only slots i >= depth + 1 exist (none for a leaf)
-  P[3] = (P[3] & 0x3FFu) | cm << LL_CM_SHIFT | (cd == static_cast<uint32_t>(N) ? LL_LEAF : 0u);
+  // (25-byte records: data32[3] is board[18..23], bits 30..31 stay 0)
   return make_uint4(P[0], P[1], P[2], P[3]);
 }
 
@@ -495,15 +541,17 @@ __device__ __forceinline__ uint4 ll_build_child(const uint4* parent, const uint2
 // sub-partition are those of equal warp id mod 4: nine warps per half put both halves' warps on every sub-partition,
 // two workers of each half on each, the exchange warps (8 and 17) on sub-partitions 0 and 1.  With two CTAs per SM the
 // CTA that became resident second ran the slower pool (DESIGN §5).
-template <int N, int T, int MINB, int PPT, int HALVES = 1>
-__global__ void __launch_bounds__(HALVES * (T + 32), MINB) nq_rounds_ll_kernel(const __grid_constant__ LlMultiParams mprm) {
-  static_assert(HALVES == 1 || (HALVES == 2 && MINB == 1), "two pools per CTA: one CTA per SM");
+//
+// REC: the record width of the pool's plain arena, which decides the fat node's data32[3] (see the top of this file):
+// NQ_REC (nq_rounds_ll_kernel, every variant) or NQ_REC24 (nq_rounds_ll_wide_kernel: one pool per launch).
+template <int N, int T, int PPT, int HALVES, int REC>
+__device__ __forceinline__ void nq_rounds_ll_body(const LlMultiParams& mprm) {
   constexpr int LL_PPT = PPT;
   constexpr int TX = T + 32;  // the whole CTA (HALVES = 1) or half: workers + exchange warp
   const int half = HALVES == 2 && threadIdx.x >= TX ? 1 : 0;
   const LlParams& prm = mprm.pool[blockIdx.y + gridDim.y * half];
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  LlSmem<T, PPT>& sm = reinterpret_cast<LlSmem<T, PPT>*>(smem_raw)[half];
+  LlSmem<T, PPT, REC>& sm = reinterpret_cast<LlSmem<T, PPT, REC>*>(smem_raw)[half];
   const int bar_w = LL_BAR_W + LL_BAR_HALF * half, bar_scan = LL_BAR_SCAN + LL_BAR_HALF * half,
             bar_hand = LL_BAR_HAND + LL_BAR_HALF * half;
   const int t = threadIdx.x - TX * half, lane = t & 31, wid = t >> 5;
@@ -772,9 +820,17 @@ __global__ void __launch_bounds__(HALVES * (T + 32), MINB) nq_rounds_ll_kernel(c
         const int i = LL_PPT * t + q;
         cm[q] = 0;
         if (i < len) {
-          const uint32_t w3 = sm.parent[i].w;
-          cm[q] = w3 >> LL_CM_SHIFT & 0xFFFFFu;
-          leaves += (w3 & LL_LEAF) ? 1 : 0;
+          if constexpr (REC == NQ_REC) {
+            const uint32_t w3 = sm.parent[i].w;
+            cm[q] = w3 >> LL_CM_SHIFT & 0xFFFFFu;
+            leaves += (w3 & LL_LEAF) ? 1 : 0;
+          } else {  // (no stored mask or leaf flag: evaluated from the board, the depth and the diagonal masks)
+            const uint4 p = sm.parent[i];
+            const uint2 dg = sm.diag[i];
+            const uint32_t P[4] = {p.x, p.y, p.z, p.w}, depth = ll_depth(p.x, p.y, p.z);
+            cm[q] = ll_child_mask<N>(P, depth, ~(dg.x | dg.y));
+            leaves += depth == static_cast<uint32_t>(N) ? 1 : 0;
+          }
           mine += __popc(cm[q]);
           if (i < len0) mine0 += __popc(cm[q]);
         }
@@ -783,8 +839,8 @@ __global__ void __launch_bounds__(HALVES * (T + 32), MINB) nq_rounds_ll_kernel(c
       if (prm.prof != 0)
 #pragma unroll
         for (int q = 0; q < LL_PPT; q++) prof_fertile += cm[q] != 0u ? 1u : 0u;
-      // ---- (3) block scan: children | leaves << 20 | children of the bottom sub-slice << 32 (at most 13 056, 768
-      // and 13 056 per CTA: no field overflows into the next)
+      // ---- (3) block scan: children | leaves << 20 | children of the bottom sub-slice << 32 (at most 768 x 24 =
+      // 18 432, 768 and 18 432 per CTA: no field overflows into the next)
       unsigned long long incl = static_cast<unsigned long long>(mine) | static_cast<unsigned long long>(leaves) << 20 |
                                 static_cast<unsigned long long>(mine0) << 32;
 #pragma unroll
@@ -821,7 +877,7 @@ __global__ void __launch_bounds__(HALVES * (T + 32), MINB) nq_rounds_ll_kernel(c
       // ---- (5) my children (first window), built and evaluated while the other CTAs' counts are on their way
       auto build_window = [&](int c0, int cnt) {
         for (int c = t; c < cnt; c += T)
-          sm.stage[c] = ll_build_child<N>(sm.parent, sm.diag, sm.item[c0 + c], &sm.stage_diag[c]);
+          sm.stage[c] = ll_build_child<N, REC>(sm.parent, sm.diag, sm.item[c0 + c], &sm.stage_diag[c]);
       };
       build_window(0, min(LL_CAP, my_children));
       TSB_PROF(prof_w, 0, LL_PROF_BUILD)
@@ -888,6 +944,16 @@ __global__ void __launch_bounds__(HALVES * (T + 32), MINB) nq_rounds_ll_kernel(c
       for (int i = 0; i < LL_PROF_N; i++) st->prof[i] = sm.prof[i];
   }
 #undef TSB_PROF
+}
+template <int N, int T, int MINB, int PPT, int HALVES = 1>
+__global__ void __launch_bounds__(HALVES * (T + 32), MINB) nq_rounds_ll_kernel(const __grid_constant__ LlMultiParams mprm) {
+  static_assert(HALVES == 1 || (HALVES == 2 && MINB == 1), "two pools per CTA: one CTA per SM");
+  nq_rounds_ll_body<N, T, PPT, HALVES, NQ_REC>(mprm);
+}
+// 25-byte records (wide handles, N <= 24): one pool per launch, one CTA per SM, two parents per worker thread
+template <int N>
+__global__ void __launch_bounds__(LL_T + 32, 1) nq_rounds_ll_wide_kernel(const __grid_constant__ LlMultiParams mprm) {
+  nq_rounds_ll_body<N, LL_T, 2, 1, NQ_REC24>(mprm);
 }
 
 // ---- diagnostics (tsb_debug_flag_exchange, tools/flag_exchange.py): cycles per round of bare all-to-all flag exchanges

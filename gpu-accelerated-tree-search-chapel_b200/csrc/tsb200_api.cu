@@ -963,7 +963,7 @@ void enable_peer(int a, int b) {
 struct tsb_nq : Base {
   tsb_nq* sibling[3] = {nullptr, nullptr, nullptr};  // further pools on the same device, owned by this handle (tsb_nq_sibling)
   int N = 0, g = 1;
-  bool wide = false;  // MAX_QUEENS = 24 build (tsb_nq_create_wide): 25-byte tsb_nq_node24 records, no persistent kernel
+  bool wide = false;  // MAX_QUEENS = 24 build (tsb_nq_create_wide): 25-byte tsb_nq_node24 records, one pool per launch
   int tile_threads = 0;  // env TSB200_NQ_TILE_THREADS = 128: always the TMA-pipelined kernel (tests force it on small chunks)
   tsb::FatNode* d_fat = nullptr;  // the pool in the self-validating 32-byte format, while the LL kernel owns it
   long long fat_cap = 0;
@@ -1093,20 +1093,29 @@ bool nq_nodes_valid(int N, size_t rec, const uint8_t* nodes, int64_t n) {
   return true;
 }
 
-template <int N>
+template <int N, int R>
 int nq_ll_launch_n(tsb_nq* h, const tsb::LlMultiParams& prm, int grid, int pools, int ppt, cudaStream_t s) {
   // (one pool: one CTA per SM; two or three: two CTAs of LL_T workers + the exchange warp per SM, capped at 112
   // registers; three or four pools: 66 CTAs per pool with 768 parents each on 132 SMs, see ll_slice.  Four pools:
-  // one CTA per SM of two such halves, each running one pool (nq_rounds_ll_kernel, HALVES = 2), grid (grid, 2).)
+  // one CTA per SM of two such halves, each running one pool (nq_rounds_ll_kernel, HALVES = 2), grid (grid, 2).
+  // 25-byte records: one pool, nq_ll_grid.)
   const int halves = pools == tsb::LL_MAX_POOLS ? 2 : 1;
-  const int var = pools == 1 ? 0 : (ppt == 2 ? 1 : 2) + (halves == 2 ? 2 : 0);
-  auto kernel = var == 0   ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 2>
-                : var == 1 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 2>
-                : var == 2 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 3>
-                : var == 3 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 2, 2>
-                           : tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 3, 2>;
-  static_assert(2 * sizeof(tsb::LlSmem<tsb::LL_T, 3>) + 128 <= 227 * 1024, "two halves' shared memory in one CTA");
-  const size_t smem = halves * (ppt == 2 ? sizeof(tsb::LlSmem<tsb::LL_T, 2>) : sizeof(tsb::LlSmem<tsb::LL_T, 3>)) + 128;
+  void (*kernel)(const tsb::LlMultiParams);
+  size_t smem;
+  if constexpr (R == tsb::NQ_REC24) {
+    if (pools != 1 || ppt != 2) return TSB_EINVAL;
+    kernel = tsb::nq_rounds_ll_wide_kernel<N>;
+    smem = sizeof(tsb::LlSmem<tsb::LL_T, 2, R>) + 128;
+  } else {
+    const int var = pools == 1 ? 0 : (ppt == 2 ? 1 : 2) + (halves == 2 ? 2 : 0);
+    kernel = var == 0   ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 2>
+             : var == 1 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 2>
+             : var == 2 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 2, 3>
+             : var == 3 ? tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 2, 2>
+                        : tsb::nq_rounds_ll_kernel<N, tsb::LL_T, 1, 3, 2>;
+    static_assert(2 * sizeof(tsb::LlSmem<tsb::LL_T, 3>) + 128 <= 227 * 1024, "two halves' shared memory in one CTA");
+    smem = halves * (ppt == 2 ? sizeof(tsb::LlSmem<tsb::LL_T, 2>) : sizeof(tsb::LlSmem<tsb::LL_T, 3>)) + 128;
+  }
   int rc = h->configure(kernel, smem);
   if (rc != TSB_OK) return rc;
   void* args[] = {const_cast<tsb::LlMultiParams*>(&prm)};
@@ -1117,12 +1126,15 @@ int nq_ll_launch_n(tsb_nq* h, const tsb::LlMultiParams& prm, int grid, int pools
   return TSB_OK;
 }
 // the plain arena's [0, pool.size) -> d_fat
-template <int N>
+template <int N, int R>
 int nq_fat_import(tsb_nq* h) {
   const long long size = h->pool.size;
   if (size > 0) {
-    tsb::nq_fat_import_kernel<N><<<static_cast<unsigned>((size + 255) / 256), 256, 0, h->stream>>>(
-        h->pool.arena[h->pool.cur], h->d_fat, size);
+    const unsigned blocks = static_cast<unsigned>((size + 255) / 256);
+    if constexpr (R == tsb::NQ_REC24)
+      tsb::nq_fat_import_wide_kernel<N><<<blocks, 256, 0, h->stream>>>(h->pool.arena[h->pool.cur], h->d_fat, size);
+    else
+      tsb::nq_fat_import_kernel<N><<<blocks, 256, 0, h->stream>>>(h->pool.arena[h->pool.cur], h->d_fat, size);
     TSB_CUDA(cudaGetLastError());
     h->launches++;
   }
@@ -1158,14 +1170,14 @@ int nq_fat_tag_window(tsb_nq* h, int64_t max_rounds, unsigned* epoch_last, bool*
   *epoch_last = w.epoch_last;
   return TSB_OK;
 }
-// the pool back in the plain 21-byte arena (whoever needs the node records calls this first)
+// the pool back in the plain arena of 21- or 25-byte records (whoever needs the node records calls this first)
 int nq_materialize(tsb_nq* h) {
   if (!h->in_fat) return TSB_OK;
   TSB_CUDA(cudaSetDevice(h->device));
   const long long size = h->pool.size;
   if (size > 0) {
-    tsb::nq_fat_export_kernel<<<static_cast<unsigned>((size + 255) / 256), 256, 0, h->stream>>>(
-        h->d_fat, h->pool.arena[h->pool.cur], size);
+    auto kernel = h->wide ? tsb::nq_fat_export_wide_kernel : tsb::nq_fat_export_kernel;
+    kernel<<<static_cast<unsigned>((size + 255) / 256), 256, 0, h->stream>>>(h->d_fat, h->pool.arena[h->pool.cur], size);
     TSB_CUDA(cudaGetLastError());
     h->launches++;
     TSB_CUDA(cudaStreamSynchronize(h->stream));
@@ -1179,9 +1191,9 @@ int nq_materialize(tsb_nq* h) {
 // flag exchange among all SMs' CTAs costs 2-3x one among half of them (tools/flag_exchange.py); the per-CTA work grows
 // the other way.
 // *ppt: parents per thread of the kernel variant to launch (2, or 3 when the pool's CTAs would not cover M with 2).
+// Wide handles (25-byte records) run one pool per launch: 0 for pools > 1.
 int nq_ll_grid(const tsb_nq* h, int M, int pools, int* ppt = nullptr) {
-  // (a wide handle's 24-queen boards do not fit the 32-byte nodes of the persistent kernel: two-kernel rounds)
-  if (h->wide || !h->di.coop || env_no_rounds() || pools < 1 || pools > tsb::LL_MAX_POOLS) return 0;
+  if (!h->di.coop || env_no_rounds() || pools < 1 || pools > (h->wide ? 1 : tsb::LL_MAX_POOLS)) return 0;
   const int sms = std::min(h->di.sms, tsb::LL_MAX_SMS);
   const int most = tsb::ll_ctas_per_pool(sms, pools);  // (ll_tiers.h: the drivers size their warm-up by the same tiers)
   const int per = static_cast<long long>(most) * tsb::ll_slice(2) >= M ? 2 : 3;
@@ -1211,7 +1223,8 @@ struct NqRounds {
       // room for the worst case of the next round
       rc = p.make_stack(h->stream, need);
       if (rc == TSB_OK) rc = nq_ensure_fat(h, p.cap);
-      if (rc == TSB_OK) rc = with_queens(h->N, [h](auto q) { return nq_fat_import<decltype(q)::value>(h); });
+      if (rc == TSB_OK)
+        rc = with_board(h, [h](auto n, auto r) { return nq_fat_import<decltype(n)::value, decltype(r)::value>(h); });
       if (rc != TSB_OK) return rc;
       h->in_fat = true;
       *queued = true;
@@ -1221,7 +1234,9 @@ struct NqRounds {
     return nq_fat_tag_window(h, left, &prm->epoch_last, queued);
   }
   int launch(tsb_nq* h0, const tsb::LlMultiParams& mp, int grid, int pools, int ppt) const {
-    return with_queens(h0->N, [&](auto q) { return nq_ll_launch_n<decltype(q)::value>(h0, mp, grid, pools, ppt, h0->stream); });
+    return with_board(h0, [&](auto n, auto r) {
+      return nq_ll_launch_n<decltype(n)::value, decltype(r)::value>(h0, mp, grid, pools, ppt, h0->stream);
+    });
   }
   // SPACE: back to the plain arena, which grows before the next launch; RELAUNCH (layer table full, or the tag window
   // used up): a fresh launch trusts the whole pool; DONE or PAUSE: the pool leaves

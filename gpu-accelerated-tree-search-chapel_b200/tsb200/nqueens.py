@@ -23,7 +23,7 @@ def nq_node_dtype(N: int) -> np.dtype:
 class NQueensEvaluator:
     """Owns what `on device var parents_d, labels_d` owns in the reference (nqueens_gpu_chpl.chpl:194-195).
     N > 20, or max_queens=24 for any N, creates a MAX_QUEENS = 24 handle (tsb_nq_create_wide): its nodes are
-    NQ_NODE24_DTYPE records (`node_dtype`), and its device pools run two-kernel rounds."""
+    NQ_NODE24_DTYPE records (`node_dtype`), and its device pools run one pool per launch of the persistent kernel."""
 
     wide, node_dtype = False, NQ_NODE_DTYPE  # (an object that wraps a tsb_nq_create handle)
 

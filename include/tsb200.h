@@ -125,9 +125,10 @@ int tsb_nq_create(tsb_nq** h, int device, int N, int g, int M_max);
  * `-sMAX_QUEENS=24` program may still run --N 14).  Every N-Queens entry point below works on such a handle with
  * 25-byte tsb_nq_node24 records (parents, children and pool nodes) and N label bytes per parent; the push check
  * reads board[N..24) == 0.  Differences from a tsb_nq_create handle:
- *   - the persistent kernel is not used (its 32-byte nodes do not hold a 24-queen board): tsb_nq_pool_run is the
- *     tsb_nq_pool_step loop, tsb_nq_pools_per_launch returns 1, tsb_nq_pool_run_multi runs the pools one after the
- *     other;
+ *   - the persistent kernel serves one pool per launch (its 32-byte nodes hold a 24-queen board in place of the
+ *     stored child mask, which it evaluates when it reads a parent): tsb_nq_pool_run runs in it up to the one-pool
+ *     capacity (67 584 parents on an H100) and in tsb_nq_pool_step rounds above it, tsb_nq_pools_per_launch returns
+ *     1, tsb_nq_pool_run_multi runs the pools one after the other (each in its own launches);
  *   - tsb_nq_pool_steal and tsb_nq_pool_run_multi take wide handles only together (TSB_EINVAL for a mix). */
 int tsb_nq_create_wide(tsb_nq** h, int device, int max_queens, int N, int g, int M_max);
 /* the MAX_QUEENS of the build a handle serves: 20 (tsb_nq_create) or 24 (tsb_nq_create_wide); TSB_EINVAL for NULL */
@@ -176,7 +177,8 @@ int tsb_nq_pool_drain(tsb_nq* h, void* nodes, int64_t capacity_nodes, int64_t* n
  * 512 x #SMs (the reference's default --M 50000) the whole loop of nqueens_gpu_chpl.chpl:197-215 runs inside ONE
  * persistent cooperative kernel (per round one exchange of the child counts among its CTAs plus one store -> L2 ->
  * poll hop of the self-validating nodes, instead of two launches and a host round trip); larger M falls back to one
- * tsb_nq_pool_step per round.  Totals over the rounds come back. */
+ * tsb_nq_pool_step per round, and so does env TSB200_NO_ROUNDS=1.  The same on a tsb_nq_create_wide handle (N <= 24,
+ * 25-byte records).  Totals over the rounds come back. */
 /* work stealing between two device pools (the reference steals between its per-GPU host pools,
  * nqueens_multigpu_chpl.chpl:255-312): if the victim holds >= 2 m nodes, the oldest size / 2 of them
  * (popFrontBulkFree, lib/commons/Pool_par.chpl:178-191) move to the top of the thief's pool, device to device
@@ -392,7 +394,8 @@ typedef struct {
 int tsb_nq_warmup(int N, int min_size, void* nodes, int64_t capacity_nodes, int64_t* n, uint64_t* tree, uint64_t* sol);
 /* nqueens_gpu_chpl.chpl:152-248 / nqueens_multigpu_chpl.chpl:158-352 */
 /* N in 1..24: N <= 20 runs on tsb_nq_create handles exactly as before, N = 21..24 on tsb_nq_create_wide handles (the
- * same searches, with 25-byte nodes; the device pools of tsb_nq_search_device[_part] then run two-kernel rounds) */
+ * same searches, with 25-byte nodes; the device pools of tsb_nq_search_device[_part] then run one pool per task, in
+ * the persistent kernel up to the one-pool capacity) */
 int tsb_nq_search(int N, int g, int m, int M, int D, tsb_search_stats* out);
 /* the same search as a MAX_QUEENS = max_queens build runs it (only 24: TSB_EINVAL otherwise): 25-byte nodes and
  * tsb_nq_create_wide handles for every N in 1..24 (tsb_nq_search_device_wide: the device-pool search) */

@@ -1,6 +1,8 @@
 """The whole search of a board of 21 to 24 queens (default N = 21) on the GPU(s), as a `-sMAX_QUEENS=24` build of the
 reference runs it: the 3-step search with the pool of step 2 resident on the device (tsb_nq_search_device, 25-byte
-nodes, two-kernel rounds).  Prints the explored tree, the solutions against the published count (OEIS A000170), the
+nodes, one device pool per task).  Chunks of up to the one-pool capacity of the persistent kernel (67 584 parents on
+an H100; the reference's default is --M 50000) run the whole offload loop in that kernel, larger ones (the default
+here) two kernels per round.  Prints the explored tree, the solutions against the published count (OEIS A000170), the
 time, and the name and power limit of every card the search used; exits 1 when the solution count differs.
 
   python tools/nq_wide_search.py [--N 21] [--M 4194304] [--D 1] [--host]
