@@ -37,6 +37,8 @@ struct PfspLb1Tables {
                                        // ph[job*half_stride(M) + q] = p[2q][job] | p[2q+1][job] << 16
 };
 static_assert(sizeof(PfspLb1Tables) % 16 == 0, "blob must be a multiple of 16 B");
+// the 16-bit lanes of ph and of the simd16 kernels: every intermediate of their bounds must stay below this
+constexpr long long PF_LANE_LIMIT = 1 << 16;
 
 __device__ __forceinline__ void stage_blob(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
   if (threadIdx.x == 0) {
@@ -371,6 +373,25 @@ struct Lb2Const {
   uint32_t jp[PF_MAXP * PF_MAXJ];
 };
 static_assert(sizeof(Lb2Const) <= 16 * 1024, "must fit the kernel parameter space next to the other arguments");
+// The words of Lb2Const, decoded in lb2_phase_b (Lb2Const) (the pair words of pfsp_wide.cuh too).  Instances whose values do
+// not fit these fields get no lb2.
+//   pair word: ma0 | ma1 << 5 | min_tails[ma0] << 10 | min_tails[ma1] << 21
+//   job word:  job | p[ma0][job] << 5 | p[ma1][job] << 12 | lag << 19
+constexpr uint32_t LB2_MACH_MASK = 31, LB2_TAIL_MAX = 2047;
+constexpr int LB2_MB_SHIFT = 5, LB2_TA_SHIFT = 10, LB2_TB_SHIFT = 21;
+constexpr uint32_t LB2_JOB_MASK = 31, LB2_P_MAX = 127, LB2_LAG_MAX = 8191;
+constexpr int LB2_PA_SHIFT = 5, LB2_PB_SHIFT = 12, LB2_LAG_SHIFT = 19;
+static_assert(LB2_TB_SHIFT + 11 == 32 && LB2_LAG_SHIFT + 13 == 32, "the top field of a word is read without a mask");
+inline bool lb2_fits(int v, uint32_t max) { return v >= 0 && static_cast<uint32_t>(v) <= max; }
+inline uint32_t lb2_pair_word(int a, int b, int tail_a, int tail_b) {
+  return static_cast<uint32_t>(a) | static_cast<uint32_t>(b) << LB2_MB_SHIFT |
+         (static_cast<uint32_t>(tail_a) & LB2_TAIL_MAX) << LB2_TA_SHIFT |
+         (static_cast<uint32_t>(tail_b) & LB2_TAIL_MAX) << LB2_TB_SHIFT;
+}
+inline uint32_t lb2_job_word(int job, int pa, int pb, int lag) {
+  return static_cast<uint32_t>(job) | (static_cast<uint32_t>(pa) & LB2_P_MAX) << LB2_PA_SHIFT |
+         (static_cast<uint32_t>(pb) & LB2_P_MAX) << LB2_PB_SHIFT | (static_cast<uint32_t>(lag) & LB2_LAG_MAX) << LB2_LAG_SHIFT;
+}
 // v3, for instances with at most 10 machines (45 pairs) whose values fit 16 bits: one table word per USE (nothing
 // is unpacked) and the Johnson recurrence of a pair (compute_cmax_johnson, Bound_johnson.chpl:188-212)
 //     t0 += p0[j];   t1 = max(t1, t0 + lag[j]) + p1[j]        over the unscheduled jobs j in Johnson order
@@ -392,6 +413,15 @@ struct Lb2TabU {
   uint32_t tails[LB2U_PAIRS + 3]; // min_tails[ma0] | min_tails[ma1] << 16
 };
 static_assert(sizeof(Lb2TabU) % 16 == 0, "blob must be a multiple of 16 B");
+// the entries of Lb2TabU, decoded in lb2_phase_b (Lb2ConstU); values fit 16 bits (the simd16 route's condition)
+constexpr int LB2U_MB_SHIFT = 8, LB2U_TB_SHIFT = 16;
+inline uint32_t lb2u_mach_word(int a, int b) { return static_cast<uint32_t>(a) | static_cast<uint32_t>(b) << LB2U_MB_SHIFT; }
+inline uint32_t lb2u_tails_word(int tail_a, int tail_b) {
+  return static_cast<uint32_t>(tail_a) | static_cast<uint32_t>(tail_b) << LB2U_TB_SHIFT;
+}
+inline uint4 lb2u_entry(int job, int pa, int pb, int lag) {
+  return make_uint4(1u << job, static_cast<uint32_t>(pa + lag), static_cast<uint32_t>(pa - pb), 0u);
+}
 struct Lb2ConstU {  // kernel-parameter form of the route: just the device address of the table
   const Lb2TabU* tab;
 };
@@ -478,17 +508,17 @@ __device__ __forceinline__ void lb2_phase_b(Lb2Smem<M>& sm, const Lb2Const& C, c
       bool over = false;
       for (int l = l0; l < l1; l++) {
         const uint32_t pi = C.pair[l];
-        int tmp0 = sm.fc[pi & 31u][t], tmp1 = sm.fc[(pi >> 5) & 31u][t];
+        int tmp0 = sm.fc[pi & LB2_MACH_MASK][t], tmp1 = sm.fc[(pi >> LB2_MB_SHIFT) & LB2_MACH_MASK][t];
         const uint32_t* jp = &C.jp[l * PF_MAXJ];
 #pragma unroll
         for (int j = 0; j < PF_MAXJ; j++) {
           const uint32_t w = jp[j];
-          if (!(mask & (1u << (w & 31u)))) {
-            tmp0 += static_cast<int>((w >> 5) & 127u);
-            tmp1 = max(tmp1, tmp0 + static_cast<int>(w >> 19)) + static_cast<int>((w >> 12) & 127u);
+          if (!(mask & (1u << (w & LB2_JOB_MASK)))) {
+            tmp0 += static_cast<int>((w >> LB2_PA_SHIFT) & LB2_P_MAX);
+            tmp1 = max(tmp1, tmp0 + static_cast<int>(w >> LB2_LAG_SHIFT)) + static_cast<int>((w >> LB2_PB_SHIFT) & LB2_P_MAX);
           }
         }
-        const int c = max(tmp1 + static_cast<int>(pi >> 21), tmp0 + static_cast<int>((pi >> 10) & 2047u));
+        const int c = max(tmp1 + static_cast<int>(pi >> LB2_TB_SHIFT), tmp0 + static_cast<int>((pi >> LB2_TA_SHIFT) & LB2_TAIL_MAX));
         lb = max(lb, c);
         if (lb > best) {
           over = true;
@@ -530,7 +560,7 @@ __device__ __forceinline__ void lb2_phase_b(Lb2Smem<M>& sm, const Lb2ConstU&, co
       bool over = false;
       for (int l = l0; l < l1; l++) {
         const uint32_t mm = sm.tabu.mach[l];
-        const int ma0 = mm & 255u, ma1 = mm >> 8;
+        const int ma0 = mm & ((1u << LB2U_MB_SHIFT) - 1), ma1 = mm >> LB2U_MB_SHIFT;
         const uint4* te = &sm.tabu.e[l * PF_MAXJ];
         int E = 0, m = -(1 << 28);
 #pragma unroll
@@ -544,7 +574,8 @@ __device__ __forceinline__ void lb2_phase_b(Lb2Smem<M>& sm, const Lb2ConstU&, co
         const uint32_t tl = sm.tabu.tails[l];
         const int t0 = sm.fc[ma0][t];
         const int t1f = sm.rc[ma1][t] + max(sm.fc[ma1][t], t0 + m);
-        const int c = max(t1f + static_cast<int>(tl >> 16), t0 + sm.rc[ma0][t] + static_cast<int>(tl & 0xFFFFu));
+        const int c = max(t1f + static_cast<int>(tl >> LB2U_TB_SHIFT),
+                          t0 + sm.rc[ma0][t] + static_cast<int>(tl & ((1u << LB2U_TB_SHIFT) - 1)));
         lb = max(lb, c);
         if (lb > best) {
           over = true;

@@ -17,6 +17,7 @@
 #pragma once
 #include <cstddef>
 
+#include "pfsp_kernels.cuh"
 #include "tsb_ptx.cuh"
 
 namespace tsb {
@@ -35,9 +36,17 @@ struct PfspWideTables {
   int32_t min_heads[PW_MAXM];
   int32_t min_tails[PW_MAXM];
   int32_t pj[PW_MAXJ * PW_PSTRIDE];  // pj[job * PW_PSTRIDE + k]
-  uint32_t pair[PW_MAXP + 4];        // in machine_pair_order: a | b << 5 | tail_a << 10 | tail_b << 21
-  uint32_t jp[PW_MAXP * PW_MAXJ];    // jp[l * jobs + pos] = job | p_a << 6 | p_b << 13 | lag << 20
+  uint32_t pair[PW_MAXP + 4];        // in machine_pair_order: lb2_pair_word (pfsp_kernels.cuh)
+  uint32_t jp[PW_MAXP * PW_MAXJ];    // jp[l * jobs + pos] = pw_job_word
 };
+// the Johnson words, decoded in pfsp_wide_kernel: job | p_a << 6 | p_b << 13 | lag << 20 (p_a, p_b <= LB2_P_MAX)
+constexpr uint32_t PW_JOB_MASK = 63, PW_LAG_MAX = 4095;
+constexpr int PW_PA_SHIFT = 6, PW_PB_SHIFT = 13, PW_LAG_SHIFT = 20;
+static_assert(PW_LAG_SHIFT + 12 == 32, "the lag is read without a mask");
+inline uint32_t pw_job_word(int job, int pa, int pb, int lag) {
+  return static_cast<uint32_t>(job) | (static_cast<uint32_t>(pa) & LB2_P_MAX) << PW_PA_SHIFT |
+         (static_cast<uint32_t>(pb) & LB2_P_MAX) << PW_PB_SHIFT | (static_cast<uint32_t>(lag) & PW_LAG_MAX) << PW_LAG_SHIFT;
+}
 static_assert(sizeof(PfspWideTables) % 16 == 0 && offsetof(PfspWideTables, jp) % 16 == 0, "staged with 16-byte loads");
 
 struct PfspWideSmem {
@@ -138,17 +147,17 @@ __global__ void __launch_bounds__(PW_THREADS) pfsp_wide_kernel(const uint8_t* __
           lb = 0;
           for (int l = 0; l < tab.pairs; l++) {
             const uint32_t pw = tab.pair[l];
-            const int a = pw & 31u, b = (pw >> 5) & 31u;
+            const int a = pw & LB2_MACH_MASK, b = (pw >> LB2_MB_SHIFT) & LB2_MACH_MASK;
             int t0 = sm.fc[a * PW_THREADS + t], t1 = sm.fc[b * PW_THREADS + t];
             const uint32_t* jp = &tab.jp[l * jobs];
             for (int pos = 0; pos < jobs; pos++) {  // compute_cmax_johnson (:188-212)
               const uint32_t e = jp[pos];
-              if (!((flags >> (e & 63u)) & 1ull)) {
-                t0 += (e >> 6) & 127u;
-                t1 = max(t1, t0 + static_cast<int>(e >> 20)) + static_cast<int>((e >> 13) & 127u);
+              if (!((flags >> (e & PW_JOB_MASK)) & 1ull)) {
+                t0 += (e >> PW_PA_SHIFT) & LB2_P_MAX;
+                t1 = max(t1, t0 + static_cast<int>(e >> PW_LAG_SHIFT)) + static_cast<int>((e >> PW_PB_SHIFT) & LB2_P_MAX);
               }
             }
-            const int c = max(t1 + static_cast<int>(pw >> 21), t0 + static_cast<int>((pw >> 10) & 2047u));
+            const int c = max(t1 + static_cast<int>(pw >> LB2_TB_SHIFT), t0 + static_cast<int>((pw >> LB2_TA_SHIFT) & LB2_TAIL_MAX));
             lb = max(lb, c);
             if (lb > best) break;  // :232-236
           }

@@ -11,6 +11,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <iterator>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <string>
@@ -947,6 +949,180 @@ int pool_steal(Base& victim, Base& thief, int m, int64_t* n_stolen, Plain&& plai
   return TSB_OK;
 }
 
+// Everything the kernels of a PFSP handle read, packed once from the tsb_pfsp_create arguments: a handle and its
+// siblings share one immutable copy, so a sibling takes its owner's route as it was fixed at creation
+struct PfspPacked {
+  int jobs = 0, machines = 0;
+  int pairs = 0;         // 0: no lb2 on this handle
+  int mt = 0;            // template machine count (5, 10 or 20)
+  bool wide = false;     // MAX_JOBS = 50: 208-byte nodes, the general kernels of pfsp_wide.cuh
+  bool simd16 = false;   // lb1 / lb1_d children two per register (values < 2^16, min_tails non-increasing)
+  bool lb2u = false;     // <= 10 machines: lb2 on the shared-memory-resident table `tabu`
+  bool valid = true;     // every machine pair, mp_order and Johnson index in range
+  tsb::PfspLb1Tables t1;   // 20 jobs
+  tsb::PfspWideTables tw;  // 50 jobs (lb2 tables included)
+  tsb::Lb2Const lb2c;      // 20 jobs: packed Johnson tables, passed to the lb2 kernels by value (constant bank)
+  tsb::Lb2TabU tabu;
+};
+
+// The tables for the reference built with MAX_JOBS = max_jobs (20 or 50), from arguments whose pointers and shape
+// tsb_pfsp_create_wide has checked.  Indices out of range clear `valid`; values that do not fit the lb2 words leave
+// the handle without lb2.  TSB200_NO_SIMD16 / TSB200_NO_LB2U (any value but "0" for the latter) turn routes off.
+std::shared_ptr<const PfspPacked> pfsp_pack(int max_jobs, int jobs, int machines, const int32_t* p_times,
+                                            const int32_t* min_heads, const int32_t* min_tails, int nb_pairs,
+                                            const int32_t* johnson, const int32_t* lags, const int32_t* mp0,
+                                            const int32_t* mp1, const int32_t* mp_order) {
+  auto t = std::make_shared<PfspPacked>();  // (value-initialised: every table and its padding start at zero)
+  t->jobs = jobs;
+  t->machines = machines;
+  t->pairs = nb_pairs;
+  t->mt = machines <= 5 ? 5 : machines <= 10 ? 10 : 20;
+  t->wide = max_jobs != TSB_MAX_JOBS;
+  tsb::PfspLb1Tables& t1 = t->t1;
+  tsb::PfspWideTables& tw = t->tw;
+  t1.jobs = tw.jobs = jobs;
+  t1.machines = tw.machines = machines;
+  t1.pairs = tw.pairs = nb_pairs;
+  t1.mp = tsb::row_stride(t->mt);
+  // lb1 (zero padding up to the template machine count is value-neutral: the reference itself evaluates 20-wide
+  // zero-padded tuples, lib/pfsp/Bound_simple.chpl:125-135)
+  int32_t* total = t->wide ? tw.total : t1.total;
+  int32_t* pj = t->wide ? tw.pj : t1.pj;
+  const int mp = t->wide ? tsb::PW_PSTRIDE : t1.mp, hs = tsb::half_stride(t->mt);
+  long long sum_all = 0, max_head = 0, max_tail = 0;
+  bool nonneg = true, tails_monotone = true;
+  for (int k = 0; k < machines; k++) {
+    (t->wide ? tw.min_heads : t1.min_heads)[k] = min_heads[k];
+    (t->wide ? tw.min_tails : t1.min_tails)[k] = min_tails[k];
+    max_head = std::max<long long>(max_head, min_heads[k]);
+    max_tail = std::max<long long>(max_tail, min_tails[k]);
+    nonneg &= min_heads[k] >= 0 && min_tails[k] >= 0;
+    if (k > 0) tails_monotone &= min_tails[k] <= min_tails[k - 1];
+    for (int j = 0; j < jobs; j++) {
+      const int32_t pv = p_times[k * jobs + j];
+      total[k] += pv;
+      pj[j * mp + k] = pv;
+      nonneg &= pv >= 0;
+      sum_all += pv;
+      if (!t->wide) t1.ph[j * hs + (k >> 1)] |= static_cast<uint32_t>(pv & 0xFFFF) << (16 * (k & 1));
+    }
+  }
+  // every intermediate of the bounds is <= sum of all processing times + largest head + largest tail
+  t->simd16 = !t->wide && nonneg && tails_monotone && sum_all + max_head + max_tail < tsb::PF_LANE_LIMIT &&
+              !std::getenv("TSB200_NO_SIMD16");
+  // lb2: Johnson tables in machine_pair_order
+  const uint32_t lag_max = t->wide ? tsb::PW_LAG_MAX : tsb::LB2_LAG_MAX;
+  bool fits = true;
+  for (int l = 0; l < nb_pairs; l++) {
+    const int i = mp_order[l];
+    if (i < 0 || i >= nb_pairs) {
+      t->valid = false;
+      continue;
+    }
+    const int a = mp0[i], b = mp1[i];
+    if (a < 0 || a >= machines || b < 0 || b >= machines) {
+      t->valid = false;
+      continue;
+    }
+    fits &= tsb::lb2_fits(min_tails[a], tsb::LB2_TAIL_MAX) && tsb::lb2_fits(min_tails[b], tsb::LB2_TAIL_MAX);
+    (t->wide ? tw.pair : t->lb2c.pair)[l] = tsb::lb2_pair_word(a, b, min_tails[a], min_tails[b]);
+    for (int j = 0; j < jobs; j++) {
+      const int job = johnson[i * jobs + j];
+      if (job < 0 || job >= jobs) {
+        t->valid = false;
+        continue;
+      }
+      const int pa = p_times[a * jobs + job], pb = p_times[b * jobs + job], lg = lags[i * jobs + job];
+      fits &= tsb::lb2_fits(pa, tsb::LB2_P_MAX) && tsb::lb2_fits(pb, tsb::LB2_P_MAX) && tsb::lb2_fits(lg, lag_max);
+      if (t->wide)
+        tw.jp[l * jobs + j] = tsb::pw_job_word(job, pa, pb, lg);
+      else
+        t->lb2c.jp[l * tsb::PF_MAXJ + j] = tsb::lb2_job_word(job, pa, pb, lg);
+    }
+  }
+  if (!fits) t->pairs = 0;  // values outside the Taillard range: no lb2 on this handle
+  const char* no_u = std::getenv("TSB200_NO_LB2U");
+  t->lb2u = t->valid && t->pairs > 0 && nb_pairs <= tsb::LB2U_PAIRS && t->mt <= 10 && t->simd16 &&
+            !(no_u && *no_u && *no_u != '0');
+  for (int l = 0; l < nb_pairs && t->lb2u; l++) {
+    const int i = mp_order[l], a = mp0[i], b = mp1[i];
+    t->tabu.mach[l] = tsb::lb2u_mach_word(a, b);
+    t->tabu.tails[l] = tsb::lb2u_tails_word(min_tails[a], min_tails[b]);
+    for (int j = 0; j < jobs; j++) {
+      const int job = johnson[i * jobs + j];
+      t->tabu.e[l * tsb::PF_MAXJ + j] = tsb::lb2u_entry(job, p_times[a * jobs + job], p_times[b * jobs + job],
+                                                        lags[i * jobs + job]);
+    }
+  }
+  return t;
+}
+
+// handle-level entry points of both handle types
+int register_host(Base* h, void* ptr, size_t bytes) {
+  if (!h) return TSB_EINVAL;
+  TSB_CUDA(cudaSetDevice(h->device));
+  return h->reg.add(ptr, bytes);
+}
+int unregister_host(Base* h, void* ptr) {
+  if (!h) return TSB_EINVAL;
+  TSB_CUDA(cudaSetDevice(h->device));
+  return h->reg.remove(ptr);
+}
+int set_xfer(Base* h, int mode) {
+  if (!h || mode < 0 || mode > 2) return TSB_EINVAL;
+  h->xfer = mode;
+  return TSB_OK;
+}
+int last_xfer(const Base* h) { return h ? h->last_xfer : TSB_EINVAL; }
+void* stream_of(const Base* h) { return h ? static_cast<void*>(h->stream) : nullptr; }
+int64_t pool_size(const Base* h) { return h ? h->pool.size : -1; }
+
+// the handle and the siblings it owns; each handle type frees its own device buffers in its destructor
+template <class H>
+void destroy(H* h) {
+  if (!h) return;
+  for (H*& x : h->sibling) {
+    destroy(x);
+    x = nullptr;
+  }
+  h->fini();
+  delete h;
+}
+
+// launches of the handle and of its siblings
+template <class H>
+uint64_t kernel_launches(const H* h) {
+  if (!h) return 0;
+  uint64_t n = h->launches;
+  for (const H* x : h->sibling)
+    if (x) n += x->launches;
+  return n;
+}
+
+// sibling `index` (1..3) of h, created by make(&slot) on first use and owned by h
+template <class H, class Make>
+int sibling_of(H* h, int index, H** sibling, Make&& make) {
+  if (!h || !sibling || index < 1 || index > static_cast<int>(std::size(h->sibling))) return TSB_EINVAL;
+  H*& s = h->sibling[index - 1];
+  if (!s)
+    if (const int rc = make(&s); rc != TSB_OK) return rc;
+  *sibling = s;
+  return TSB_OK;
+}
+
+// the pools of one tsb_*_pool_run_multi call: distinct handles of one kind (`same(h, h0)`) on one device, each
+// taking chunks of M parents
+template <class H, class Same>
+bool one_group(H* const* hs, int K, int M, Same&& same) {
+  for (int i = 0; i < K; i++) {
+    const H* h = hs[i];
+    if (!h || M > h->M_max || h->device != hs[0]->device || !same(*h, *hs[0])) return false;
+    for (int j = 0; j < i; j++)
+      if (hs[j] == h) return false;
+  }
+  return true;
+}
+
 void enable_peer(int a, int b) {
   if (a == b) return;
   int can = 0;
@@ -961,6 +1137,9 @@ void enable_peer(int a, int b) {
 
 // ============================================================================ handles
 struct tsb_nq : Base {
+  ~tsb_nq() {
+    if (d_fat) cudaFree(d_fat);
+  }
   tsb_nq* sibling[3] = {nullptr, nullptr, nullptr};  // further pools on the same device, owned by this handle (tsb_nq_sibling)
   int N = 0, g = 1;
   bool wide = false;  // MAX_QUEENS = 24 build (tsb_nq_create_wide): 25-byte tsb_nq_node24 records, one pool per launch
@@ -975,15 +1154,17 @@ struct tsb_nq : Base {
 };
 
 struct tsb_pfsp : Base {
+  ~tsb_pfsp() {
+    if (d_tab1) cudaFree(d_tab1);
+    if (d_wtab) cudaFree(d_wtab);
+    if (d_tabu) cudaFree(d_tabu);
+  }
   tsb_pfsp* sibling[3] = {nullptr, nullptr, nullptr};  // further pools on the same device, owned by this handle (tsb_pfsp_sibling)
-  int jobs = 0, machines = 0, pairs = 0, mt = 0;  // mt = template machine count (5, 10 or 20)
+  std::shared_ptr<const PfspPacked> tab;  // the tables and route, shared with the owner or the siblings
+  // device copies of tab's tables: t1 or tw, and tabu on the lb2u route
   tsb::PfspLb1Tables* d_tab1 = nullptr;
-  tsb::Lb2Const* lb2c = nullptr;  // packed Johnson tables, passed to the lb2 kernels by value (constant bank)
-  tsb::Lb2ConstU* lb2u = nullptr; // <= 10 machines: address of the shared-memory-resident table (tsb::Lb2TabU)
-  tsb::Lb2TabU* d_tabu = nullptr;
-  bool simd16 = false;  // lb1 / lb1_d children two per register (values < 2^16, min_tails non-increasing)
-  bool wide = false;    // MAX_JOBS = 50 build: 208-byte nodes, the general kernels of pfsp_wide.cuh
   tsb::PfspWideTables* d_wtab = nullptr;
+  tsb::Lb2TabU* d_tabu = nullptr;
   uint64_t slow_rounds = 0;
   std::vector<tsb_pfsp_node> h_chunk, h_kids;  // slow path scratch
   std::vector<int32_t> h_bounds;
@@ -1352,9 +1533,9 @@ int launch_lb2_mc(tsb_pfsp* h, const CT& C, const uint8_t* in, uint8_t* out, lon
 template <int M>
 int launch_lb2_m(tsb_pfsp* h, const uint8_t* in, uint8_t* out, long long count, int best, cudaStream_t s) {
   if constexpr (M <= 10) {
-    if (h->lb2u) return launch_lb2_mc<M>(h, *h->lb2u, in, out, count, best, s);
+    if (h->d_tabu) return launch_lb2_mc<M>(h, tsb::Lb2ConstU{h->d_tabu}, in, out, count, best, s);
   }
-  return launch_lb2_mc<M>(h, *h->lb2c, in, out, count, best, s);
+  return launch_lb2_mc<M>(h, h->tab->lb2c, in, out, count, best, s);
 }
 
 template <int KIND, int M>
@@ -1379,13 +1560,13 @@ int launch_wide_m(tsb_pfsp* h, int lb_kind, const uint8_t* in, uint8_t* out, lon
 int launch_pfsp(tsb_pfsp* h, int lb_kind, const uint8_t* in, uint8_t* out, long long count, int64_t best64,
                 cudaStream_t s) {
   const int best = clamp_best(best64);
-  return with_machines(h->mt, [&](auto mt) {
+  return with_machines(h->tab->mt, [&](auto mt) {
     constexpr int M = decltype(mt)::value;
-    if (h->wide) return launch_wide_m<M>(h, lb_kind, in, out, count, best, s);
+    if (h->tab->wide) return launch_wide_m<M>(h, lb_kind, in, out, count, best, s);
     if (lb_kind == TSB_LB1)
-      return h->simd16 ? launch_lb1_km<1, M, true>(h, in, out, count, s) : launch_lb1_km<1, M, false>(h, in, out, count, s);
+      return h->tab->simd16 ? launch_lb1_km<1, M, true>(h, in, out, count, s) : launch_lb1_km<1, M, false>(h, in, out, count, s);
     if (lb_kind == TSB_LB1_D)
-      return h->simd16 ? launch_lb1_km<0, M, true>(h, in, out, count, s) : launch_lb1_km<0, M, false>(h, in, out, count, s);
+      return h->tab->simd16 ? launch_lb1_km<0, M, true>(h, in, out, count, s) : launch_lb1_km<0, M, false>(h, in, out, count, s);
     return launch_lb2_m<M>(h, in, out, count, best, s);
   });
 }
@@ -1413,17 +1594,17 @@ int pfsp_expand_m(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const tsb::Exp
     };
     bool done = false;
     if constexpr (M <= 10) {
-      if (h->lb2u) {
-        rc = go(tsb::pfsp_expand_count_lb2_kernel<M, tsb::Lb2ConstU>, *h->lb2u);
+      if (h->d_tabu) {
+        rc = go(tsb::pfsp_expand_count_lb2_kernel<M, tsb::Lb2ConstU>, tsb::Lb2ConstU{h->d_tabu});
         done = true;
       }
     }
-    if (!done) rc = go(tsb::pfsp_expand_count_lb2_kernel<M, tsb::Lb2Const>, *h->lb2c);
+    if (!done) rc = go(tsb::pfsp_expand_count_lb2_kernel<M, tsb::Lb2Const>, h->tab->lb2c);
     if (rc != TSB_OK) return rc;
   } else {
     auto k1 = lb_kind == TSB_LB1
-                  ? (h->simd16 ? tsb::pfsp_expand_count_lb1_kernel<1, M, true> : tsb::pfsp_expand_count_lb1_kernel<1, M, false>)
-                  : (h->simd16 ? tsb::pfsp_expand_count_lb1_kernel<0, M, true> : tsb::pfsp_expand_count_lb1_kernel<0, M, false>);
+                  ? (h->tab->simd16 ? tsb::pfsp_expand_count_lb1_kernel<1, M, true> : tsb::pfsp_expand_count_lb1_kernel<1, M, false>)
+                  : (h->tab->simd16 ? tsb::pfsp_expand_count_lb1_kernel<0, M, true> : tsb::pfsp_expand_count_lb1_kernel<0, M, false>);
     const size_t smem1 = sizeof(tsb::Lb1CountSmem) + 128;
     rc = h->grid_for(k1, tsb::PF_THREADS, smem1, recs, tsb::PF_TILE, &g1);
     if (rc != TSB_OK) return rc;
@@ -1471,7 +1652,7 @@ int pfsp_expand_round(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const std:
   if (rc != TSB_OK) return rc;
   prm.epoch = ++ex.epoch;
   prm.best = best_launch;
-  rc = with_machines(h->mt, [&](auto mt) {
+  rc = with_machines(h->tab->mt, [&](auto mt) {
     return pfsp_expand_m<decltype(mt)::value>(h, lb_kind, arena, prm, children_d, s);
   });
   if (rc != TSB_OK) return rc;
@@ -1501,13 +1682,13 @@ int pfsp_expand_round(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const std:
   rc = launch_pfsp(h, lb_kind, h->d_in, h->d_out, n, *best, s);
   if (rc != TSB_OK) return rc;
   h->h_chunk.resize(static_cast<size_t>(n));
-  h->h_bounds.resize(static_cast<size_t>(n) * h->jobs);
+  h->h_bounds.resize(static_cast<size_t>(n) * h->tab->jobs);
   rc = h->copy_d2h(h->h_chunk.data(), h->d_in, static_cast<size_t>(n) * sizeof(tsb_pfsp_node), s);
-  if (rc == TSB_OK) rc = h->copy_d2h(h->h_bounds.data(), h->d_out, static_cast<size_t>(n) * h->jobs * 4, s);
+  if (rc == TSB_OK) rc = h->copy_d2h(h->h_bounds.data(), h->d_out, static_cast<size_t>(n) * h->tab->jobs * 4, s);
   if (rc != TSB_OK) return rc;
   h->h_kids.clear();
   uint64_t sol = 0;
-  pfsp_generate_children_host(h->jobs, h->h_chunk.data(), static_cast<int>(n), h->h_bounds.data(), best, &h->h_kids,
+  pfsp_generate_children_host(h->tab->jobs, h->h_chunk.data(), static_cast<int>(n), h->h_bounds.data(), best, &h->h_kids,
                               &sol);
   rc = h->copy_h2d(children_d, h->h_kids.data(), h->h_kids.size() * sizeof(tsb_pfsp_node), s);
   if (rc != TSB_OK) return rc;
@@ -1532,10 +1713,10 @@ int pfsp_rounds_grid(const tsb_pfsp* h, int lb_kind, int M) {
 // f(kernel): the persistent kernel of h's route for lb1 / lb1_d
 template <class F>
 int with_pfsp_rounds_kernel(const tsb_pfsp* h, int lb_kind, F&& f) {
-  return with_machines(h->mt, [&](auto mt) -> int {
+  return with_machines(h->tab->mt, [&](auto mt) -> int {
     constexpr int MT = decltype(mt)::value;
-    if (lb_kind == TSB_LB1) return h->simd16 ? f(tsb::pfsp_rounds_kernel<1, MT, true>) : f(tsb::pfsp_rounds_kernel<1, MT, false>);
-    return h->simd16 ? f(tsb::pfsp_rounds_kernel<0, MT, true>) : f(tsb::pfsp_rounds_kernel<0, MT, false>);
+    if (lb_kind == TSB_LB1) return h->tab->simd16 ? f(tsb::pfsp_rounds_kernel<1, MT, true>) : f(tsb::pfsp_rounds_kernel<1, MT, false>);
+    return h->tab->simd16 ? f(tsb::pfsp_rounds_kernel<0, MT, true>) : f(tsb::pfsp_rounds_kernel<0, MT, false>);
   });
 }
 constexpr size_t kPfRoundsSmem = sizeof(tsb::PfRoundsSmem) + 128;
@@ -1622,40 +1803,41 @@ struct PfspRounds {
   PfspRounds of_pool(int i) const { return {lb_kind, best + i}; }
 };
 
-// a handle with h's device, M_max and tables (its route included) and an empty pool; the device tables are copied
-// device to device, so none of the arrays h was created from is needed
-int pfsp_clone(const tsb_pfsp* h, tsb_pfsp** out) {
-  tsb_pfsp* c = new (std::nothrow) tsb_pfsp();
-  if (!c) return TSB_ENOMEM;
-  c->jobs = h->jobs;
-  c->machines = h->machines;
-  c->pairs = h->pairs;
-  c->mt = h->mt;
-  c->simd16 = h->simd16;
-  c->pool.set_format(sizeof(tsb_pfsp_node), tsb::PF_TILE, 2, h->jobs, h->pool.default_cap);
-  auto copy = [&]() -> int {
-    int rc = c->init(h->device, h->M_max, sizeof(tsb_pfsp_node), static_cast<size_t>(h->jobs) * 4);
-    if (rc != TSB_OK) return rc;
-    TSB_CUDA(cudaMalloc(&c->d_tab1, sizeof(tsb::PfspLb1Tables)));
-    TSB_CUDA(cudaMemcpyAsync(c->d_tab1, h->d_tab1, sizeof(tsb::PfspLb1Tables), cudaMemcpyDeviceToDevice, c->stream));
-    if (h->lb2c) {
-      c->lb2c = new (std::nothrow) tsb::Lb2Const(*h->lb2c);
-      if (!c->lb2c) return TSB_ENOMEM;
-    }
-    if (h->lb2u) {
-      TSB_CUDA(cudaMalloc(&c->d_tabu, sizeof(tsb::Lb2TabU)));
-      TSB_CUDA(cudaMemcpyAsync(c->d_tabu, h->d_tabu, sizeof(tsb::Lb2TabU), cudaMemcpyDeviceToDevice, c->stream));
-      c->lb2u = new (std::nothrow) tsb::Lb2ConstU{c->d_tabu};
-      if (!c->lb2u) return TSB_ENOMEM;
-    }
-    TSB_CUDA(cudaStreamSynchronize(c->stream));
+// A handle with chunks of up to M_max parents on `device`, an empty pool and the tables `tab` (its own, or its owner's
+// for a sibling).  Tables with an index out of range give TSB_EINVAL, after the errors of the device itself.
+int pfsp_open(int device, int M_max, std::shared_ptr<const PfspPacked> tab, tsb_pfsp** out) {
+  tsb_pfsp* h = new (std::nothrow) tsb_pfsp();
+  if (!h) return TSB_ENOMEM;
+  h->tab = std::move(tab);
+  const PfspPacked& t = *h->tab;
+  const size_t rec = t.wide ? tsb::PW_REC : sizeof(tsb_pfsp_node);
+  // (88-byte nodes: extents on even records start on a 16-byte boundary)
+  h->pool.set_format(rec, tsb::PF_TILE, 2, t.jobs, std::max<long long>(1LL << 20, 4LL * M_max * t.jobs));
+  int rc = h->init(device, M_max, rec, static_cast<size_t>(t.jobs) * 4);
+  if (rc == TSB_OK && !t.valid) rc = TSB_EINVAL;
+  auto upload = [h](auto** dst, const auto& src) -> int {
+    TSB_CUDA(cudaMalloc(dst, sizeof(src)));
+    TSB_CUDA(cudaMemcpyAsync(*dst, &src, sizeof(src), cudaMemcpyHostToDevice, h->stream));
+    TSB_CUDA(cudaStreamSynchronize(h->stream));
     return TSB_OK;
   };
-  if (const int rc = copy(); rc != TSB_OK) {
-    tsb_pfsp_destroy(c);
+  if (rc == TSB_OK) rc = t.wide ? upload(&h->d_wtab, t.tw) : upload(&h->d_tab1, t.t1);
+  if (rc == TSB_OK && t.lb2u) rc = upload(&h->d_tabu, t.tabu);
+  if (rc != TSB_OK) {
+    destroy(h);
     return rc;
   }
-  *out = c;
+  *out = h;
+  return TSB_OK;
+}
+
+// The checks of a PFSP entry point on its handle and bound: TSB_EINVAL for a null handle, an unknown bound or lb2 on
+// a handle without machine pairs.  `pool`: an entry point of the fused expand or the device pool, which exist for
+// 20 jobs only: TSB_EUNSUPPORTED first on a 50-job handle.
+int pfsp_check(const tsb_pfsp* h, bool pool, int lb_kind = TSB_LB1) {
+  if (!h) return TSB_EINVAL;
+  if (pool && h->tab->wide) return TSB_EUNSUPPORTED;
+  if (lb_kind < 0 || lb_kind > 2 || (lb_kind == TSB_LB2 && h->tab->pairs == 0)) return TSB_EINVAL;
   return TSB_OK;
 }
 
@@ -1824,8 +2006,7 @@ static int nq_create(tsb_nq** out, int device, bool wide, int N, int g, int M_ma
   h->pool.set_format(rec, tsb::NQ_TILE, 1, N, std::max<long long>(1LL << 22, 4LL * M_max * N));
   int rc = h->init(device, M_max, rec, static_cast<size_t>(N));
   if (rc != TSB_OK) {
-    h->fini();
-    delete h;
+    destroy(h);
     return rc;
   }
   *out = h;
@@ -1837,16 +2018,7 @@ int tsb_nq_create_wide(tsb_nq** out, int device, int max_queens, int N, int g, i
   return nq_create(out, device, true, N, g, M_max);
 }
 
-void tsb_nq_destroy(tsb_nq* h) {
-  if (!h) return;
-  for (tsb_nq*& x : h->sibling) {
-    if (x) tsb_nq_destroy(x);
-    x = nullptr;
-  }
-  h->fini();
-  if (h->d_fat) cudaFree(h->d_fat);
-  delete h;
-}
+void tsb_nq_destroy(tsb_nq* h) { destroy(h); }
 
 // ---- fused evaluate + generate_children, and the device-resident pool (SURVEY §8f rows 1, 3)
 int tsb_nq_expand_device(tsb_nq* h, const void* parents_d, int count, void* children_d, uint64_t* n_children,
@@ -1884,7 +2056,7 @@ int tsb_nq_pool_push(tsb_nq* h, const void* nodes, int64_t n) {
   return pool_push(*h, nodes, n, [h] { return nq_materialize(h); });
 }
 
-int64_t tsb_nq_pool_size(const tsb_nq* h) { return h ? h->pool.size : -1; }
+int64_t tsb_nq_pool_size(const tsb_nq* h) { return pool_size(h); }
 
 int tsb_nq_pool_step(tsb_nq* h, int m, int M, int64_t* n_parents, uint64_t* n_children, uint64_t* n_solutions) {
   if (!h || m < 1 || M < 1 || M > h->M_max || !n_parents || !n_children || !n_solutions) return TSB_EINVAL;
@@ -1902,13 +2074,7 @@ int tsb_nq_pool_run(tsb_nq* h, int m, int M, int64_t max_rounds, uint64_t* n_rou
 }
 
 int tsb_nq_sibling(tsb_nq* h, int index, tsb_nq** sibling) {
-  if (!h || !sibling || index < 1 || index >= tsb::LL_MAX_POOLS) return TSB_EINVAL;
-  if (!h->sibling[index - 1]) {
-    int rc = nq_create(&h->sibling[index - 1], h->device, h->wide, h->N, h->g, h->M_max);
-    if (rc != TSB_OK) return rc;
-  }
-  *sibling = h->sibling[index - 1];
-  return TSB_OK;
+  return sibling_of(h, index, sibling, [h](tsb_nq** s) { return nq_create(s, h->device, h->wide, h->N, h->g, h->M_max); });
 }
 
 int tsb_nq_pools_per_launch(const tsb_nq* h, int M) {
@@ -1918,13 +2084,8 @@ int tsb_nq_pools_per_launch(const tsb_nq* h, int M) {
 
 int tsb_nq_pool_run_multi(tsb_nq* const* handles, int n_pools, int m, int M, int64_t max_rounds, uint64_t* out) {
   if (!handles || n_pools < 1 || n_pools > tsb::LL_MAX_POOLS || m < 1 || M < 1 || max_rounds < 0 || !out) return TSB_EINVAL;
-  for (int i = 0; i < n_pools; i++) {
-    const tsb_nq* h = handles[i];
-    if (!h || M > h->M_max || h->device != handles[0]->device || h->N != handles[0]->N || h->wide != handles[0]->wide)
-      return TSB_EINVAL;
-    for (int j = 0; j < i; j++)
-      if (handles[j] == h) return TSB_EINVAL;
-  }
+  if (!one_group(handles, n_pools, M, [](const tsb_nq& h, const tsb_nq& h0) { return h.N == h0.N && h.wide == h0.wide; }))
+    return TSB_EINVAL;
   return pool_run_multi(NqRounds{}, handles, n_pools, m, M, max_rounds, out);
 }
 
@@ -1962,31 +2123,12 @@ int tsb_nq_evaluate_device(tsb_nq* h, const void* parents_d, int count, uint8_t*
   return launch_nq(h, static_cast<const uint8_t*>(parents_d), labels_d, count, s);
 }
 
-int tsb_nq_register_host(tsb_nq* h, void* ptr, size_t bytes) {
-  if (!h) return TSB_EINVAL;
-  TSB_CUDA(cudaSetDevice(h->device));
-  return h->reg.add(ptr, bytes);
-}
-int tsb_nq_unregister_host(tsb_nq* h, void* ptr) {
-  if (!h) return TSB_EINVAL;
-  TSB_CUDA(cudaSetDevice(h->device));
-  return h->reg.remove(ptr);
-}
-
-int tsb_nq_set_xfer(tsb_nq* h, int mode) {
-  if (!h || mode < 0 || mode > 2) return TSB_EINVAL;
-  h->xfer = mode;
-  return TSB_OK;
-}
-int tsb_nq_last_xfer(const tsb_nq* h) { return h ? h->last_xfer : TSB_EINVAL; }
-uint64_t tsb_nq_kernel_launches(const tsb_nq* h) {
-  if (!h) return 0;
-  uint64_t n = h->launches;
-  for (const tsb_nq* x : h->sibling)
-    if (x) n += x->launches;
-  return n;
-}
-void* tsb_nq_stream(const tsb_nq* h) { return h ? static_cast<void*>(h->stream) : nullptr; }
+int tsb_nq_register_host(tsb_nq* h, void* ptr, size_t bytes) { return register_host(h, ptr, bytes); }
+int tsb_nq_unregister_host(tsb_nq* h, void* ptr) { return unregister_host(h, ptr); }
+int tsb_nq_set_xfer(tsb_nq* h, int mode) { return set_xfer(h, mode); }
+int tsb_nq_last_xfer(const tsb_nq* h) { return last_xfer(h); }
+uint64_t tsb_nq_kernel_launches(const tsb_nq* h) { return kernel_launches(h); }
+void* tsb_nq_stream(const tsb_nq* h) { return stream_of(h); }
 int tsb_nq_max_queens(const tsb_nq* h) {
   if (!h) return TSB_EINVAL;
   return h->wide ? TSB_MAX_QUEENS_WIDE : TSB_MAX_QUEENS;
@@ -1996,126 +2138,8 @@ int tsb_nq_max_queens(const tsb_nq* h) {
 int tsb_pfsp_create(tsb_pfsp** out, int device, int jobs, int machines, int M_max, const int32_t* p_times,
                     const int32_t* min_heads, const int32_t* min_tails, int nb_pairs, const int32_t* johnson,
                     const int32_t* lags, const int32_t* mp0, const int32_t* mp1, const int32_t* mp_order) {
-  if (!out || !p_times || !min_heads || !min_tails || M_max < 1 || nb_pairs < 0) return TSB_EINVAL;
-  if (nb_pairs > 0 && (!johnson || !lags || !mp0 || !mp1 || !mp_order)) return TSB_EINVAL;
-  if (jobs != TSB_MAX_JOBS || machines < 1 || machines > TSB_MAX_MACHINES || nb_pairs > TSB_MAX_PAIRS)
-    return TSB_EUNSUPPORTED;
-  tsb_pfsp* h = new (std::nothrow) tsb_pfsp();
-  if (!h) return TSB_ENOMEM;
-  h->jobs = jobs;
-  h->machines = machines;
-  h->pairs = nb_pairs;
-  h->mt = machines <= 5 ? 5 : machines <= 10 ? 10 : 20;
-  // (88-byte nodes: extents on even records start on a 16-byte boundary)
-  h->pool.set_format(sizeof(tsb_pfsp_node), tsb::PF_TILE, 2, jobs, std::max<long long>(1LL << 20, 4LL * M_max * jobs));
-  int rc = h->init(device, M_max, sizeof(tsb_pfsp_node), static_cast<size_t>(jobs) * 4);
-  // tables -> device blob (zero padding up to the template machine count is value-neutral:
-  // the reference itself evaluates 20-wide zero-padded tuples, lib/pfsp/Bound_simple.chpl:125-135)
-  std::vector<tsb::PfspLb1Tables> t1v(1);
-  tsb::PfspLb1Tables& t1 = t1v[0];
-  std::memset(&t1, 0, sizeof(t1));
-  const int mp = tsb::row_stride(h->mt);
-  t1.jobs = jobs;
-  t1.machines = machines;
-  t1.pairs = nb_pairs;
-  t1.mp = mp;
-  long long sum_all = 0, max_head = 0, max_tail = 0;
-  bool nonneg = true, tails_monotone = true;
-  const int hs = tsb::half_stride(h->mt);
-  for (int k = 0; k < machines; k++) {
-    t1.min_heads[k] = min_heads[k];
-    t1.min_tails[k] = min_tails[k];
-    max_head = std::max<long long>(max_head, min_heads[k]);
-    max_tail = std::max<long long>(max_tail, min_tails[k]);
-    nonneg &= min_heads[k] >= 0 && min_tails[k] >= 0;
-    if (k > 0) tails_monotone &= min_tails[k] <= min_tails[k - 1];
-    for (int j = 0; j < jobs; j++) {
-      const int32_t pv = p_times[k * jobs + j];
-      t1.total[k] += pv;
-      t1.pj[j * mp + k] = pv;
-      nonneg &= pv >= 0;
-      sum_all += pv;
-      t1.ph[j * hs + (k >> 1)] |= static_cast<uint32_t>(pv & 0xFFFF) << (16 * (k & 1));
-    }
-  }
-  // every intermediate of the bounds is <= sum of all processing times + largest head + largest tail
-  h->simd16 = nonneg && tails_monotone && sum_all + max_head + max_tail < 65536 && !std::getenv("TSB200_NO_SIMD16");
-  // lb2: packed Johnson tables in machine_pair_order (tsb::Lb2Const); value ranges checked, indices checked
-  bool bad = false, wide = false;
-  if (nb_pairs > 0) {
-    h->lb2c = new (std::nothrow) tsb::Lb2Const();
-    if (!h->lb2c) rc = TSB_ENOMEM;
-  }
-  for (int l = 0; l < nb_pairs && h->lb2c; l++) {
-    const int i = mp_order[l];
-    if (i < 0 || i >= nb_pairs) {
-      bad = true;
-      continue;
-    }
-    const int a = mp0[i], b = mp1[i];
-    if (a < 0 || a >= machines || b < 0 || b >= machines) {
-      bad = true;
-      continue;
-    }
-    wide |= min_tails[a] < 0 || min_tails[a] > 2047 || min_tails[b] < 0 || min_tails[b] > 2047;
-    h->lb2c->pair[l] = static_cast<uint32_t>(a) | static_cast<uint32_t>(b) << 5 |
-                       static_cast<uint32_t>(min_tails[a] & 2047) << 10 | static_cast<uint32_t>(min_tails[b] & 2047) << 21;
-    for (int j = 0; j < jobs; j++) {
-      const int job = johnson[i * jobs + j];
-      if (job < 0 || job >= jobs) {
-        bad = true;
-        continue;
-      }
-      const int pa = p_times[a * jobs + job], pb = p_times[b * jobs + job], lg = lags[i * jobs + job];
-      wide |= pa < 0 || pa > 127 || pb < 0 || pb > 127 || lg < 0 || lg > 8191;
-      h->lb2c->jp[l * tsb::PF_MAXJ + j] = static_cast<uint32_t>(job) | static_cast<uint32_t>(pa & 127) << 5 |
-                                          static_cast<uint32_t>(pb & 127) << 12 | static_cast<uint32_t>(lg & 8191) << 19;
-    }
-  }
-  // one-word-per-use table for the lb2 kernels of instances with <= 10 machines (env TSB200_NO_LB2U=1 disables)
-  std::vector<tsb::Lb2TabU> tuv;
-  const char* no_u = std::getenv("TSB200_NO_LB2U");
-  if (rc == TSB_OK && !bad && !wide && nb_pairs > 0 && nb_pairs <= tsb::LB2U_PAIRS && h->mt <= 10 && h->simd16 &&
-      !(no_u && *no_u && *no_u != '0')) {
-    tuv.resize(1);
-    tsb::Lb2TabU& tu = tuv[0];
-    std::memset(&tu, 0, sizeof(tu));
-    for (int l = 0; l < nb_pairs; l++) {
-      const int i = mp_order[l], a = mp0[i], b = mp1[i];
-      tu.mach[l] = static_cast<uint32_t>(a) | static_cast<uint32_t>(b) << 8;
-      tu.tails[l] = static_cast<uint32_t>(min_tails[a]) | static_cast<uint32_t>(min_tails[b]) << 16;
-      for (int j = 0; j < jobs; j++) {
-        const int job = johnson[i * jobs + j];
-        const int pa = p_times[a * jobs + job], pb = p_times[b * jobs + job], lg = lags[i * jobs + job];
-        tu.e[l * tsb::PF_MAXJ + j] = make_uint4(1u << job, static_cast<uint32_t>(pa + lg),
-                                                 static_cast<uint32_t>(pa - pb), 0u);
-      }
-    }
-  }
-  if (rc == TSB_OK && bad) rc = TSB_EINVAL;
-  if (rc == TSB_OK && wide) {  // processing times > 127 / lags > 8191 (outside the Taillard range): no lb2 on this handle
-    delete h->lb2c;
-    h->lb2c = nullptr;
-    h->pairs = 0;
-  }
-  auto upload = [&]() -> int {
-    TSB_CUDA(cudaMalloc(&h->d_tab1, sizeof(t1)));
-    TSB_CUDA(cudaMemcpyAsync(h->d_tab1, &t1, sizeof(t1), cudaMemcpyHostToDevice, h->stream));
-    if (!tuv.empty()) {
-      TSB_CUDA(cudaMalloc(&h->d_tabu, sizeof(tsb::Lb2TabU)));
-      TSB_CUDA(cudaMemcpyAsync(h->d_tabu, tuv.data(), sizeof(tsb::Lb2TabU), cudaMemcpyHostToDevice, h->stream));
-      h->lb2u = new (std::nothrow) tsb::Lb2ConstU{h->d_tabu};
-    }
-    TSB_CUDA(cudaStreamSynchronize(h->stream));
-    return TSB_OK;
-  };
-  if (rc == TSB_OK) rc = upload();
-  if (rc != TSB_OK) {
-    tsb_pfsp_destroy(h);
-    return rc;
-  }
-  *out = h;
-  return TSB_OK;
+  return tsb_pfsp_create_wide(out, device, TSB_MAX_JOBS, jobs, machines, M_max, p_times, min_heads, min_tails, nb_pairs,
+                              johnson, lags, mp0, mp1, mp_order);
 }
 
 // The reference built with MAX_JOBS = max_jobs (lib/pfsp/PFSP_node.chpl:7): 20 = tsb_pfsp_create; 50 = 208-byte nodes,
@@ -2124,99 +2148,22 @@ int tsb_pfsp_create(tsb_pfsp** out, int device, int jobs, int machines, int M_ma
 int tsb_pfsp_create_wide(tsb_pfsp** out, int device, int max_jobs, int jobs, int machines, int M_max, const int32_t* p_times,
                          const int32_t* min_heads, const int32_t* min_tails, int nb_pairs, const int32_t* johnson,
                          const int32_t* lags, const int32_t* mp0, const int32_t* mp1, const int32_t* mp_order) {
-  if (max_jobs == TSB_MAX_JOBS)
-    return tsb_pfsp_create(out, device, jobs, machines, M_max, p_times, min_heads, min_tails, nb_pairs, johnson, lags, mp0,
-                           mp1, mp_order);
   if (!out || !p_times || !min_heads || !min_tails || M_max < 1 || nb_pairs < 0) return TSB_EINVAL;
   if (nb_pairs > 0 && (!johnson || !lags || !mp0 || !mp1 || !mp_order)) return TSB_EINVAL;
-  if (max_jobs != TSB_MAX_JOBS_WIDE || jobs != max_jobs || machines < 1 || machines > TSB_MAX_MACHINES ||
-      nb_pairs > TSB_MAX_PAIRS)
+  if ((max_jobs != TSB_MAX_JOBS && max_jobs != TSB_MAX_JOBS_WIDE) || jobs != max_jobs || machines < 1 ||
+      machines > TSB_MAX_MACHINES || nb_pairs > TSB_MAX_PAIRS)
     return TSB_EUNSUPPORTED;
-  tsb_pfsp* h = new (std::nothrow) tsb_pfsp();
-  if (!h) return TSB_ENOMEM;
-  h->jobs = jobs;
-  h->machines = machines;
-  h->pairs = nb_pairs;
-  h->wide = true;
-  h->mt = machines <= 5 ? 5 : machines <= 10 ? 10 : 20;
-  int rc = h->init(device, M_max, tsb::PW_REC, static_cast<size_t>(jobs) * 4);
-  std::vector<tsb::PfspWideTables> tv(1);
-  tsb::PfspWideTables& t = tv[0];
-  std::memset(&t, 0, sizeof(t));
-  t.jobs = jobs;
-  t.machines = machines;
-  t.pairs = nb_pairs;
-  bool bad = false, wide_values = false;
-  for (int k = 0; k < machines; k++) {
-    t.min_heads[k] = min_heads[k];
-    t.min_tails[k] = min_tails[k];
-    for (int j = 0; j < jobs; j++) {
-      const int32_t pv = p_times[k * jobs + j];
-      t.total[k] += pv;
-      t.pj[j * tsb::PW_PSTRIDE + k] = pv;
-    }
-  }
-  for (int l = 0; l < nb_pairs; l++) {
-    const int i = mp_order[l];
-    if (i < 0 || i >= nb_pairs) {
-      bad = true;
-      continue;
-    }
-    const int a = mp0[i], b = mp1[i];
-    if (a < 0 || a >= machines || b < 0 || b >= machines) {
-      bad = true;
-      continue;
-    }
-    wide_values |= min_tails[a] < 0 || min_tails[a] > 2047 || min_tails[b] < 0 || min_tails[b] > 2047;
-    t.pair[l] = static_cast<uint32_t>(a) | static_cast<uint32_t>(b) << 5 | static_cast<uint32_t>(min_tails[a] & 2047) << 10 |
-                static_cast<uint32_t>(min_tails[b] & 2047) << 21;
-    for (int j = 0; j < jobs; j++) {
-      const int job = johnson[i * jobs + j];
-      if (job < 0 || job >= jobs) {
-        bad = true;
-        continue;
-      }
-      const int pa = p_times[a * jobs + job], pb = p_times[b * jobs + job], lg = lags[i * jobs + job];
-      wide_values |= pa < 0 || pa > 127 || pb < 0 || pb > 127 || lg < 0 || lg > 4095;
-      t.jp[l * jobs + j] = static_cast<uint32_t>(job) | static_cast<uint32_t>(pa & 127) << 6 | static_cast<uint32_t>(pb & 127) << 13 |
-                           static_cast<uint32_t>(lg & 4095) << 20;
-    }
-  }
-  if (rc == TSB_OK && bad) rc = TSB_EINVAL;
-  if (rc == TSB_OK && wide_values) h->pairs = 0;  // values outside the Taillard range: no lb2 on this handle
-  auto upload = [&]() -> int {
-    TSB_CUDA(cudaMalloc(&h->d_wtab, sizeof(t)));
-    TSB_CUDA(cudaMemcpyAsync(h->d_wtab, &t, sizeof(t), cudaMemcpyHostToDevice, h->stream));
-    TSB_CUDA(cudaStreamSynchronize(h->stream));
-    return TSB_OK;
-  };
-  if (rc == TSB_OK) rc = upload();
-  if (rc != TSB_OK) {
-    tsb_pfsp_destroy(h);
-    return rc;
-  }
-  *out = h;
-  return TSB_OK;
+  return pfsp_open(device, M_max,
+                   pfsp_pack(max_jobs, jobs, machines, p_times, min_heads, min_tails, nb_pairs, johnson, lags, mp0, mp1,
+                             mp_order),
+                   out);
 }
 
-void tsb_pfsp_destroy(tsb_pfsp* h) {
-  if (!h) return;
-  for (tsb_pfsp*& x : h->sibling) {
-    if (x) tsb_pfsp_destroy(x);
-    x = nullptr;
-  }
-  h->fini();
-  if (h->d_tab1) cudaFree(h->d_tab1);
-  if (h->d_wtab) cudaFree(h->d_wtab);
-  delete h->lb2c;
-  delete h->lb2u;
-  if (h->d_tabu) cudaFree(h->d_tabu);
-  delete h;
-}
+void tsb_pfsp_destroy(tsb_pfsp* h) { destroy(h); }
 
 int tsb_pfsp_evaluate(tsb_pfsp* h, int lb_kind, const void* parents, int count, int64_t best, int32_t* bounds) {
-  if (!h || count < 0 || count > h->M_max || lb_kind < 0 || lb_kind > 2) return TSB_EINVAL;
-  if (lb_kind == TSB_LB2 && h->pairs == 0) return TSB_EINVAL;
+  if (int rc = pfsp_check(h, false, lb_kind); rc != TSB_OK) return rc;
+  if (count < 0 || count > h->M_max) return TSB_EINVAL;
   if (count == 0) return TSB_OK;
   if (!parents || !bounds) return TSB_EINVAL;
   TSB_CUDA(cudaSetDevice(h->device));
@@ -2228,8 +2175,8 @@ int tsb_pfsp_evaluate(tsb_pfsp* h, int lb_kind, const void* parents, int count, 
 
 int tsb_pfsp_evaluate_device(tsb_pfsp* h, int lb_kind, const void* parents_d, int count, int64_t best,
                              int32_t* bounds_d, void* stream) {
-  if (!h || count < 0 || lb_kind < 0 || lb_kind > 2) return TSB_EINVAL;
-  if (lb_kind == TSB_LB2 && h->pairs == 0) return TSB_EINVAL;
+  if (int rc = pfsp_check(h, false, lb_kind); rc != TSB_OK) return rc;
+  if (count < 0) return TSB_EINVAL;
   if (count == 0) return TSB_OK;
   if (!parents_d || !bounds_d) return TSB_EINVAL;
   if ((reinterpret_cast<uintptr_t>(parents_d) | reinterpret_cast<uintptr_t>(bounds_d)) & 15) return TSB_EALIGN;
@@ -2239,44 +2186,25 @@ int tsb_pfsp_evaluate_device(tsb_pfsp* h, int lb_kind, const void* parents_d, in
                      count, best, s);
 }
 
-int tsb_pfsp_register_host(tsb_pfsp* h, void* ptr, size_t bytes) {
-  if (!h) return TSB_EINVAL;
-  TSB_CUDA(cudaSetDevice(h->device));
-  return h->reg.add(ptr, bytes);
-}
-int tsb_pfsp_unregister_host(tsb_pfsp* h, void* ptr) {
-  if (!h) return TSB_EINVAL;
-  TSB_CUDA(cudaSetDevice(h->device));
-  return h->reg.remove(ptr);
-}
-
-int tsb_pfsp_set_xfer(tsb_pfsp* h, int mode) {
-  if (!h || mode < 0 || mode > 2) return TSB_EINVAL;
-  h->xfer = mode;
-  return TSB_OK;
-}
-int tsb_pfsp_last_xfer(const tsb_pfsp* h) { return h ? h->last_xfer : TSB_EINVAL; }
-uint64_t tsb_pfsp_kernel_launches(const tsb_pfsp* h) {
-  if (!h) return 0;
-  uint64_t n = h->launches;
-  for (const tsb_pfsp* x : h->sibling)
-    if (x) n += x->launches;
-  return n;
-}
-void* tsb_pfsp_stream(const tsb_pfsp* h) { return h ? static_cast<void*>(h->stream) : nullptr; }
+int tsb_pfsp_register_host(tsb_pfsp* h, void* ptr, size_t bytes) { return register_host(h, ptr, bytes); }
+int tsb_pfsp_unregister_host(tsb_pfsp* h, void* ptr) { return unregister_host(h, ptr); }
+int tsb_pfsp_set_xfer(tsb_pfsp* h, int mode) { return set_xfer(h, mode); }
+int tsb_pfsp_last_xfer(const tsb_pfsp* h) { return last_xfer(h); }
+uint64_t tsb_pfsp_kernel_launches(const tsb_pfsp* h) { return kernel_launches(h); }
+void* tsb_pfsp_stream(const tsb_pfsp* h) { return stream_of(h); }
 
 uint64_t tsb_pfsp_slow_rounds(const tsb_pfsp* h) { return h ? h->slow_rounds : 0; }
 
 int tsb_pfsp_route(const tsb_pfsp* h) {
   if (!h) return TSB_EINVAL;
-  return h->mt | (h->simd16 ? TSB_ROUTE_SIMD16 : 0) | (h->pairs > 0 ? TSB_ROUTE_LB2 : 0) | (h->lb2u ? TSB_ROUTE_LB2U : 0);
+  const PfspPacked& t = *h->tab;
+  return t.mt | (t.simd16 ? TSB_ROUTE_SIMD16 : 0) | (t.pairs > 0 ? TSB_ROUTE_LB2 : 0) | (t.lb2u ? TSB_ROUTE_LB2U : 0);
 }
 
 int tsb_pfsp_expand_device(tsb_pfsp* h, int lb_kind, const void* parents_d, int count, int64_t* best,
                            void* children_d, uint64_t* n_children, uint64_t* n_solutions, void* stream) {
-  if (h && h->wide) return TSB_EUNSUPPORTED;  // (the fused expand / device pool exist for MAX_JOBS = 20 only)
-  if (!h || count < 0 || lb_kind < 0 || lb_kind > 2 || !best || !n_children || !n_solutions) return TSB_EINVAL;
-  if (lb_kind == TSB_LB2 && h->pairs == 0) return TSB_EINVAL;
+  if (int rc = pfsp_check(h, true, lb_kind); rc != TSB_OK) return rc;
+  if (count < 0 || !best || !n_children || !n_solutions) return TSB_EINVAL;
   *n_children = *n_solutions = 0;
   if (count == 0) return TSB_OK;
   if (!parents_d || !children_d || count > h->M_max) return TSB_EINVAL;
@@ -2294,10 +2222,8 @@ int tsb_pfsp_expand_device(tsb_pfsp* h, int lb_kind, const void* parents_d, int 
 
 int tsb_pfsp_expand(tsb_pfsp* h, int lb_kind, const void* parents, int count, int64_t* best, void* children,
                     uint64_t capacity, uint64_t* n_children, uint64_t* n_solutions) {
-  if (h && h->wide) return TSB_EUNSUPPORTED;  // (the fused expand / device pool exist for MAX_JOBS = 20 only)
-  if (!h || count < 0 || count > h->M_max || lb_kind < 0 || lb_kind > 2 || !best || !n_children || !n_solutions)
-    return TSB_EINVAL;
-  if (lb_kind == TSB_LB2 && h->pairs == 0) return TSB_EINVAL;
+  if (int rc = pfsp_check(h, true, lb_kind); rc != TSB_OK) return rc;
+  if (count < 0 || count > h->M_max || !best || !n_children || !n_solutions) return TSB_EINVAL;
   *n_children = *n_solutions = 0;
   if (count == 0) return TSB_OK;
   if (!parents || !children) return TSB_EINVAL;
@@ -2308,20 +2234,17 @@ int tsb_pfsp_expand(tsb_pfsp* h, int lb_kind, const void* parents, int count, in
 }
 
 int tsb_pfsp_pool_push(tsb_pfsp* h, const void* nodes, int64_t n) {
-  if (h && h->wide) return TSB_EUNSUPPORTED;  // (the fused expand / device pool exist for MAX_JOBS = 20 only)
-  if (!h || n < 0 || (n && !nodes)) return TSB_EINVAL;
+  if (int rc = pfsp_check(h, true); rc != TSB_OK) return rc;
+  if (n < 0 || (n && !nodes)) return TSB_EINVAL;
   return pool_push(*h, nodes, n, pfsp_plain);
 }
 
-int64_t tsb_pfsp_pool_size(const tsb_pfsp* h) { return h ? h->pool.size : -1; }
+int64_t tsb_pfsp_pool_size(const tsb_pfsp* h) { return pool_size(h); }
 
 int tsb_pfsp_pool_step(tsb_pfsp* h, int lb_kind, int m, int M, int64_t* best, int64_t* n_parents,
                        uint64_t* n_children, uint64_t* n_solutions) {
-  if (h && h->wide) return TSB_EUNSUPPORTED;  // (the fused expand / device pool exist for MAX_JOBS = 20 only)
-  if (!h || lb_kind < 0 || lb_kind > 2 || m < 1 || M < 1 || M > h->M_max || !best || !n_parents || !n_children ||
-      !n_solutions)
-    return TSB_EINVAL;
-  if (lb_kind == TSB_LB2 && h->pairs == 0) return TSB_EINVAL;
+  if (int rc = pfsp_check(h, true, lb_kind); rc != TSB_OK) return rc;
+  if (m < 1 || M < 1 || M > h->M_max || !best || !n_parents || !n_children || !n_solutions) return TSB_EINVAL;
   return pool_step(*h, m, M, n_parents, n_children, n_solutions, pfsp_plain,
                    [h, lb_kind, best](auto arena, const auto& pieces, auto kids, auto nc, auto ns) {
                      return pfsp_expand_round(h, lb_kind, arena, pieces, kids, h->stream, best, nc, ns, /*early=*/true);
@@ -2329,7 +2252,7 @@ int tsb_pfsp_pool_step(tsb_pfsp* h, int lb_kind, int m, int M, int64_t* best, in
 }
 
 int tsb_pfsp_pool_steal(tsb_pfsp* victim, tsb_pfsp* thief, int m, int64_t* n_stolen) {
-  if (!victim || !thief || victim == thief || m < 1 || !n_stolen || victim->jobs != thief->jobs) return TSB_EINVAL;
+  if (!victim || !thief || victim == thief || m < 1 || !n_stolen || victim->tab->jobs != thief->tab->jobs) return TSB_EINVAL;
   return pool_steal(*victim, *thief, m, n_stolen, pfsp_plain);
 }
 
@@ -2340,28 +2263,19 @@ int tsb_pfsp_pool_drain(tsb_pfsp* h, void* nodes, int64_t capacity, int64_t* n) 
 
 int tsb_pfsp_pool_run(tsb_pfsp* h, int lb_kind, int m, int M, int64_t max_rounds, int64_t* best, uint64_t* n_rounds,
                       uint64_t* n_parents, uint64_t* n_children, uint64_t* n_solutions) {
-  if (h && h->wide) return TSB_EUNSUPPORTED;  // (the fused expand / device pool exist for MAX_JOBS = 20 only)
-  if (!h || lb_kind < 0 || lb_kind > 2 || m < 1 || M < 1 || M > h->M_max || max_rounds < 0 || !best || !n_rounds ||
-      !n_parents || !n_children || !n_solutions)
+  if (int rc = pfsp_check(h, true, lb_kind); rc != TSB_OK) return rc;
+  if (m < 1 || M < 1 || M > h->M_max || max_rounds < 0 || !best || !n_rounds || !n_parents || !n_children || !n_solutions)
     return TSB_EINVAL;
-  if (lb_kind == TSB_LB2 && h->pairs == 0) return TSB_EINVAL;
   return pool_run(PfspRounds{lb_kind, best}, h, m, M, max_rounds, n_rounds, n_parents, n_children, n_solutions);
 }
 
 int tsb_pfsp_sibling(tsb_pfsp* h, int index, tsb_pfsp** sibling) {
-  if (h && h->wide) return TSB_EUNSUPPORTED;  // (the device pool exists for MAX_JOBS = 20 only)
-  if (!h || !sibling || index < 1 || index >= tsb::PFR_MAX_POOLS) return TSB_EINVAL;
-  if (!h->sibling[index - 1]) {
-    TSB_CUDA(cudaSetDevice(h->device));
-    int rc = pfsp_clone(h, &h->sibling[index - 1]);
-    if (rc != TSB_OK) return rc;
-  }
-  *sibling = h->sibling[index - 1];
-  return TSB_OK;
+  if (int rc = pfsp_check(h, true); rc != TSB_OK) return rc;
+  return sibling_of(h, index, sibling, [h](tsb_pfsp** s) { return pfsp_open(h->device, h->M_max, h->tab, s); });
 }
 
 int tsb_pfsp_pools_per_launch(const tsb_pfsp* h, int lb_kind, int M) {
-  if (!h || h->wide || M < 1 || M > h->M_max) return 1;
+  if (pfsp_check(h, true) != TSB_OK || M < 1 || M > h->M_max) return 1;
   if (cudaSetDevice(h->device) != cudaSuccess) {
     (void)cudaGetLastError();
     return 1;
@@ -2375,18 +2289,12 @@ int tsb_pfsp_pool_run_multi(tsb_pfsp* const* handles, int n_pools, int lb_kind, 
   if (!handles || n_pools < 1 || n_pools > tsb::PFR_MAX_POOLS || lb_kind < 0 || lb_kind > 2 || m < 1 || M < 1 ||
       max_rounds < 0 || !best || !out)
     return TSB_EINVAL;
-  for (int i = 0; i < n_pools; i++) {
-    if (!handles[i]) return TSB_EINVAL;
-    if (handles[i]->wide) return TSB_EUNSUPPORTED;  // (the device pool exists for MAX_JOBS = 20 only)
-  }
-  const tsb_pfsp* h0 = handles[0];
-  for (int i = 0; i < n_pools; i++) {
-    const tsb_pfsp* h = handles[i];
-    if (M > h->M_max || h->device != h0->device || tsb_pfsp_route(h) != tsb_pfsp_route(h0)) return TSB_EINVAL;
-    for (int j = 0; j < i; j++)
-      if (handles[j] == h) return TSB_EINVAL;
-  }
-  if (lb_kind == TSB_LB2 && h0->pairs == 0) return TSB_EINVAL;
+  for (int i = 0; i < n_pools; i++)
+    if (int rc = pfsp_check(handles[i], true); rc != TSB_OK) return rc;
+  if (!one_group(handles, n_pools, M,
+                 [](const tsb_pfsp& h, const tsb_pfsp& h0) { return tsb_pfsp_route(&h) == tsb_pfsp_route(&h0); }))
+    return TSB_EINVAL;
+  if (int rc = pfsp_check(handles[0], true, lb_kind); rc != TSB_OK) return rc;
   return pool_run_multi(PfspRounds{lb_kind, best}, handles, n_pools, m, M, max_rounds, out);
 }
 

@@ -5,6 +5,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 PKG_DIR = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB_PATH = os.environ.get("TSB200_LIB") or os.path.join(PKG_DIR, "libtsb200.so")  # (TSB200_LIB: A/B builds)
 
@@ -170,3 +172,79 @@ def lib() -> C.CDLL:
 def check(code: int, where: str) -> None:
     if code != OK:
         raise TsbError(code, where)
+
+
+class Evaluator:
+    """What NQueensEvaluator and PfspEvaluator share: the handle's lifecycle and the entry points that take only the
+    handle, called as f"{_abi}_<name>" (tsb_nq_* or tsb_pfsp_*)"""
+
+    _abi = ""
+    _h = C.c_void_p()
+    _owner = None  # a sibling's handle belongs to the evaluator it came from
+
+    def _fn(self, name: str):
+        return getattr(lib(), f"{self._abi}_{name}")
+
+    def _check(self, name: str, *args) -> None:
+        check(self._fn(name)(self._h, *args), f"{self._abi}_{name}")
+
+    def close(self):
+        if self._h and self._owner is None:
+            self._fn("destroy")(self._h)
+        self._h = C.c_void_p()
+
+    __del__ = close
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def set_xfer(self, mode: int):
+        self._check("set_xfer", mode)
+
+    def register_host(self, arr: np.ndarray) -> None:
+        """page-lock + map a long-lived host array (the driver's chunk arrays, allocated once per search) so that
+        evaluate_gpu works on it in place; the array must outlive the evaluator or be unregistered"""
+        self._check("register_host", arr.ctypes.data, arr.nbytes)
+
+    def unregister_host(self, arr: np.ndarray) -> None:
+        self._check("unregister_host", arr.ctypes.data)
+
+    @property
+    def kernel_launches(self) -> int:
+        return int(self._fn("kernel_launches")(self._h))
+
+    @property
+    def last_xfer(self) -> int:
+        """route of the last evaluate call: XFER_ROUTE_ZEROCOPY | _PIPELINED | _IN_STAGED | _OUT_STAGED bits"""
+        r = int(self._fn("last_xfer")(self._h))
+        check(min(r, 0), f"{self._abi}_last_xfer")
+        return r
+
+    @property
+    def stream(self) -> int:
+        """the handle's cudaStream_t (pool / expand / host-buffer entry points launch on it)"""
+        return int(self._fn("stream")(self._h) or 0)
+
+    @property
+    def pool_size(self) -> int:
+        return int(self._fn("pool_size")(self._h))
+
+    @property
+    def pool_dtype(self) -> np.dtype:
+        """the records of the device pool"""
+        return self.node_dtype
+
+    def pool_steal_from(self, victim: "Evaluator", m: int) -> int:
+        got = C.c_int64(0)
+        check(self._fn("pool_steal")(victim._h, self._h, m, C.byref(got)), f"{self._abi}_pool_steal")
+        return int(got.value)
+
+    def pool_drain(self) -> np.ndarray:
+        n = self.pool_size
+        out = np.empty(max(n, 1), dtype=self.pool_dtype)
+        got = C.c_int64(0)
+        self._check("pool_drain", out.ctypes.data, n, C.byref(got))
+        return out[: got.value].copy()

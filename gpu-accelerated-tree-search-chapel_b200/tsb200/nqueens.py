@@ -5,7 +5,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import MAX_QUEENS, MAX_QUEENS_WIDE, SearchStats, check, lib
+from ._lib import MAX_QUEENS, MAX_QUEENS_WIDE, Evaluator, SearchStats, check, lib
 
 # lib/nqueens/NQueens_node.chpl:9-11
 NQ_NODE_DTYPE = np.dtype([("depth", np.uint8), ("board", np.uint8, (MAX_QUEENS,))])
@@ -20,12 +20,13 @@ def nq_node_dtype(N: int) -> np.dtype:
     return NQ_NODE_DTYPE if N <= MAX_QUEENS else NQ_NODE24_DTYPE
 
 
-class NQueensEvaluator:
+class NQueensEvaluator(Evaluator):
     """Owns what `on device var parents_d, labels_d` owns in the reference (nqueens_gpu_chpl.chpl:194-195).
     N > 20, or max_queens=24 for any N, creates a MAX_QUEENS = 24 handle (tsb_nq_create_wide): its nodes are
     NQ_NODE24_DTYPE records (`node_dtype`), and its device pools run one pool per launch of the persistent kernel."""
 
     wide, node_dtype = False, NQ_NODE_DTYPE  # (an object that wraps a tsb_nq_create handle)
+    _abi = "tsb_nq"
 
     def __init__(self, N: int, g: int = 1, M: int = 50000, device: int = 0, max_queens: int | None = None):
         self.N, self.g, self.M, self.device = N, g, M, device
@@ -38,46 +39,6 @@ class NQueensEvaluator:
             check(lib().tsb_nq_create_wide(C.byref(self._h), device, max_queens, N, g, M), "tsb_nq_create_wide")
         else:
             check(lib().tsb_nq_create(C.byref(self._h), device, N, g, M), "tsb_nq_create")
-
-    def close(self):
-        if self._h:
-            lib().tsb_nq_destroy(self._h)
-            self._h = C.c_void_p()
-
-    __del__ = close
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
-
-    def set_xfer(self, mode: int):
-        check(lib().tsb_nq_set_xfer(self._h, mode), "tsb_nq_set_xfer")
-
-    def register_host(self, arr: np.ndarray) -> None:
-        """page-lock + map a long-lived host array (the driver's `parents` / `labels`, allocated once per search)
-        so that evaluate_gpu works on it in place; the array must outlive the evaluator or be unregistered"""
-        check(lib().tsb_nq_register_host(self._h, arr.ctypes.data, arr.nbytes), "tsb_nq_register_host")
-
-    def unregister_host(self, arr: np.ndarray) -> None:
-        check(lib().tsb_nq_unregister_host(self._h, arr.ctypes.data), "tsb_nq_unregister_host")
-
-    @property
-    def kernel_launches(self) -> int:
-        return int(lib().tsb_nq_kernel_launches(self._h))
-
-    @property
-    def last_xfer(self) -> int:
-        """route of the last evaluate call: XFER_ROUTE_ZEROCOPY | _PIPELINED | _IN_STAGED | _OUT_STAGED bits"""
-        r = int(lib().tsb_nq_last_xfer(self._h))
-        check(min(r, 0), "tsb_nq_last_xfer")
-        return r
-
-    @property
-    def stream(self) -> int:
-        """the handle's cudaStream_t (pool / expand / host-buffer entry points launch on it)"""
-        return int(lib().tsb_nq_stream(self._h) or 0)
 
     def evaluate_gpu(self, parents: np.ndarray, size: int, labels: np.ndarray) -> None:
         """evaluate_gpu(parents_d, size, labels_d) of nqueens_gpu_chpl.chpl:97-123 including the copies of
@@ -117,10 +78,6 @@ class NQueensEvaluator:
         assert nodes.dtype == self.node_dtype and nodes.flags.c_contiguous
         check(lib().tsb_nq_pool_push(self._h, nodes.ctypes.data, nodes.shape[0]), "tsb_nq_pool_push")
 
-    @property
-    def pool_size(self) -> int:
-        return int(lib().tsb_nq_pool_size(self._h))
-
     def pool_step(self, m: int, M: int):
         """(parents popped, children appended, solutions) of one device-side offload round"""
         np_, nc, ns = C.c_int64(0), C.c_uint64(0), C.c_uint64(0)
@@ -133,11 +90,6 @@ class NQueensEvaluator:
         check(lib().tsb_nq_search_on(self._h, self.N, m, self.M if M is None else M, C.byref(st)), "tsb_nq_search_on")
         return st
 
-    def pool_steal_from(self, victim: "NQueensEvaluator", m: int) -> int:
-        got = C.c_int64(0)
-        check(lib().tsb_nq_pool_steal(victim._h, self._h, m, C.byref(got)), "tsb_nq_pool_steal")
-        return int(got.value)
-
     def pools_per_launch(self, M: int) -> int:
         """pools one launch of the persistent kernel serves best for chunks of M parents (tsb_nq_pools_per_launch)"""
         return int(lib().tsb_nq_pools_per_launch(self._h, M))
@@ -149,13 +101,6 @@ class NQueensEvaluator:
         check(lib().tsb_nq_pool_run(self._h, m, M, max_rounds, C.byref(nr), C.byref(np_), C.byref(nc), C.byref(ns)),
               "tsb_nq_pool_run")
         return int(nr.value), int(np_.value), int(nc.value), int(ns.value)
-
-    def pool_drain(self) -> np.ndarray:
-        n = self.pool_size
-        out = np.empty(max(n, 1), dtype=self.node_dtype)
-        got = C.c_int64(0)
-        check(lib().tsb_nq_pool_drain(self._h, out.ctypes.data, n, C.byref(got)), "tsb_nq_pool_drain")
-        return out[: got.value].copy()
 
     def evaluate_device(self, parents_ptr: int, count: int, labels_ptr: int, stream: int = 0) -> None:
         """device-resident form; pointers are raw device addresses (e.g. torch.Tensor.data_ptr())"""

@@ -5,7 +5,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import LB1, LB1_D, LB2, PfspTables, PfspTables50, SearchStats, check, lib
+from ._lib import LB1, LB1_D, LB2, Evaluator, PfspTables, PfspTables50, SearchStats, check, lib
 
 # lib/pfsp/PFSP_node.chpl:9-12
 PFSP_NODE_DTYPE = np.dtype([("depth", np.int32), ("limit1", np.int32), ("prmu", np.int32, (20,))])
@@ -15,6 +15,11 @@ PFSP_NODE50_DTYPE = np.dtype([("depth", np.int32), ("limit1", np.int32), ("prmu"
 assert PFSP_NODE50_DTYPE.itemsize == 208
 # the Chapel CLI spells the bounds as strings (pfsp_gpu_chpl.chpl:15), the C ABI as the C baseline's ints
 LB_NAMES = {"lb1_d": LB1_D, "lb1": LB1, "lb2": LB2}
+
+
+def _lb(lb) -> int:
+    """the C ABI's code of a bound given as "lb1" | "lb1_d" | "lb2" or as the code itself"""
+    return LB_NAMES[lb] if isinstance(lb, str) else int(lb)
 
 
 LB2_VARIANTS = {"full": 0, "nabeshima": 1, "lageweg": 2, "learn": 3}  # lib/pfsp/Bound_johnson.chpl:6
@@ -36,9 +41,12 @@ def taillard_tables50(inst: int, variant="full") -> PfspTables50:
     return t
 
 
-class PfspEvaluator:
+class PfspEvaluator(Evaluator):
     """Owns parents_d / bounds_d / lbound1_d / lbound2_d of pfsp_gpu_chpl.chpl:359-371.  Instances with more than
     20 jobs (ta031..ta060) create a MAX_JOBS = 50 handle: nodes are PFSP_NODE50_DTYPE, evaluate only."""
+
+    _abi = "tsb_pfsp"
+    pool_dtype = PFSP_NODE_DTYPE  # (the device pool exists for 20 jobs only)
 
     def __init__(self, inst: int | None = None, tables=None, M: int = 50000, device: int = 0):
         if tables is None:
@@ -53,48 +61,12 @@ class PfspEvaluator:
         else:
             check(lib().tsb_pfsp_create_from_tables(C.byref(self._h), device, M, C.byref(self.tables)), "tsb_pfsp_create")
 
-    _owner = None  # a sibling's handle belongs to the evaluator it came from
-
-    def close(self):
-        if self._h and self._owner is None:
-            lib().tsb_pfsp_destroy(self._h)
-        self._h = C.c_void_p()
-
-    __del__ = close
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        self.close()
-
-    def set_xfer(self, mode: int):
-        check(lib().tsb_pfsp_set_xfer(self._h, mode), "tsb_pfsp_set_xfer")
-
-    def register_host(self, arr: np.ndarray) -> None:
-        """page-lock + map a long-lived host array (the driver's `parents` / `bounds`); see NQueensEvaluator"""
-        check(lib().tsb_pfsp_register_host(self._h, arr.ctypes.data, arr.nbytes), "tsb_pfsp_register_host")
-
-    def unregister_host(self, arr: np.ndarray) -> None:
-        check(lib().tsb_pfsp_unregister_host(self._h, arr.ctypes.data), "tsb_pfsp_unregister_host")
-
-    @property
-    def kernel_launches(self) -> int:
-        return int(lib().tsb_pfsp_kernel_launches(self._h))
-
-    @property
-    def last_xfer(self) -> int:
-        """route of the last evaluate call: XFER_ROUTE_ZEROCOPY | _PIPELINED | _IN_STAGED | _OUT_STAGED bits"""
-        r = int(lib().tsb_pfsp_last_xfer(self._h))
-        check(min(r, 0), "tsb_pfsp_last_xfer")
-        return r
-
     def evaluate_gpu(self, parents: np.ndarray, size: int, best: int, lb, bounds: np.ndarray) -> None:
         """evaluate_gpu(parents_d, size, best, lbound1_d, lbound2_d, bounds_d) of pfsp_gpu_chpl.chpl:257-270 with
         the copies of :384/:386; `size` = jobs * poolSize; lb is "lb1" | "lb1_d" | "lb2" or the int code"""
         assert parents.dtype == self.node_dtype and parents.flags.c_contiguous
         assert bounds.dtype == np.int32 and bounds.flags.c_contiguous
-        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        kind = _lb(lb)
         if size % self.jobs:
             raise ValueError("size must be jobs * poolSize")
         count = size // self.jobs
@@ -108,7 +80,7 @@ class PfspEvaluator:
         return bounds
 
     def evaluate_device(self, lb, parents_ptr: int, count: int, best: int, bounds_ptr: int, stream: int = 0) -> None:
-        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        kind = _lb(lb)
         check(lib().tsb_pfsp_evaluate_device(self._h, kind, parents_ptr, count, int(best), bounds_ptr, stream),
               "tsb_pfsp_evaluate_device")
 
@@ -118,7 +90,7 @@ class PfspEvaluator:
         """(children, n_solutions, best_after): evaluate_gpu (pfsp_gpu_chpl.chpl:192-270) + generate_children
         (:273-303) of one chunk in one device pass"""
         assert parents.dtype == PFSP_NODE_DTYPE and parents.flags.c_contiguous
-        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        kind = _lb(lb)
         cap = parents.shape[0] * self.jobs
         out = np.empty(max(cap, 1), dtype=PFSP_NODE_DTYPE)
         nc, ns, b = C.c_uint64(0), C.c_uint64(0), C.c_int64(int(best))
@@ -129,7 +101,7 @@ class PfspEvaluator:
     def expand_device(self, lb, parents_ptr: int, count: int, best: int, children_ptr: int, stream: int = 0):
         """(n_children, n_solutions, best_after) of expand on device arrays (parents 16-byte aligned, children 8-byte
         aligned), ordered on `stream` (0: the handle's stream)"""
-        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        kind = _lb(lb)
         nc, ns, b = C.c_uint64(0), C.c_uint64(0), C.c_int64(int(best))
         check(lib().tsb_pfsp_expand_device(self._h, kind, parents_ptr, count, C.byref(b), children_ptr, C.byref(nc),
                                            C.byref(ns), stream), "tsb_pfsp_expand_device")
@@ -138,10 +110,6 @@ class PfspEvaluator:
     def pool_push(self, nodes: np.ndarray) -> None:
         assert nodes.dtype == PFSP_NODE_DTYPE and nodes.flags.c_contiguous
         check(lib().tsb_pfsp_pool_push(self._h, nodes.ctypes.data, nodes.shape[0]), "tsb_pfsp_pool_push")
-
-    @property
-    def pool_size(self) -> int:
-        return int(lib().tsb_pfsp_pool_size(self._h))
 
     @property
     def slow_rounds(self) -> int:
@@ -156,7 +124,7 @@ class PfspEvaluator:
 
     def pool_step(self, lb, m: int, M: int, best: int):
         """(parents popped, children appended, solutions, best_after) of one device-side offload round"""
-        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        kind = _lb(lb)
         np_, nc, ns, b = C.c_int64(0), C.c_uint64(0), C.c_uint64(0), C.c_int64(int(best))
         check(lib().tsb_pfsp_pool_step(self._h, kind, m, M, C.byref(b), C.byref(np_), C.byref(nc), C.byref(ns)),
               "tsb_pfsp_pool_step")
@@ -165,7 +133,7 @@ class PfspEvaluator:
     def pool_run(self, lb, m: int, M: int, best: int, max_rounds: int = 2**62):
         """(rounds, parents, children, solutions, best_after): pool_step rounds until the pool holds fewer than m
         nodes or max_rounds are done, for lb1 / lb1_d and M up to 20 000 in one persistent kernel"""
-        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        kind = _lb(lb)
         b = C.c_int64(int(best))
         nr, np_, nc, ns = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
         check(lib().tsb_pfsp_pool_run(self._h, kind, m, M, max_rounds, C.byref(b), C.byref(nr), C.byref(np_),
@@ -175,7 +143,7 @@ class PfspEvaluator:
     def search(self, inst: int, lb, ub: int = 1, m: int = 25, M: int | None = None, pools: int = 1) -> SearchStats:
         """the whole 3-step search (pfsp_gpu_chpl.chpl:306-431) with the pool of step 2 on this handle's device;
         pools > 1: on this handle and its first pools - 1 siblings (tsb_pfsp_search_on_pools)"""
-        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        kind = _lb(lb)
         st = SearchStats()
         M = self.M if M is None else M
         if pools == 1:
@@ -200,26 +168,15 @@ class PfspEvaluator:
 
     def pools_per_launch(self, lb, M: int) -> int:
         """pools one launch of the persistent kernel can serve for chunks of M parents (tsb_pfsp_pools_per_launch)"""
-        kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+        kind = _lb(lb)
         return int(lib().tsb_pfsp_pools_per_launch(self._h, kind, M))
 
-    def pool_steal_from(self, victim: "PfspEvaluator", m: int) -> int:
-        got = C.c_int64(0)
-        check(lib().tsb_pfsp_pool_steal(victim._h, self._h, m, C.byref(got)), "tsb_pfsp_pool_steal")
-        return int(got.value)
-
-    def pool_drain(self) -> np.ndarray:
-        n = self.pool_size
-        out = np.empty(max(n, 1), dtype=PFSP_NODE_DTYPE)
-        got = C.c_int64(0)
-        check(lib().tsb_pfsp_pool_drain(self._h, out.ctypes.data, n, C.byref(got)), "tsb_pfsp_pool_drain")
-        return out[: got.value].copy()
 
 
 def pfsp_pool_run_multi(evaluators, lb, m: int, M: int, bests, max_rounds: int = 2**62):
     """up to max_rounds rounds of each evaluator's device pool, each with its own incumbent, in shared launches of the
     persistent kernel (tsb_pfsp_pool_run_multi): [(rounds, parents, children, solutions, best_after)] per pool"""
-    kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+    kind = _lb(lb)
     K = len(evaluators)
     if len(bests) != K:
         raise ValueError("one incumbent per pool")
@@ -234,7 +191,7 @@ def pfsp_search_device(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: in
                        pools: int = 1) -> SearchStats:
     """same search, the pool(s) of step 2 resident on the device(s) (tsb_pfsp_pool_*); pools > 1: that many device
     pools per task (tsb_pfsp_search_device_pools)"""
-    kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+    kind = _lb(lb)
     st = SearchStats()
     if pools == 1:
         check(lib().tsb_pfsp_search_device(inst, kind, ub, m, M, D, C.byref(st)), "tsb_pfsp_search_device")
@@ -246,7 +203,7 @@ def pfsp_search_device(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: in
 
 def pfsp_search(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1) -> SearchStats:
     """pfsp_gpu_chpl.chpl:306-431 (D = 1) / pfsp_multigpu_chpl.chpl (static split), C++ emulation driver"""
-    kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+    kind = _lb(lb)
     st = SearchStats()
     check(lib().tsb_pfsp_search(inst, kind, ub, m, M, D, C.byref(st)), "tsb_pfsp_search")
     return st
@@ -254,7 +211,7 @@ def pfsp_search(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: int = 500
 
 def pfsp_search_device_part(inst: int, lb, ub: int, m: int, M: int, D: int, part: int, device: int = 0,
                             pools: int = 1) -> SearchStats:
-    kind = LB_NAMES[lb] if isinstance(lb, str) else int(lb)
+    kind = _lb(lb)
     st = SearchStats()
     if pools == 1:
         check(lib().tsb_pfsp_search_device_part(inst, kind, ub, m, M, D, part, device, C.byref(st)),
