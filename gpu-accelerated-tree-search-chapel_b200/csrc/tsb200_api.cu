@@ -1866,6 +1866,7 @@ const char* tsb_strerror(int code) {
     case TSB_ENODEV: return "no such CUDA device";
     case TSB_EALIGN: return "device pointer not 16-byte aligned";
     case TSB_EUNSUPPORTED: return "unsupported instance shape (jobs must be 20, machines 1..20)";
+    case TSB_ESTOPPED: return "search stopped; its checkpoint file holds it";
   }
   return "unknown error";
 }

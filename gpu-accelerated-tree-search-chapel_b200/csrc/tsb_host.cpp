@@ -11,6 +11,7 @@
 #include <algorithm>
 #include <chrono>
 #include <climits>
+#include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -24,6 +25,7 @@
 #include <vector>
 
 #include "ll_tiers.h"
+#include "search_ckpt.h"
 #include "tsb200.h"
 
 namespace {
@@ -149,6 +151,21 @@ void nq_generate_children(int N, const Node* parents, int size, const uint8_t* l
   }
 }
 
+// tsb_search_request_stop: set from any thread or a signal handler, cleared by the search that stops on it
+std::atomic<int> g_stop_request{0};
+static_assert(std::atomic<int>::is_always_lock_free, "tsb_search_request_stop must be async-signal-safe");
+
+// The stop condition of a resumable search (tsb_*_search_device_ckpt): its deadline or a stop request.  A task asks
+// between two library calls, after its first one; once one task sees it, every task stops at its next boundary.
+struct StopCtl {
+  double deadline = 0;                // now_s() + seconds at the call (infinity: no time limit)
+  std::atomic<bool> stopping{false};  // latched
+  bool check() {
+    if (!stopping.load() && (g_stop_request.load() != 0 || now_s() >= deadline)) stopping.store(true);
+    return stopping.load();
+  }
+};
+
 struct GpuTaskResult {
   uint64_t tree = 0, sol = 0, offloads = 0, parents = 0, launches = 0;
   int64_t best = 0;
@@ -178,6 +195,7 @@ struct StealBoard {
   bool failed;                  // a task could not create its handle: nobody steals
   int idle = 0;
   bool done = false;
+  bool stop = false;  // a task stopped for a checkpoint: nobody steals, every waiting task stops too
   uint64_t steals = 0;
   // every task's handle exists before anybody steals
   void publish_handle(int me, void* h, long long my_size) {
@@ -229,9 +247,9 @@ int board_service(StealBoard* sb, int me, long long my_size, long long floor_, S
   sb->cv.notify_all();
   return rc;
 }
-// out of work: true = stole something (keep going), false = everybody is idle (terminate)
-inline bool board_acquire(StealBoard* sb, int me, long long my_size, long long floor_) {
-  if (!sb) return false;
+// out of work: 1 = stole something (keep going), 0 = everybody is idle (terminate), -1 = the search stops
+inline int board_acquire(StealBoard* sb, int me, long long my_size, long long floor_) {
+  if (!sb) return 0;
   std::unique_lock<std::mutex> lk(sb->mu);
   sb->size[me] = my_size;
   const auto deny_mine = [&] {  // I have nothing to give
@@ -244,12 +262,16 @@ inline bool board_acquire(StealBoard* sb, int me, long long my_size, long long f
   deny_mine();
   ++sb->idle;
   for (;;) {
+    if (sb->stop) {
+      deny_mine();
+      return -1;
+    }
     if (sb->idle == sb->D) {
       sb->done = true;
       sb->cv.notify_all();
-      return false;
+      return 0;
     }
-    if (sb->done) return false;
+    if (sb->done) return 0;
     int v = -1;
     for (int i = 0; i < sb->D && !sb->failed; i++)  // the fullest pool nobody is already asking
       if (i != me && sb->request[i] < 0 && sb->size[i] >= floor_ && (v < 0 || sb->size[i] > sb->size[v])) v = i;
@@ -262,8 +284,8 @@ inline bool board_acquire(StealBoard* sb, int me, long long my_size, long long f
     sb->reply[me] = 0;
     --sb->idle;  // waiting for a victim is not being idle: the victim may hand over half of its pool
     sb->cv.wait(lk, [&] { return sb->reply[me] != 0 || sb->done; });
-    if (sb->reply[me] > 0) return true;
-    if (sb->done) return false;
+    if (sb->reply[me] > 0) return 1;
+    if (sb->done) return 0;
     ++sb->idle;
     sb->size[v] = std::min<long long>(sb->size[v], floor_ - 1);  // (it publishes again after its next launch)
   }
@@ -274,6 +296,16 @@ inline void board_abort(StealBoard* sb, int me) {
   if (!sb) return;
   std::lock_guard<std::mutex> lk(sb->mu);
   sb->failed = sb->done = true;
+  if (sb->request[me] >= 0) sb->reply[sb->request[me]] = -1;
+  sb->request[me] = -1;
+  sb->cv.notify_all();
+}
+
+// a task stops for a checkpoint: the request waiting for it is denied, and no task asks anybody any more
+inline void board_stop(StealBoard* sb, int me) {
+  if (!sb) return;
+  std::lock_guard<std::mutex> lk(sb->mu);
+  sb->stop = true;
   if (sb->request[me] >= 0) sb->reply[sb->request[me]] = -1;
   sb->request[me] = -1;
   sb->cv.notify_all();
@@ -295,6 +327,10 @@ void static_split(Pool<Node>& pool, int D, std::vector<Pool<Node>>& multi) {
 
 // rounds per library call when nodes may move between pools (a victim serves requests between calls)
 inline int64_t rounds_per_call(bool moves, int M) { return !moves ? INT64_MAX : small_chunks(M) ? 256 : 4; }
+
+// rounds per call of a resumable search where the search above makes one unbounded call: a stop waits for the call
+// in flight, and pool_run resumes bit-exactly, so the cap changes no chunk sequence
+constexpr int64_t kCkptRoundsPerCall = 1024;
 
 // (env set: nodes never move between the device pools of a search, the static split alone)
 inline bool steal_allowed() { return !std::getenv("TSB200_NO_STEAL"); }
@@ -323,15 +359,36 @@ int drain_to_host(H* h, Pool<Node>& pool) {
   for (int64_t i = 0; i < n && rc == TSB_OK; i++) pool.pushBack(rest[i]);
   return rc;
 }
+// drain a device pool into records of `rec` bytes, in logical order
+template <class H>
+int drain_to_bytes(H* h, size_t rec, std::vector<uint8_t>& out) {
+  const int64_t left = pool_size(h);
+  std::vector<uint8_t> buf((static_cast<size_t>(left) + 1) * rec);
+  int64_t n = 0;
+  const int rc = pool_drain(h, buf.data(), left, &n);
+  buf.erase(buf.begin() + static_cast<long>(rc == TSB_OK ? static_cast<size_t>(n) * rec : 0), buf.end());
+  out.swap(buf);
+  return rc;
+}
+
+// one task's share of a resumable search: the device pools it resumes from (nullptr: it starts from its host pool),
+// the search's stop condition, and, when it stopped, the pools it left
+struct TaskCkpt {
+  const std::vector<tsb::ckpt::PoolState>* resume = nullptr;
+  StopCtl* stop = nullptr;
+  bool stopped = false;
+  std::vector<tsb::ckpt::PoolState> pools;
+};
 
 // The offload loop of one task whose P >= 1 pools (a handle and its siblings) are resident on the device: all rounds
 // of step 2 inside the library (one persistent kernel for small M, two kernels per round otherwise; the pools' rounds
 // share its launches, S::run_multi = tsb_*_pool_run_multi), `rounds` rounds per call; the host only reads counters.
 // `balance`: a pool of the group that runs dry takes the oldest half of the fullest one (as between tasks).  Between
-// two calls a thief task is served from the fullest pool of the group.  best[i]: pool i's incumbent.
+// two calls a thief task is served from the fullest pool of the group.  best[i]: pool i's incumbent.  `stop` (a
+// resumable search): asked after every call; true = the task stopped with its pools as they are.
 template <class S, class H>
-void devpool_rounds(const S& s, const std::vector<H*>& hs, int m, int M, int64_t rounds, bool balance, StealBoard* sb,
-                    int me, int64_t* best, GpuTaskResult& r) {
+bool devpool_rounds(const S& s, const std::vector<H*>& hs, int m, int M, int64_t rounds, bool balance, StealBoard* sb,
+                    int me, int64_t* best, GpuTaskResult& r, StopCtl* stop) {
   const int P = static_cast<int>(hs.size());
   const auto fullest = [&] {
     int v = 0;
@@ -359,7 +416,9 @@ void devpool_rounds(const S& s, const std::vector<H*>& hs, int m, int M, int64_t
       total += pool_size(x);
     }
     if (most < m) {
-      if (!board_acquire(sb, me, total, floor_)) break;
+      const int got = board_acquire(sb, me, total, floor_);
+      if (got < 0) return true;
+      if (got == 0) break;
       continue;
     }
     r.rc = s.run_multi(hs.data(), P, m, M, rounds, best, out.data());
@@ -371,43 +430,74 @@ void devpool_rounds(const S& s, const std::vector<H*>& hs, int m, int M, int64_t
       r.sol += out[4 * i + 3];
     }
     r.rc = board_service(sb, me, pool_size(hs[fullest()]), floor_, steal);
+    if (r.rc == TSB_OK && stop && stop->check()) {
+      board_stop(sb, me);
+      return true;
+    }
   }
   if (r.rc != TSB_OK) board_abort(sb, me);
+  return false;
 }
 
 // One task's step 2 on device pools: its pool -> the P = S::pools_on(h, M) device pools of h and its siblings (for
 // P > 1 split once more, by the reference's own strided split), all rounds, and the leftovers (fewer than m nodes per
 // pool) back to the task's pool.  Each of several pools is one reference task with its own incumbent
 // (pfsp_multigpu_chpl.chpl:384), min-reduced here, and hands its leftovers back as a reference task does (popBack).
+// `ck` (a resumable search): the task resumes its pools and incumbents from a checkpoint instead of splitting its pool,
+// caps unbounded calls at kCkptRoundsPerCall rounds, and when it stops leaves its pools in ck->pools.
 template <class S, class H, class Node>
-void devpool_on(const S& s, H* h, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me) {
+void devpool_on(const S& s, H* h, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me,
+                TaskCkpt* ck) {
   const uint64_t l0 = kernel_launches(h);
   const int P = s.pools_on(h, M);
+  const std::vector<tsb::ckpt::PoolState>* resume = ck ? ck->resume : nullptr;
+  if (resume && static_cast<int>(resume->size()) != P) r.rc = TSB_EINVAL;  // (written where P differed)
   std::vector<H*> hs{h};
   for (int i = 1; i < P && r.rc == TSB_OK; i++) {
     H* sib = nullptr;
     r.rc = pool_sibling(h, i, &sib);
     hs.push_back(sib);
   }
-  std::vector<Pool<Node>> part;
-  if (r.rc == TSB_OK) static_split(pool, P, part);
-  long long most = 0;
-  for (int i = 0; i < P && r.rc == TSB_OK; i++) {
-    r.rc = pool_push(hs[i], &part[i].el[part[i].front], static_cast<int64_t>(part[i].size));
-    most = std::max<long long>(most, pool_size(hs[i]));
-  }
-  if (sb) sb->publish_handle(me, r.rc == TSB_OK ? h : nullptr, most);
   std::unique_ptr<int64_t[]> best(new int64_t[P]);
   std::fill(best.get(), best.get() + P, r.best);
-  if (r.rc == TSB_OK) devpool_rounds(s, hs, m, M, s.rounds(P, sb != nullptr, M), s.balance, sb, me, best.get(), r);
+  long long most = 0;
+  if (resume) {
+    for (int i = 0; i < P && r.rc == TSB_OK; i++) {
+      const tsb::ckpt::PoolState& in = (*resume)[i];
+      if (!in.nodes.empty()) r.rc = pool_push(hs[i], in.nodes.data(), static_cast<int64_t>(in.nodes.size() / sizeof(Node)));
+      best[i] = in.best;
+      most = std::max<long long>(most, pool_size(hs[i]));
+    }
+  } else {
+    std::vector<Pool<Node>> part;
+    if (r.rc == TSB_OK) static_split(pool, P, part);
+    for (int i = 0; i < P && r.rc == TSB_OK; i++) {
+      r.rc = pool_push(hs[i], &part[i].el[part[i].front], static_cast<int64_t>(part[i].size));
+      most = std::max<long long>(most, pool_size(hs[i]));
+    }
+  }
+  if (sb) sb->publish_handle(me, r.rc == TSB_OK ? h : nullptr, most);
+  int64_t rounds = s.rounds(P, sb != nullptr, M);
+  if (ck && rounds == INT64_MAX) rounds = kCkptRoundsPerCall;
+  bool stopped = false;
+  if (r.rc == TSB_OK)
+    stopped = devpool_rounds(s, hs, m, M, rounds, s.balance, sb, me, best.get(), r, ck ? ck->stop : nullptr);
   r.best = *std::min_element(best.get(), best.get() + P);
+  if (stopped) {  // every pool with its incumbent, in logical order, for the checkpoint
+    ck->stopped = true;
+    ck->pools.resize(P);
+    for (int i = 0; i < P && r.rc == TSB_OK; i++) {
+      ck->pools[i].best = best[i];
+      r.rc = drain_to_bytes(hs[i], sizeof(Node), ck->pools[i].nodes);
+    }
+  }
   for (H* x : hs) {
-    if (r.rc != TSB_OK) break;
+    if (r.rc != TSB_OK || stopped) break;
     Pool<Node> rest;
     r.rc = drain_to_host(x, P == 1 ? pool : rest);
     for (Node n; rest.popBack(n);) pool.pushBack(n);
   }
-  r.launches = kernel_launches(h) - l0;
+  r.launches += kernel_launches(h) - l0;
 }
 
 // Several pools per task (TSB200_POOLS=1 turns it off, =2 caps it at two): for chunks that fit the persistent kernel a
@@ -747,7 +837,8 @@ struct NqSearch {
     r.launches = tsb_nq_kernel_launches(h);
     tsb_nq_destroy(h);
   }
-  void device_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me) const {
+  void device_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me,
+                   TaskCkpt* ck) const {
     const double tt0 = now_s();
     tsb_nq* h = nq_handle_cache().acquire<Node>(device, N, g, M, &r.rc);
     if (r.rc != TSB_OK) {
@@ -755,7 +846,7 @@ struct NqSearch {
       return;
     }
     const double tt1 = now_s();
-    devpool_on(*this, h, m, M, pool, r, sb, me);
+    devpool_on(*this, h, m, M, pool, r, sb, me, ck);
     const double tt2 = now_s();
     nq_handle_cache().release(h, device, N, g, M, sizeof(Node), r.rc == TSB_OK);
     if (std::getenv("TSB200_TRACE"))
@@ -817,14 +908,15 @@ struct PfspSearch {
     r.launches = tsb_pfsp_kernel_launches(h);
     tsb_pfsp_destroy(h);
   }
-  void device_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me) const {
+  void device_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me,
+                   TaskCkpt* ck) const {
     tsb_pfsp* h = nullptr;
     r.rc = tsb_pfsp_create_from_tables(&h, device, M, &hb.t);
     if (r.rc != TSB_OK) {
       if (sb) sb->publish_handle(me, nullptr, 0);
       return;
     }
-    devpool_on(*this, h, m, M, pool, r, sb, me);
+    devpool_on(*this, h, m, M, pool, r, sb, me, ck);
     tsb_pfsp_destroy(h);
   }
   int pools_on(tsb_pfsp*, int) const { return pools; }
@@ -834,21 +926,36 @@ struct PfspSearch {
   }
 };
 
+// A resumable search (tsb_*_search_device_ckpt): where its checkpoint goes and with which parameters, the state it
+// resumes from (nullptr: a new search) and its stop condition
+struct SearchCkpt {
+  const char* path;
+  tsb::ckpt::Params params;
+  const tsb::ckpt::State* resume;
+  StopCtl stop;
+};
+
 // The drivers' search (nqueens_multigpu_chpl.chpl, pfsp_multigpu_chpl.chpl; D = 1: nqueens_gpu_chpl.chpl,
 // pfsp_gpu_chpl.chpl) with the same Pool contract: step 1 on the CPU, step 2 on D tasks, step 3 on the CPU.
 // part < 0: the whole search.  part >= 0: only task `part` of the D-way static split, on `device` (one rank of a
 // process-per-GPU launch): the step-1 tree is credited to part 0 and every part drains its own leftovers, so the
 // per-part counts add up to the whole search's.  `on` != nullptr: D = 1 on device pools of a handle the caller created
 // (set-up outside the search's timers, as the Chapel drivers' `on device var` declarations are).
+// `ck` (D tasks on device pools, part < 0): a resumed search skips step 1 and continues step 2 from the checkpoint; a
+// search that stops writes the checkpoint and returns TSB_ESTOPPED with the counts so far.
 template <class S>
 int three_step_search(const S& s, int m, int M, int D, int part, int device, typename S::Handle* on,
-                      tsb_search_stats* out) {
+                      tsb_search_stats* out, SearchCkpt* ck = nullptr) {
   using Node = typename S::Node;
+  const tsb::ckpt::State* from = ck ? ck->resume : nullptr;
+  if (from && s.steal && D > 1)  // (tasks that steal leave step 2 together: none can have finished alone)
+    for (const auto& t : from->tasks)
+      if (t.finished) return TSB_EINVAL;
   if (!on)
     if (int rc = tsb_init_devices(part < 0 ? D : device + 1); rc != TSB_OK) return rc;  // contexts exist before the timers start
   int64_t best = s.initial_best;
   Pool<Node> pool;
-  pool.pushBack(s.root());
+  if (!from) pool.pushBack(s.root());
   uint64_t tree = 0, sol = 0;
   Node parent;
   double t0 = now_s();
@@ -858,15 +965,41 @@ int three_step_search(const S& s, int m, int M, int D, int part, int device, typ
   }
   double t1 = now_s();
   out->t_step1 = t1 - t0;
+  std::vector<GpuTaskResult> res(D);
+  std::vector<TaskCkpt> tck(ck ? D : 0);
+  for (TaskCkpt& t : tck) t.stop = &ck->stop;
+  if (from) {  // step 1 and the tasks' counters as the checkpoint has them
+    tree = from->tree1;
+    sol = from->sol1;
+    best = from->best1;
+    out->t_step1 = from->t_step1;
+    for (int gid = 0; gid < D; gid++) {
+      const tsb::ckpt::TaskState& t = from->tasks[gid];
+      GpuTaskResult& r = res[gid];
+      r.tree = t.tree, r.sol = t.sol, r.offloads = t.offloads, r.parents = t.parents, r.launches = t.launches;
+      if (!t.finished) tck[gid].resume = &t.pools;
+    }
+  }
   // step 2: on device pools, every task's pool moves to its device and stays there; tasks that run dry steal from
   // the fullest device pool peer-to-peer
-  std::vector<GpuTaskResult> res(D);
   for (auto& r : res) r.best = best;  // per-task best_l = best (pfsp_multigpu_chpl.chpl:384)
-  const auto task = [&](int dev, Pool<Node>& from, GpuTaskResult& r, StealBoard* sb, int me) {
-    if (s.devpool)
-      s.device_task(dev, m, M, from, r, sb, me);
-    else
-      s.host_task(dev, m, M, from, r);
+  if (from)
+    for (int gid = 0; gid < D; gid++) res[gid].best = from->tasks[gid].best;
+  // a task that had left step 2 when the checkpoint was written does not run again: its host pool holds its leftovers
+  const auto finished = [&](int gid) { return from && from->tasks[gid].finished; };
+  const auto task = [&](int dev, Pool<Node>& own, GpuTaskResult& r, StealBoard* sb, int me) {
+    if (finished(me)) {
+      const std::vector<uint8_t>& left = from->tasks[me].left;
+      for (size_t i = 0; i + sizeof(Node) <= left.size(); i += sizeof(Node)) {
+        Node n;
+        std::memcpy(&n, &left[i], sizeof(Node));
+        own.pushBack(n);
+      }
+    } else if (s.devpool) {
+      s.device_task(dev, m, M, own, r, sb, me, ck ? &tck[me] : nullptr);
+    } else {
+      s.host_task(dev, m, M, own, r);
+    }
   };
   // a task's leftovers back to the global pool (:315-320); several pools per task already handed theirs back to the
   // task's pool one by one, as the reference's tasks do, so that order stays
@@ -879,31 +1012,36 @@ int three_step_search(const S& s, int m, int M, int D, int part, int device, typ
   // task g drives GPU g; with fewer than D GPUs present the tasks wrap around (g % ndev): the
   // per-task pools stay independent, so counts are unchanged — used to test D > 1 on one GPU
   const int ndev = std::max(1, tsb_device_count());
+  std::vector<Pool<Node>> multi;
+  bool stopped = false;  // (a resumable search: some task stopped for the checkpoint)
   if (on) {
-    devpool_on(s, on, m, M, pool, res[0], nullptr, 0);
+    devpool_on(s, on, m, M, pool, res[0], nullptr, 0, nullptr);
   } else if (part >= 0) {
     if (part != 0) tree = sol = 0;  // step 1 is credited to part 0
-    std::vector<Pool<Node>> multi;
     static_split(pool, D, multi);
     task(device, multi[part], res[part], nullptr, 0);
     hand_back(multi[part]);
   } else if (D == 1) {
     task(0, pool, res[0], nullptr, 0);
+    stopped = ck && tck[0].stopped;
   } else {
-    std::vector<Pool<Node>> multi;
     static_split(pool, D, multi);
     StealBoard board(D);
     StealBoard* sb = s.steal ? &board : nullptr;
     std::vector<std::thread> th;
     for (int gid = 0; gid < D; gid++)
       th.emplace_back([&, gid] {
+        if (finished(gid)) return task(gid, multi[gid], res[gid], nullptr, gid);
         bind_task(gid % ndev);
         task(gid % ndev, multi[gid], res[gid], sb, gid);
       });
     for (auto& x : th) x.join();
-    for (int gid = 0; gid < D; gid++) hand_back(multi[gid]);
-    out->steals = board.steals;
+    for (const TaskCkpt& t : tck) stopped = stopped || t.stopped;
+    for (int gid = 0; gid < D && !stopped; gid++) hand_back(multi[gid]);
+    out->steals = (from ? from->steals : 0) + board.steals;
   }
+  const uint64_t tree1 = tree, sol1 = sol;
+  const int64_t best1 = best;
   for (int gid = 0; gid < D; gid++) {
     if (res[gid].rc != TSB_OK) return res[gid].rc;
     tree += res[gid].tree;
@@ -915,7 +1053,43 @@ int three_step_search(const S& s, int m, int M, int D, int part, int device, typ
     out->per_gpu_tree[gid] = res[gid].tree;
   }
   double t2 = now_s();
-  out->t_step2 = t2 - t1;
+  out->t_step2 = (from ? from->t_step2 : 0) + (t2 - t1);
+  if (stopped) {  // the checkpoint: step 1, every task's counters, and its device pools or (finished) its leftovers
+    tsb::ckpt::State st;
+    st.p = ck->params;
+    st.tree1 = tree1, st.sol1 = sol1, st.best1 = best1;
+    st.t_step1 = out->t_step1, st.t_step2 = out->t_step2, st.steals = out->steals;
+    st.tasks.resize(D);
+    for (int gid = 0; gid < D; gid++) {
+      const GpuTaskResult& r = res[gid];
+      tsb::ckpt::TaskState& t = st.tasks[gid];
+      t.tree = r.tree, t.sol = r.sol, t.offloads = r.offloads, t.parents = r.parents, t.launches = r.launches;
+      t.best = r.best;
+      t.finished = !tck[gid].stopped;
+      if (t.finished) {
+        const Pool<Node>& own = D == 1 ? pool : multi[gid];
+        const auto* b = reinterpret_cast<const uint8_t*>(own.el.data() + own.front);
+        t.left.assign(b, b + own.size * sizeof(Node));
+      } else {
+        t.pools = std::move(tck[gid].pools);
+      }
+    }
+    const double tw = now_s();
+    if (int rc = tsb::ckpt::save(ck->path, st); rc != TSB_OK) return rc;
+    if (std::getenv("TSB200_TRACE")) {
+      size_t nodes = 0;
+      for (const auto& t : st.tasks) {
+        nodes += t.left.size();
+        for (const auto& x : t.pools) nodes += x.nodes.size();
+      }
+      std::fprintf(stderr, "[tsb200] checkpoint: %zu nodes written in %.1f ms\n", nodes / sizeof(Node),
+                   (now_s() - tw) * 1e3);
+    }
+    out->explored_tree = tree;
+    out->explored_sol = sol;
+    out->best = best;
+    return TSB_ESTOPPED;
+  }
   while (pool.popBack(parent)) s.decompose(parent, tree, sol, best, pool);  // step 3
   out->t_step3 = now_s() - t2;
   out->explored_tree = tree;
@@ -926,25 +1100,44 @@ int three_step_search(const S& s, int m, int M, int D, int part, int device, typ
 
 template <class Node>
 int nq_search(int N, int g, int m, int M, int D, bool devpool, int part, int device, tsb_nq* on,
-              tsb_search_stats* out) {
+              tsb_search_stats* out, SearchCkpt* ck = nullptr) {
   constexpr bool wide = std::is_same_v<Node, tsb_nq_node24>;
   if (!out || N < 1 || N > (wide ? TSB_MAX_QUEENS_WIDE : TSB_MAX_QUEENS) || g < 1 || m < 1 || M < 1 || D < 1 || D > 8 ||
       part >= D)
     return TSB_EINVAL;
   std::memset(out, 0, sizeof(*out));
-  return three_step_search(NqSearch<Node>(N, g, M, devpool), m, M, D, part, device, on, out);
+  return three_step_search(NqSearch<Node>(N, g, M, devpool), m, M, D, part, device, on, out, ck);
 }
 
 // pools > 1 (device pools only): every task's share split once more into `pools` device pools (devpool_on)
 int pfsp_search(int inst, int lb_kind, int ub, int m, int M, int D, bool devpool, int part, int device, tsb_pfsp* on,
-                tsb_search_stats* out, int pools = 1) {
+                tsb_search_stats* out, int pools = 1, SearchCkpt* ck = nullptr) {
   if (!out || lb_kind < 0 || lb_kind > 2 || (ub != 0 && ub != 1) || m < 1 || M < 1 || D < 1 || D > 8 || part >= D ||
       pools < 1 || pools > 4)
     return TSB_EINVAL;
   std::memset(out, 0, sizeof(*out));
   std::vector<tsb_pfsp_tables> tv(1);
   if (int rc = tsb_pfsp_tables_build(&tv[0], inst); rc != TSB_OK) return rc;
-  return three_step_search(PfspSearch(tv[0], inst, lb_kind, ub, devpool, pools), m, M, D, part, device, on, out);
+  return three_step_search(PfspSearch(tv[0], inst, lb_kind, ub, devpool, pools), m, M, D, part, device, on, out,
+                           ck);
+}
+
+// the resumable searches: resume from `path` if a checkpoint is there (refused before any device call if it is damaged
+// or was written for other parameters), run `run` under a stop condition, remove the checkpoint when the search ends
+template <class Run>
+int ckpt_search(const char* path, double seconds, const tsb::ckpt::Params& p, Run&& run) {
+  if (!path || !*path || std::isnan(seconds)) return TSB_EINVAL;
+  tsb::ckpt::State st;
+  const double t0 = now_s();
+  const int got = tsb::ckpt::load(path, p, &st);
+  if (got < 0) return got;
+  if (got && std::getenv("TSB200_TRACE")) std::fprintf(stderr, "[tsb200] checkpoint: read in %.1f ms\n", (now_s() - t0) * 1e3);
+  SearchCkpt ck{path, p, got ? &st : nullptr, {}};
+  ck.stop.deadline = seconds < 0 ? HUGE_VAL : now_s() + seconds;
+  const int rc = run(&ck);
+  if (rc == TSB_OK) std::remove(path);
+  if (rc == TSB_ESTOPPED) g_stop_request.store(0);
+  return rc;
 }
 
 template <class Node>
@@ -1072,5 +1265,26 @@ int tsb_pfsp_search_on_pools(tsb_pfsp* h, int inst, int lb_kind, int ub, int m, 
   if (!h) return TSB_EINVAL;
   return pfsp_search(inst, lb_kind, ub, m, M, 1, true, -1, 0, h, out, pools);
 }
+
+int tsb_nq_search_device_ckpt(int max_queens, int N, int g, int m, int M, int D, const char* path, double seconds,
+                              tsb_search_stats* out) {
+  if (max_queens != TSB_MAX_QUEENS && max_queens != TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
+  return with_nq_node(max_queens == TSB_MAX_QUEENS_WIDE || N > TSB_MAX_QUEENS, [&](auto node) {
+    using Node = decltype(node);
+    // (N-Queens has no pools argument: how many pools a task runs is checked against the checkpoint per task)
+    const tsb::ckpt::Params p{tsb::ckpt::kNQueens, sizeof(Node), N, g, 0, m, M, D, 0};
+    return ckpt_search(path, seconds, p, [&](SearchCkpt* ck) {
+      return nq_search<Node>(N, g, m, M, D, true, -1, 0, nullptr, out, ck);
+    });
+  });
+}
+int tsb_pfsp_search_device_ckpt(int inst, int lb_kind, int ub, int m, int M, int D, int pools, const char* path,
+                                double seconds, tsb_search_stats* out) {
+  const tsb::ckpt::Params p{tsb::ckpt::kPfsp, sizeof(tsb_pfsp_node), inst, lb_kind, ub, m, M, D, pools};
+  return ckpt_search(path, seconds, p, [&](SearchCkpt* ck) {
+    return pfsp_search(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out, pools, ck);
+  });
+}
+void tsb_search_request_stop(void) { g_stop_request.store(1); }
 
 }  // extern "C"

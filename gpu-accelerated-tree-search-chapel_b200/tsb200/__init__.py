@@ -13,7 +13,7 @@ device every call raises.
 """
 from ._lib import (LB1, LB1_D, LB2, ROUTE_LB2, ROUTE_LB2U, ROUTE_MT_MASK, ROUTE_SIMD16, XFER_AUTO, XFER_MEMCPY,
                    XFER_ROUTE_IN_STAGED, XFER_ROUTE_OUT_STAGED, XFER_ROUTE_PIPELINED, XFER_ROUTE_ZEROCOPY,
-                   XFER_ZEROCOPY, PfspTables, PfspTables50, SearchStats, TsbError, check, lib)
+                   XFER_ZEROCOPY, PfspTables, PfspTables50, SearchStats, SearchStopped, TsbError, check, lib, request_stop)
 from .nqueens import (NQ_NODE_DTYPE, NQ_NODE24_DTYPE, NQueensEvaluator, nq_node_dtype, nqueens_search, nqueens_search_device,
                       nqueens_pool_run_multi, nqueens_search_device_part, nqueens_warmup)
 from .pfsp import (PFSP_NODE_DTYPE, PFSP_NODE50_DTYPE, LB_NAMES, LB2_VARIANTS, PfspEvaluator, taillard_tables50, pfsp_search, pfsp_search_device,
@@ -22,7 +22,7 @@ from .pfsp import (PFSP_NODE_DTYPE, PFSP_NODE50_DTYPE, LB_NAMES, LB2_VARIANTS, P
 __all__ = ["NQueensEvaluator", "PfspEvaluator", "nqueens_warmup", "nqueens_pool_run_multi", "nqueens_search", "nqueens_search_device", "nqueens_search_device_part", "pfsp_search", "pfsp_search_device",
            "pfsp_search_device_part", "pfsp_pool_run_multi",
            "taillard_tables",
-           "NQ_NODE_DTYPE", "NQ_NODE24_DTYPE", "nq_node_dtype", "PFSP_NODE_DTYPE", "PFSP_NODE50_DTYPE", "LB2_VARIANTS", "taillard_tables50", "LB_NAMES", "LB1", "LB1_D", "LB2", "TsbError", "lib", "check",
+           "NQ_NODE_DTYPE", "NQ_NODE24_DTYPE", "nq_node_dtype", "PFSP_NODE_DTYPE", "PFSP_NODE50_DTYPE", "LB2_VARIANTS", "taillard_tables50", "LB_NAMES", "LB1", "LB1_D", "LB2", "TsbError", "SearchStopped", "request_stop", "lib", "check",
            "PfspTables", "PfspTables50", "SearchStats", "XFER_AUTO", "XFER_MEMCPY", "XFER_ZEROCOPY",
            "XFER_ROUTE_ZEROCOPY", "XFER_ROUTE_PIPELINED", "XFER_ROUTE_IN_STAGED", "XFER_ROUTE_OUT_STAGED",
            "ROUTE_MT_MASK", "ROUTE_SIMD16", "ROUTE_LB2", "ROUTE_LB2U"]

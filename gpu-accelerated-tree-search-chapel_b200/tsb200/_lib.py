@@ -15,7 +15,7 @@ MAX_QUEENS, MAX_QUEENS_WIDE = 20, 24
 MAX_MACHINES = 20
 MAX_PAIRS = 190
 
-OK, EINVAL, ECUDA, ENOMEM, ENODEV, EALIGN, EUNSUPPORTED = 0, -1, -2, -3, -4, -5, -6
+OK, EINVAL, ECUDA, ENOMEM, ENODEV, EALIGN, EUNSUPPORTED, ESTOPPED = 0, -1, -2, -3, -4, -5, -6, -7
 LB1_D, LB1, LB2 = 0, 1, 2
 XFER_AUTO, XFER_MEMCPY, XFER_ZEROCOPY = 0, 1, 2
 # tsb_*_last_xfer: the route of the last host-buffer evaluate call
@@ -32,6 +32,15 @@ class TsbError(RuntimeError):
             msg += " — " + L.tsb_last_cuda_error().decode()
         super().__init__(f"{where}: {msg} ({code})")
         self.code = code
+
+
+class SearchStopped(TsbError):
+    """a resumable search stopped (time limit or request_stop()) and wrote its checkpoint; `stats` holds the counts so
+    far.  Calling the same search again with the same checkpoint continues it."""
+
+    def __init__(self, where: str, stats):
+        super().__init__(ESTOPPED, where)
+        self.stats = stats
 
 
 class PfspTables(C.Structure):
@@ -149,6 +158,9 @@ SYMBOLS = {
     "tsb_pfsp_search_device_pools": (_i, [_i, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
     "tsb_pfsp_search_device_pools_part": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
     "tsb_pfsp_search_on_pools": (_i, [_vp, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
+    "tsb_nq_search_device_ckpt": (_i, [_i, _i, _i, _i, _i, _i, C.c_char_p, C.c_double, C.POINTER(SearchStats)]),
+    "tsb_pfsp_search_device_ckpt": (_i, [_i, _i, _i, _i, _i, _i, _i, C.c_char_p, C.c_double, C.POINTER(SearchStats)]),
+    "tsb_search_request_stop": (None, []),
 }
 
 _lib = None
@@ -172,6 +184,24 @@ def lib() -> C.CDLL:
 def check(code: int, where: str) -> None:
     if code != OK:
         raise TsbError(code, where)
+
+
+def check_search(code: int, where: str, stats) -> None:
+    """check() for the resumable searches: TSB_ESTOPPED raises SearchStopped with the counts so far"""
+    if code == ESTOPPED:
+        raise SearchStopped(where, stats)
+    check(code, where)
+
+
+def ckpt_args(checkpoint, time_limit):
+    """the path and seconds arguments of tsb_*_search_device_ckpt (time_limit None: no limit)"""
+    return os.fsencode(os.fspath(checkpoint)), -1.0 if time_limit is None else float(time_limit)
+
+
+def request_stop() -> None:
+    """every resumable search running in this process (or the next one to start) stops at its next call boundary
+    and writes its checkpoint (tsb_search_request_stop; safe to call from a signal handler)"""
+    lib().tsb_search_request_stop()
 
 
 class Evaluator:

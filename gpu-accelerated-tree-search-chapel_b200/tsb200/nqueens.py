@@ -5,7 +5,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import MAX_QUEENS, MAX_QUEENS_WIDE, Evaluator, SearchStats, check, lib
+from ._lib import MAX_QUEENS, MAX_QUEENS_WIDE, Evaluator, SearchStats, check, check_search, ckpt_args, lib
 
 # lib/nqueens/NQueens_node.chpl:9-11
 NQ_NODE_DTYPE = np.dtype([("depth", np.uint8), ("board", np.uint8, (MAX_QUEENS,))])
@@ -141,10 +141,17 @@ def nqueens_search(N: int = 14, g: int = 1, m: int = 25, M: int = 50000, D: int 
 
 
 def nqueens_search_device(N: int = 14, g: int = 1, m: int = 25, M: int = 50000, D: int = 1,
-                          max_queens: int | None = None) -> SearchStats:
-    """same 3-step search, the pool(s) of step 2 resident on the device(s) (tsb_nq_pool_*)"""
+                          max_queens: int | None = None, checkpoint=None, time_limit: float | None = None) -> SearchStats:
+    """same 3-step search, the pool(s) of step 2 resident on the device(s) (tsb_nq_pool_*).
+    checkpoint=path: the resumable search (tsb_nq_search_device_ckpt): it continues from the file if there is one,
+    stops after time_limit seconds (None: no limit) or on request_stop() by writing the file and raising
+    SearchStopped, and removes the file when it ends; the returned stats are those of the whole search"""
     st = SearchStats()
-    if max_queens is None:
+    if checkpoint is not None:
+        mq = MAX_QUEENS if max_queens is None else max_queens
+        check_search(lib().tsb_nq_search_device_ckpt(mq, N, g, m, M, D, *ckpt_args(checkpoint, time_limit), C.byref(st)),
+                     "tsb_nq_search_device_ckpt", st)
+    elif max_queens is None:
         check(lib().tsb_nq_search_device(N, g, m, M, D, C.byref(st)), "tsb_nq_search_device")
     else:
         check(lib().tsb_nq_search_device_wide(max_queens, N, g, m, M, D, C.byref(st)), "tsb_nq_search_device_wide")

@@ -5,7 +5,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import LB1, LB1_D, LB2, Evaluator, PfspTables, PfspTables50, SearchStats, check, lib
+from ._lib import LB1, LB1_D, LB2, Evaluator, PfspTables, PfspTables50, SearchStats, check, check_search, ckpt_args, lib
 
 # lib/pfsp/PFSP_node.chpl:9-12
 PFSP_NODE_DTYPE = np.dtype([("depth", np.int32), ("limit1", np.int32), ("prmu", np.int32, (20,))])
@@ -188,12 +188,16 @@ def pfsp_pool_run_multi(evaluators, lb, m: int, M: int, bests, max_rounds: int =
 
 
 def pfsp_search_device(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1,
-                       pools: int = 1) -> SearchStats:
+                       pools: int = 1, checkpoint=None, time_limit: float | None = None) -> SearchStats:
     """same search, the pool(s) of step 2 resident on the device(s) (tsb_pfsp_pool_*); pools > 1: that many device
-    pools per task (tsb_pfsp_search_device_pools)"""
+    pools per task (tsb_pfsp_search_device_pools).  checkpoint / time_limit: the resumable search
+    (tsb_pfsp_search_device_ckpt), as for nqueens_search_device"""
     kind = _lb(lb)
     st = SearchStats()
-    if pools == 1:
+    if checkpoint is not None:
+        check_search(lib().tsb_pfsp_search_device_ckpt(inst, kind, ub, m, M, D, pools, *ckpt_args(checkpoint, time_limit),
+                                                       C.byref(st)), "tsb_pfsp_search_device_ckpt", st)
+    elif pools == 1:
         check(lib().tsb_pfsp_search_device(inst, kind, ub, m, M, D, C.byref(st)), "tsb_pfsp_search_device")
     else:
         check(lib().tsb_pfsp_search_device_pools(inst, kind, ub, m, M, D, pools, C.byref(st)),

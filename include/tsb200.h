@@ -74,7 +74,8 @@ enum {
   TSB_ENOMEM = -3,   /* host or device allocation failed */
   TSB_ENODEV = -4,   /* no such CUDA device / no CUDA driver */
   TSB_EALIGN = -5,   /* device pointer passed to *_evaluate_device is not 16-byte aligned */
-  TSB_EUNSUPPORTED = -6 /* instance shape outside jobs <= 20, machines in 1..20 */
+  TSB_EUNSUPPORTED = -6, /* instance shape outside jobs <= 20, machines in 1..20 */
+  TSB_ESTOPPED = -7      /* a resumable search stopped; its checkpoint file holds it; *out has the counts so far */
 };
 
 /* lower-bound selector: integer encoding of baselines/pfsp/pfsp_c.c:86-88 and
@@ -453,6 +454,33 @@ int tsb_pfsp_search_device_pools_part(int inst, int lb_kind, int ub, int m, int 
                                       int device, tsb_search_stats* out);
 int tsb_pfsp_search_on_pools(tsb_pfsp* h, int inst, int lb_kind, int ub, int m, int M, int pools,
                              tsb_search_stats* out);
+
+/* Resumable device-pool searches.  tsb_nq_search_device_ckpt is the search of tsb_nq_search_device (max_queens = 20:
+ * N <= 20 on 21-byte nodes, N > 20 on 25-byte nodes) or of tsb_nq_search_device_wide (max_queens = 24);
+ * tsb_pfsp_search_device_ckpt is that of tsb_pfsp_search_device_pools.  Every other argument is checked as by that
+ * twin.  `path` names the checkpoint file:
+ *   - no file at `path`: a new search, exactly as the twin runs it (step 1, split, step 2);
+ *   - a file at `path`: step 2 continues from it (step 1 is not redone).  A file that is damaged (size, checksum,
+ *     magic, version) or was written by the other problem, another node width or other parameters (N, g or inst,
+ *     lb_kind, ub; m, M, D, pools) gives TSB_EINVAL before any device call, and stays as it is.
+ * The search stops when `seconds` of wall clock have passed since the call began (seconds < 0: no limit; 0: as soon
+ * as every task has made one library call) or when tsb_search_request_stop was called.  A task asks between two of
+ * its library calls (tsb_*_pool_run_multi), never before its first one, so every call makes progress; where the twin
+ * makes one unbounded call (one pool per task and no thief), calls are capped at 1024 rounds, which pool_run resumes
+ * bit-exactly.  On a stop every task finishes its call, every device pool is drained in logical order, the state is
+ * written to `path`.tmp, fsync'd and renamed over `path`, and the call returns TSB_ESTOPPED with the counts so far in
+ * *out (TSB_EINVAL if the file cannot be written: a file already at `path` is then unchanged).  When the search ends
+ * it returns TSB_OK with the stats of the whole search summed over every invocation (t_step1: the first one's) and
+ * removes `path`: `while (rc == TSB_ESTOPPED) rc = <the same call>;` runs a search in slots.
+ * Reproduced exactly across stops (every field but the times and kernel_launches): D = 1, and PFSP with ub = 0 for
+ * any D; with tasks that steal (D > 1: N-Queens, PFSP with ub = 1) tree, sol and best. */
+int tsb_nq_search_device_ckpt(int max_queens, int N, int g, int m, int M, int D, const char* path, double seconds,
+                              tsb_search_stats* out);
+int tsb_pfsp_search_device_ckpt(int inst, int lb_kind, int ub, int m, int M, int D, int pools, const char* path,
+                                double seconds, tsb_search_stats* out);
+/* async-signal-safe: every resumable search running in the process (or the next one to start) stops at its next call
+ * boundary; the search that stops on it clears it */
+void tsb_search_request_stop(void);
 
 #ifdef __cplusplus
 }
