@@ -27,6 +27,8 @@
 #include "nq_kernel.cuh"
 #include "pfsp_kernels.cuh"
 #include "pfsp_wide.cuh"
+#include "pfsp_wide_expand.cuh"
+#include "pfsp_search_pool.h"
 #include "tsb200.h"
 
 // Internals shared by both handle types (the handles themselves are the header's types, defined after this block)
@@ -1167,6 +1169,7 @@ struct tsb_pfsp : Base {
   tsb::Lb2TabU* d_tabu = nullptr;
   uint64_t slow_rounds = 0;
   std::vector<tsb_pfsp_node> h_chunk, h_kids;  // slow path scratch
+  std::vector<tsb_pfsp_node50> h_chunk50, h_kids50;
   std::vector<int32_t> h_bounds;
 };
 
@@ -1616,11 +1619,36 @@ int pfsp_expand_m(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const tsb::Exp
   return TSB_OK;
 }
 
+// the same round on a 50-job handle (pfsp_wide_expand.cuh): count, build
+template <int M>
+int pfsp_wide_expand_m(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const tsb::ExpandParams& prm,
+                       uint8_t* children_d, cudaStream_t s) {
+  ExpandCtx& ex = h->ex;
+  const long long recs = static_cast<long long>(prm.n_tiles) * tsb::PW_TILE;
+  auto k1 = lb_kind == TSB_LB1_D ? tsb::pfsp_wide_expand_count_kernel<0, M>
+            : lb_kind == TSB_LB1 ? tsb::pfsp_wide_expand_count_kernel<1, M>
+                                 : tsb::pfsp_wide_expand_count_kernel<2, M>;
+  auto k3 = tsb::pfsp_wide_expand_build_kernel;
+  const size_t smem1 = sizeof(tsb::PfspWideCountSmem) + 128, smem3 = sizeof(tsb::PfspWideBuildSmem) + 128;
+  int g1 = 1, g3 = 1;
+  int rc = h->grid_for(k1, tsb::PW_THREADS, smem1, recs, tsb::PW_TILE, &g1);
+  if (rc == TSB_OK) rc = h->grid_for(k3, tsb::PW_THREADS, smem3, recs, tsb::PW_TILE, &g3);
+  if (rc != TSB_OK) return rc;
+  if ((prm.n_tiles + g3 - 1) / g3 > tsb::EXP_MAX_OWN) return TSB_EINVAL;
+  auto* d_mask = reinterpret_cast<unsigned long long*>(ex.d_cmask);
+  k1<<<g1, tsb::PW_THREADS, smem1, s>>>(arena, prm, h->d_wtab, d_mask, ex.d_tile, ex.d_st);
+  k3<<<g3, tsb::PW_THREADS, smem3, s>>>(arena, prm, d_mask, ex.d_tile, children_d, ex.d_st, ex.d_res);
+  TSB_CUDA(cudaGetLastError());
+  h->launches += 2;
+  return TSB_OK;
+}
+
 // generate_children of pfsp_gpu_chpl.chpl:273-303 on host arrays (the sequential rule, used by the slow path)
-void pfsp_generate_children_host(int jobs, const tsb_pfsp_node* parents, int size, const int32_t* bounds,
-                                 int64_t* best, std::vector<tsb_pfsp_node>* kids, uint64_t* sol) {
+template <class Node>
+void pfsp_generate_children_host(int jobs, const Node* parents, int size, const int32_t* bounds, int64_t* best,
+                                 std::vector<Node>* kids, uint64_t* sol) {
   for (int i = 0; i < size; i++) {
-    const tsb_pfsp_node& parent = parents[i];
+    const Node& parent = parents[i];
     const int depth = parent.depth;
     for (int j = parent.limit1 + 1; j < jobs; j++) {
       const int32_t lb = bounds[j + static_cast<size_t>(i) * jobs];
@@ -1628,7 +1656,7 @@ void pfsp_generate_children_host(int jobs, const tsb_pfsp_node* parents, int siz
         ++*sol;
         if (lb < *best) *best = lb;
       } else if (lb < *best) {
-        tsb_pfsp_node c = parent;
+        Node c = parent;
         c.depth = depth + 1;
         c.limit1 = parent.limit1 + 1;
         std::swap(c.prmu[depth], c.prmu[j]);
@@ -1644,16 +1672,21 @@ int pfsp_expand_round(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const std:
                       uint8_t* children_d, cudaStream_t s, int64_t* best, unsigned long long* n_children,
                       unsigned long long* n_solutions, bool early = false) {
   tsb::ExpandParams prm;
-  int rc = make_params(pieces, tsb::PF_TILE, &prm);
+  const bool wide = h->tab->wide;
+  const int tile = wide ? tsb::PW_TILE : tsb::PF_TILE;
+  int rc = make_params(pieces, tile, &prm);
   if (rc != TSB_OK) return rc;
   const int best_launch = clamp_best(*best);
   ExpandCtx& ex = h->ex;
-  rc = ex.reserve(std::max<long long>(prm.n_tiles, h->M_max / tsb::PF_TILE + 2 * tsb::EXP_MAX_PIECES), tsb::PF_TILE * 4, s);
+  // (side array: one child mask per parent, 32 bits for 20 jobs, 64 for 50)
+  rc = ex.reserve(std::max<long long>(prm.n_tiles, h->M_max / tile + 2 * tsb::EXP_MAX_PIECES), wide ? tile * 8 : tile * 4, s);
   if (rc != TSB_OK) return rc;
   prm.epoch = ++ex.epoch;
   prm.best = best_launch;
   rc = with_machines(h->tab->mt, [&](auto mt) {
-    return pfsp_expand_m<decltype(mt)::value>(h, lb_kind, arena, prm, children_d, s);
+    constexpr int M = decltype(mt)::value;
+    return wide ? pfsp_wide_expand_m<M>(h, lb_kind, arena, prm, children_d, s)
+                : pfsp_expand_m<M>(h, lb_kind, arena, prm, children_d, s);
   });
   if (rc != TSB_OK) return rc;
   rc = ex.wait_result(prm.epoch, s, early);
@@ -1672,40 +1705,53 @@ int pfsp_expand_round(tsb_pfsp* h, int lb_kind, const uint8_t* arena, const std:
   long long n = 0;
   for (const PoolExtent& x : pieces) n += x.e - x.b;
   if (n > h->M_max) return TSB_EINVAL;  // (cannot happen: every entry point checks count <= M_max first)
+  const size_t rec = h->in_rec;  // (the node record: 88 or 208 bytes)
   long long at = 0;
   if (!(arena == h->d_in && pieces.size() == 1 && pieces[0].b == 0))
     for (const PoolExtent& x : pieces) {  // the chunk, contiguous
-      TSB_CUDA(cudaMemcpyAsync(h->d_in + at * sizeof(tsb_pfsp_node), arena + x.b * sizeof(tsb_pfsp_node),
-                               static_cast<size_t>(x.e - x.b) * sizeof(tsb_pfsp_node), cudaMemcpyDeviceToDevice, s));
+      TSB_CUDA(cudaMemcpyAsync(h->d_in + at * rec, arena + x.b * rec, static_cast<size_t>(x.e - x.b) * rec,
+                               cudaMemcpyDeviceToDevice, s));
       at += x.e - x.b;
     }
   rc = launch_pfsp(h, lb_kind, h->d_in, h->d_out, n, *best, s);
   if (rc != TSB_OK) return rc;
-  h->h_chunk.resize(static_cast<size_t>(n));
-  h->h_bounds.resize(static_cast<size_t>(n) * h->tab->jobs);
-  rc = h->copy_d2h(h->h_chunk.data(), h->d_in, static_cast<size_t>(n) * sizeof(tsb_pfsp_node), s);
-  if (rc == TSB_OK) rc = h->copy_d2h(h->h_bounds.data(), h->d_out, static_cast<size_t>(n) * h->tab->jobs * 4, s);
-  if (rc != TSB_OK) return rc;
-  h->h_kids.clear();
-  uint64_t sol = 0;
-  pfsp_generate_children_host(h->tab->jobs, h->h_chunk.data(), static_cast<int>(n), h->h_bounds.data(), best, &h->h_kids,
-                              &sol);
-  rc = h->copy_h2d(children_d, h->h_kids.data(), h->h_kids.size() * sizeof(tsb_pfsp_node), s);
-  if (rc != TSB_OK) return rc;
-  *n_children = h->h_kids.size();
-  *n_solutions = sol;
-  return TSB_OK;
+  const auto redo = [&](auto& chunk, auto& kids) -> int {
+    using Node = typename std::decay_t<decltype(chunk)>::value_type;
+    chunk.resize(static_cast<size_t>(n));
+    h->h_bounds.resize(static_cast<size_t>(n) * h->tab->jobs);
+    int r = h->copy_d2h(chunk.data(), h->d_in, static_cast<size_t>(n) * sizeof(Node), s);
+    if (r == TSB_OK) r = h->copy_d2h(h->h_bounds.data(), h->d_out, static_cast<size_t>(n) * h->tab->jobs * 4, s);
+    if (r != TSB_OK) return r;
+    kids.clear();
+    uint64_t sol = 0;
+    pfsp_generate_children_host(h->tab->jobs, chunk.data(), static_cast<int>(n), h->h_bounds.data(), best, &kids, &sol);
+    r = h->copy_h2d(children_d, kids.data(), kids.size() * sizeof(Node), s);
+    if (r != TSB_OK) return r;
+    *n_children = kids.size();
+    *n_solutions = sol;
+    return TSB_OK;
+  };
+  return wide ? redo(h->h_chunk50, h->h_kids50) : redo(h->h_chunk, h->h_kids);
 }
 
 // (the PFSP pool only ever lives in its plain arena)
 int pfsp_plain() { return TSB_OK; }
 
+// one round of h's device pool (tsb_pfsp_pool_step after its checks; on 50-job handles, the searches' rounds)
+int pfsp_step(tsb_pfsp* h, int lb_kind, int m, int M, int64_t* best, int64_t* n_parents, uint64_t* n_children,
+              uint64_t* n_solutions) {
+  return pool_step(*h, m, M, n_parents, n_children, n_solutions, pfsp_plain,
+                   [h, lb_kind, best](auto arena, const auto& pieces, auto kids, auto nc, auto ns) {
+                     return pfsp_expand_round(h, lb_kind, arena, pieces, kids, h->stream, best, nc, ns, /*early=*/true);
+                   });
+}
+
 // CTAs of the persistent PFSP kernel for chunks of up to M parents (one per SM at most, each with up to PFR_SLICE
 // parents; fewer CTAs for smaller M, so that the two exchanges of a round involve only the CTAs that have parents to
 // evaluate); 0: the loop of tsb_pfsp_pool_step runs instead (lb2, M above PFR_MAX_M where the step loop is faster, M
-// beyond pf_pool_capacity, no cooperative launch, env TSB200_NO_ROUNDS=1)
+// beyond pf_pool_capacity, no cooperative launch, env TSB200_NO_ROUNDS=1, a 50-job handle)
 int pfsp_rounds_grid(const tsb_pfsp* h, int lb_kind, int M) {
-  if (lb_kind == TSB_LB2 || !h->di.coop || env_no_rounds()) return 0;
+  if (lb_kind == TSB_LB2 || h->tab->wide || !h->di.coop || env_no_rounds()) return 0;
   if (M > tsb::PFR_MAX_M || M > tsb::pf_pool_capacity(h->di.sms, 1)) return 0;
   return static_cast<int>(std::min<long long>(tsb::pf_ctas_per_pool(h->di.sms, 1),
                                               (static_cast<long long>(M) + tsb::PF_TILE - 1) / tsb::PF_TILE));
@@ -1722,9 +1768,9 @@ int with_pfsp_rounds_kernel(const tsb_pfsp* h, int lb_kind, F&& f) {
 constexpr size_t kPfRoundsSmem = sizeof(tsb::PfRoundsSmem) + 128;
 // CTAs per pool when one launch of the persistent kernel serves `pools` >= 2 pools with chunks of up to M parents
 // (pf_ctas_per_pool, fewer for small M as in pfsp_rounds_grid); 0: not in one launch (lb2, no cooperative launch, env
-// TSB200_NO_ROUNDS=1, M beyond pf_pool_capacity, or the kernel does not fit twice on an SM)
+// TSB200_NO_ROUNDS=1, a 50-job handle, M beyond pf_pool_capacity, or the kernel does not fit twice on an SM)
 int pfsp_multi_grid(tsb_pfsp* h, int lb_kind, int M, int pools) {
-  if (lb_kind == TSB_LB2 || !h->di.coop || env_no_rounds() || pools < 2 || pools > tsb::PFR_MAX_POOLS) return 0;
+  if (lb_kind == TSB_LB2 || h->tab->wide || !h->di.coop || env_no_rounds() || pools < 2 || pools > tsb::PFR_MAX_POOLS) return 0;
   if (M > tsb::pf_pool_capacity(h->di.sms, pools)) return 0;
   int per_sm = 0;
   if (with_pfsp_rounds_kernel(h, lb_kind, [&](auto kernel) -> int {
@@ -1786,7 +1832,7 @@ struct PfspRounds {
     return step_loop(1, out, [&](int64_t* np, uint64_t* nc, uint64_t* ns) { return step(h, i, m, M, np, nc, ns); });
   }
   int step(tsb_pfsp* h, int i, int m, int M, int64_t* np, uint64_t* nc, uint64_t* ns) const {
-    return tsb_pfsp_pool_step(h, lb_kind, m, M, &best[i], np, nc, ns);
+    return pfsp_step(h, lb_kind, m, M, &best[i], np, nc, ns);
   }
   // TSB200_ROUNDS_PROF: CTA 0's phases of each pool
   void report(const tsb::RoundsState* pace, const int*, int n_act, int) const {
@@ -1811,8 +1857,15 @@ int pfsp_open(int device, int M_max, std::shared_ptr<const PfspPacked> tab, tsb_
   h->tab = std::move(tab);
   const PfspPacked& t = *h->tab;
   const size_t rec = t.wide ? tsb::PW_REC : sizeof(tsb_pfsp_node);
-  // (88-byte nodes: extents on even records start on a 16-byte boundary)
-  h->pool.set_format(rec, tsb::PF_TILE, 2, t.jobs, std::max<long long>(1LL << 20, 4LL * M_max * t.jobs));
+  if (t.wide)
+    // (208-byte nodes start on a 16-byte boundary anywhere.)  The arena starts with room for one worst-case round
+    // (every slot of M_max parents survives) above a pool of 2 M_max nodes: 2.6 M nodes, 541 MB at M = 50000.  The
+    // 20-job rule (four worst-case rounds) would be 2 GB per arena, and a search task holds two arenas per pool,
+    // pools per task and tasks per GPU; a 50-job search under --ub 1 keeps far fewer nodes than its worst case, and
+    // a pool that does outgrow the arena doubles it (DevicePool::reserve).
+    h->pool.set_format(rec, tsb::PW_TILE, 1, t.jobs, std::max<long long>(1LL << 16, static_cast<long long>(M_max) * (t.jobs + 2)));
+  else  // (88-byte nodes: extents on even records start on a 16-byte boundary)
+    h->pool.set_format(rec, tsb::PF_TILE, 2, t.jobs, std::max<long long>(1LL << 20, 4LL * M_max * t.jobs));
   int rc = h->init(device, M_max, rec, static_cast<size_t>(t.jobs) * 4);
   if (rc == TSB_OK && !t.valid) rc = TSB_EINVAL;
   auto upload = [h](auto** dst, const auto& src) -> int {
@@ -2144,8 +2197,9 @@ int tsb_pfsp_create(tsb_pfsp** out, int device, int jobs, int machines, int M_ma
 }
 
 // The reference built with MAX_JOBS = max_jobs (lib/pfsp/PFSP_node.chpl:7): 20 = tsb_pfsp_create; 50 = 208-byte nodes,
-// jobs == 50 instances (ta031..ta060), evaluated by the general kernels of pfsp_wide.cuh (evaluate / evaluate_device
-// only: the fused expand and the device pool are specialised for 20 jobs)
+// jobs == 50 instances (ta031..ta060), evaluated by the general kernels of pfsp_wide.cuh.  The exported expand, pool,
+// sibling and run_multi entry points refuse such a handle (TSB_EUNSUPPORTED); the 50-job searches of tsb_host.cpp reach
+// its device pool (pfsp_wide_expand.cuh) through the library-internal functions of pfsp_search_pool.h.
 int tsb_pfsp_create_wide(tsb_pfsp** out, int device, int max_jobs, int jobs, int machines, int M_max, const int32_t* p_times,
                          const int32_t* min_heads, const int32_t* min_tails, int nb_pairs, const int32_t* johnson,
                          const int32_t* lags, const int32_t* mp0, const int32_t* mp1, const int32_t* mp_order) {
@@ -2246,10 +2300,7 @@ int tsb_pfsp_pool_step(tsb_pfsp* h, int lb_kind, int m, int M, int64_t* best, in
                        uint64_t* n_children, uint64_t* n_solutions) {
   if (int rc = pfsp_check(h, true, lb_kind); rc != TSB_OK) return rc;
   if (m < 1 || M < 1 || M > h->M_max || !best || !n_parents || !n_children || !n_solutions) return TSB_EINVAL;
-  return pool_step(*h, m, M, n_parents, n_children, n_solutions, pfsp_plain,
-                   [h, lb_kind, best](auto arena, const auto& pieces, auto kids, auto nc, auto ns) {
-                     return pfsp_expand_round(h, lb_kind, arena, pieces, kids, h->stream, best, nc, ns, /*early=*/true);
-                   });
+  return pfsp_step(h, lb_kind, m, M, best, n_parents, n_children, n_solutions);
 }
 
 int tsb_pfsp_pool_steal(tsb_pfsp* victim, tsb_pfsp* thief, int m, int64_t* n_stolen) {
@@ -2300,3 +2351,32 @@ int tsb_pfsp_pool_run_multi(tsb_pfsp* const* handles, int n_pools, int lb_kind, 
 }
 
 }  // extern "C"
+
+// ============================================================================ library-internal (pfsp_search_pool.h)
+namespace tsb::search {
+
+int pfsp_pool_push(tsb_pfsp* h, const void* nodes, int64_t n) {
+  if (!h || !h->tab->wide) return tsb_pfsp_pool_push(h, nodes, n);
+  if (n < 0 || (n && !nodes)) return TSB_EINVAL;
+  return pool_push(*h, nodes, n, pfsp_plain);
+}
+
+int pfsp_sibling(tsb_pfsp* h, int index, tsb_pfsp** sibling) {
+  if (!h || !h->tab->wide) return tsb_pfsp_sibling(h, index, sibling);
+  return sibling_of(h, index, sibling, [h](tsb_pfsp** s) { return pfsp_open(h->device, h->M_max, h->tab, s); });
+}
+
+int pfsp_pool_run_multi(tsb_pfsp* const* handles, int n_pools, int lb_kind, int m, int M, int64_t max_rounds,
+                        int64_t* best, uint64_t* out) {
+  if (!handles || !handles[0] || !handles[0]->tab->wide)
+    return tsb_pfsp_pool_run_multi(handles, n_pools, lb_kind, m, M, max_rounds, best, out);
+  if (n_pools < 1 || n_pools > tsb::PFR_MAX_POOLS || m < 1 || M < 1 || max_rounds < 0 || !best || !out) return TSB_EINVAL;
+  for (int i = 0; i < n_pools; i++)
+    if (int rc = pfsp_check(handles[i], false, lb_kind); rc != TSB_OK) return rc;
+  if (!one_group(handles, n_pools, M, [](const tsb_pfsp& h, const tsb_pfsp& h0) { return h.tab->wide == h0.tab->wide; }))
+    return TSB_EINVAL;
+  // (no persistent kernel takes 208-byte nodes: PfspRounds::grid is 0, and the pools run their rounds in turn)
+  return pool_run_multi(PfspRounds{lb_kind, best}, handles, n_pools, m, M, max_rounds, out);
+}
+
+}  // namespace tsb::search

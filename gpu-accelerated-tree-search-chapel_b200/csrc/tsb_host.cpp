@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "ll_tiers.h"
+#include "pfsp_search_pool.h"
 #include "search_ckpt.h"
 #include "tsb200.h"
 
@@ -339,13 +340,13 @@ inline bool steal_allowed() { return !std::getenv("TSB200_NO_STEAL"); }
 inline int64_t pool_size(const tsb_nq* h) { return tsb_nq_pool_size(h); }
 inline int64_t pool_size(const tsb_pfsp* h) { return tsb_pfsp_pool_size(h); }
 inline int pool_push(tsb_nq* h, const void* nodes, int64_t n) { return tsb_nq_pool_push(h, nodes, n); }
-inline int pool_push(tsb_pfsp* h, const void* nodes, int64_t n) { return tsb_pfsp_pool_push(h, nodes, n); }
+inline int pool_push(tsb_pfsp* h, const void* nodes, int64_t n) { return tsb::search::pfsp_pool_push(h, nodes, n); }
 inline int pool_drain(tsb_nq* h, void* nodes, int64_t cap, int64_t* n) { return tsb_nq_pool_drain(h, nodes, cap, n); }
 inline int pool_drain(tsb_pfsp* h, void* nodes, int64_t cap, int64_t* n) { return tsb_pfsp_pool_drain(h, nodes, cap, n); }
 inline int pool_steal(tsb_nq* v, tsb_nq* t, int m, int64_t* got) { return tsb_nq_pool_steal(v, t, m, got); }
 inline int pool_steal(tsb_pfsp* v, tsb_pfsp* t, int m, int64_t* got) { return tsb_pfsp_pool_steal(v, t, m, got); }
 inline int pool_sibling(tsb_nq* h, int i, tsb_nq** sib) { return tsb_nq_sibling(h, i, sib); }
-inline int pool_sibling(tsb_pfsp* h, int i, tsb_pfsp** sib) { return tsb_pfsp_sibling(h, i, sib); }
+inline int pool_sibling(tsb_pfsp* h, int i, tsb_pfsp** sib) { return tsb::search::pfsp_sibling(h, i, sib); }
 inline uint64_t kernel_launches(const tsb_nq* h) { return tsb_nq_kernel_launches(h); }
 inline uint64_t kernel_launches(const tsb_pfsp* h) { return tsb_pfsp_kernel_launches(h); }
 
@@ -587,9 +588,14 @@ int64_t unif(int64_t& seed, int64_t low, int64_t high) {  // lib/pfsp/Taillard.c
   return low + static_cast<int64_t>(v * static_cast<double>(high - low + 1));
 }
 
-struct HostBounds {  // CPU bounds used by decompose in steps 1 and 3 (pfsp_gpu_chpl.chpl:88-189)
-  const tsb_pfsp_tables& t;
-  explicit HostBounds(const tsb_pfsp_tables& tt) : t(tt) {}
+// CPU bounds used by decompose in steps 1 and 3 (pfsp_gpu_chpl.chpl:88-189), on the tables of a MAX_JOBS = 20
+// (tsb_pfsp_tables) or 50 (tsb_pfsp_tables50) build
+template <class Tables>
+struct HostBounds {
+  static constexpr int kMaxJobs = sizeof(Tables::p_times) / sizeof(int32_t) / TSB_MAX_MACHINES;
+  static_assert(kMaxJobs <= 64, "the scheduled set of lb2 is a 64-bit mask");
+  const Tables& t;
+  explicit HostBounds(const Tables& tt) : t(tt) {}
   void front_of(const int32_t* prmu, int limit1, int32_t* F) const {  // schedule_front
     const int N = t.jobs, M = t.machines;
     if (limit1 == -1) {
@@ -627,7 +633,7 @@ struct HostBounds {  // CPU bounds used by decompose in steps 1 and 3 (pfsp_gpu_
     int32_t F[TSB_MAX_MACHINES], R[TSB_MAX_MACHINES];
     front_of(prmu, limit1, F);
     remain_of(prmu, limit1, R);
-    std::fill(lb_begin, lb_begin + TSB_MAX_JOBS, 0);
+    std::fill(lb_begin, lb_begin + kMaxJobs, 0);
     for (int i = limit1 + 1; i < N; i++) {
       const int job = prmu[i];
       int32_t lb = F[0] + R[0] + t.min_tails[0], tmp0 = F[0] + t.p_times[job];
@@ -643,15 +649,15 @@ struct HostBounds {  // CPU bounds used by decompose in steps 1 and 3 (pfsp_gpu_
     const int N = t.jobs;
     int32_t F[TSB_MAX_MACHINES];
     front_of(prmu, limit1, F);
-    uint32_t sched = 0;
-    for (int j = 0; j <= limit1; j++) sched |= 1u << prmu[j];
+    uint64_t sched = 0;
+    for (int j = 0; j <= limit1; j++) sched |= 1ull << prmu[j];
     int32_t lb = 0;
     for (int l = 0; l < t.pairs; l++) {
       const int i = t.mp_order[l], a = t.mp0[i], b = t.mp1[i];
       int32_t t0 = F[a], t1 = F[b];
       for (int j = 0; j < N; j++) {
         const int job = t.johnson[i * N + j];
-        if (!((sched >> job) & 1u)) {
+        if (!((sched >> job) & 1ull)) {
           t0 += t.p_times[a * N + job];
           t1 = std::max(t1, t0 + t.lags[i * N + job]) + t.p_times[b * N + job];
         }
@@ -663,7 +669,8 @@ struct HostBounds {  // CPU bounds used by decompose in steps 1 and 3 (pfsp_gpu_
   }
 };
 
-inline void pfsp_child(const tsb_pfsp_node& parent, int i, tsb_pfsp_node& c) {
+template <class Node>
+inline void pfsp_child(const Node& parent, int i, Node& c) {
   c = parent;
   c.depth = parent.depth + 1;
   c.limit1 = parent.limit1 + 1;
@@ -671,13 +678,14 @@ inline void pfsp_child(const tsb_pfsp_node& parent, int i, tsb_pfsp_node& c) {
 }
 
 // decompose (pfsp_gpu_chpl.chpl:88-189)
-void pfsp_decompose(const HostBounds& hb, int lb_kind, const tsb_pfsp_node& parent, uint64_t& tree,
-                    uint64_t& sol, int64_t& best, Pool<tsb_pfsp_node>& pool) {
+template <class Tables, class Node>
+void pfsp_decompose(const HostBounds<Tables>& hb, int lb_kind, const Node& parent, uint64_t& tree, uint64_t& sol,
+                    int64_t& best, Pool<Node>& pool) {
   const int jobs = hb.t.jobs;
-  int32_t lb_begin[TSB_MAX_JOBS];
+  int32_t lb_begin[HostBounds<Tables>::kMaxJobs];
   if (lb_kind == TSB_LB1_D) hb.lb1_children(parent.prmu, parent.limit1, lb_begin);
   for (int i = parent.limit1 + 1; i < jobs; i++) {
-    tsb_pfsp_node c;
+    Node c;
     pfsp_child(parent, i, c);
     const int32_t lb = lb_kind == TSB_LB1_D ? lb_begin[parent.prmu[i]]
                        : lb_kind == TSB_LB1 ? hb.lb1(c.prmu, c.limit1)
@@ -693,10 +701,11 @@ void pfsp_decompose(const HostBounds& hb, int lb_kind, const tsb_pfsp_node& pare
 }
 
 // generate_children (pfsp_gpu_chpl.chpl:273-303)
-void pfsp_generate_children(int jobs, const tsb_pfsp_node* parents, int size, const int32_t* bounds,
-                            uint64_t& tree, uint64_t& sol, int64_t& best, Pool<tsb_pfsp_node>& pool) {
+template <class Node>
+void pfsp_generate_children(int jobs, const Node* parents, int size, const int32_t* bounds, uint64_t& tree,
+                            uint64_t& sol, int64_t& best, Pool<Node>& pool) {
   for (int i = 0; i < size; i++) {
-    const tsb_pfsp_node& parent = parents[i];
+    const Node& parent = parents[i];
     const int depth = parent.depth;
     for (int j = parent.limit1 + 1; j < jobs; j++) {
       const int32_t lb = bounds[j + static_cast<size_t>(i) * jobs];
@@ -704,7 +713,7 @@ void pfsp_generate_children(int jobs, const tsb_pfsp_node* parents, int size, co
         ++sol;
         if (lb < best) best = lb;
       } else if (lb < best) {
-        tsb_pfsp_node c;
+        Node c;
         pfsp_child(parent, j, c);
         pool.pushBack(c);
         ++tree;
@@ -862,18 +871,29 @@ struct NqSearch {
   }
 };
 
-// PFSP on the tables of a Taillard instance; `pools` device pools per task, as many as the caller asks for
+// a handle of the build the tables are for: tsb_pfsp_create (20 jobs) or tsb_pfsp_create_wide (50 jobs)
+inline int pfsp_create_for(tsb_pfsp** h, int device, int M, const tsb_pfsp_tables* t) {
+  return tsb_pfsp_create_from_tables(h, device, M, t);
+}
+inline int pfsp_create_for(tsb_pfsp** h, int device, int M, const tsb_pfsp_tables50* t) {
+  return tsb_pfsp_create50_from_tables(h, device, M, t);
+}
+
+// PFSP on the tables of a Taillard instance; `pools` device pools per task, as many as the caller asks for.
+// Node / Tables: tsb_pfsp_node / tsb_pfsp_tables (MAX_JOBS = 20) or tsb_pfsp_node50 / tsb_pfsp_tables50 (MAX_JOBS = 50:
+// 50-job handles, whose device pools run one after the other, with no shared launch)
+template <class NodeT, class Tables>
 struct PfspSearch {
-  using Node = tsb_pfsp_node;
+  using Node = NodeT;
   using Handle = tsb_pfsp;
-  HostBounds hb;
+  HostBounds<Tables> hb;
   int lb_kind;
   bool devpool;
   int pools;
   // moves between pools keep the counts only while best is constant: --ub 1 (SURVEY A.6)
   bool steal, balance;
   int64_t initial_best;
-  PfspSearch(const tsb_pfsp_tables& t, int inst, int lb_kind_, int ub, bool devpool_, int pools_)
+  PfspSearch(const Tables& t, int inst, int lb_kind_, int ub, bool devpool_, int pools_)
       : hb(t), lb_kind(lb_kind_), devpool(devpool_), pools(pools_), steal(devpool_ && ub == 1 && steal_allowed()),
         balance(pools_ > 1 && ub == 1 && steal_allowed()),
         initial_best(ub == 1 ? tsb_taillard_best_ub(inst) : INT64_MAX) {}  // pfsp_gpu_chpl.chpl:37
@@ -888,13 +908,13 @@ struct PfspSearch {
   }
   void host_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r) const {
     tsb_pfsp* h = nullptr;
-    r.rc = tsb_pfsp_create_from_tables(&h, device, M, &hb.t);
+    r.rc = pfsp_create_for(&h, device, M, &hb.t);
     if (r.rc != TSB_OK) return;
     const int jobs = hb.t.jobs;
-    std::vector<tsb_pfsp_node> parents(M);
+    std::vector<Node> parents(M);
     std::vector<int32_t> bounds(static_cast<size_t>(M) * jobs);
     // the chunk arrays live for the whole step 2 (pfsp_gpu_chpl.chpl:355-356): page-lock them once
-    tsb_pfsp_register_host(h, parents.data(), parents.size() * sizeof(tsb_pfsp_node));
+    tsb_pfsp_register_host(h, parents.data(), parents.size() * sizeof(Node));
     tsb_pfsp_register_host(h, bounds.data(), bounds.size() * sizeof(int32_t));
     for (;;) {
       const int n = pool.popBackBulk(m, M, parents.data());
@@ -911,7 +931,7 @@ struct PfspSearch {
   void device_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me,
                    TaskCkpt* ck) const {
     tsb_pfsp* h = nullptr;
-    r.rc = tsb_pfsp_create_from_tables(&h, device, M, &hb.t);
+    r.rc = pfsp_create_for(&h, device, M, &hb.t);
     if (r.rc != TSB_OK) {
       if (sb) sb->publish_handle(me, nullptr, 0);
       return;
@@ -922,7 +942,7 @@ struct PfspSearch {
   int pools_on(tsb_pfsp*, int) const { return pools; }
   int64_t rounds(int, bool sb, int M) const { return rounds_per_call(balance || sb, M); }
   int run_multi(tsb_pfsp* const* hs, int P, int m, int M, int64_t rounds, int64_t* best, uint64_t* out) const {
-    return tsb_pfsp_pool_run_multi(hs, P, lb_kind, m, M, rounds, best, out);
+    return tsb::search::pfsp_pool_run_multi(hs, P, lb_kind, m, M, rounds, best, out);
   }
 };
 
@@ -1109,17 +1129,27 @@ int nq_search(int N, int g, int m, int M, int D, bool devpool, int part, int dev
   return three_step_search(NqSearch<Node>(N, g, M, devpool), m, M, D, part, device, on, out, ck);
 }
 
-// pools > 1 (device pools only): every task's share split once more into `pools` device pools (devpool_on)
+inline int pfsp_tables_for(tsb_pfsp_tables* t, int inst) { return tsb_pfsp_tables_build(t, inst); }
+inline int pfsp_tables_for(tsb_pfsp_tables50* t, int inst) {
+  // (the 50-job instances only: tsb_pfsp_tables50_build also takes the smaller ones)
+  if (inst < 31 || inst > 60) return TSB_EUNSUPPORTED;
+  return tsb_pfsp_tables50_build(t, inst, TSB_LB2_FULL);
+}
+
+// pools > 1 (device pools only): every task's share split once more into `pools` device pools (devpool_on).
+// Node: tsb_pfsp_node (a MAX_JOBS = 20 build) or tsb_pfsp_node50 (MAX_JOBS = 50, ta031..ta060).
+template <class Node = tsb_pfsp_node>
 int pfsp_search(int inst, int lb_kind, int ub, int m, int M, int D, bool devpool, int part, int device, tsb_pfsp* on,
                 tsb_search_stats* out, int pools = 1, SearchCkpt* ck = nullptr) {
+  using Tables = std::conditional_t<std::is_same_v<Node, tsb_pfsp_node50>, tsb_pfsp_tables50, tsb_pfsp_tables>;
   if (!out || lb_kind < 0 || lb_kind > 2 || (ub != 0 && ub != 1) || m < 1 || M < 1 || D < 1 || D > 8 || part >= D ||
       pools < 1 || pools > 4)
     return TSB_EINVAL;
   std::memset(out, 0, sizeof(*out));
-  std::vector<tsb_pfsp_tables> tv(1);
-  if (int rc = tsb_pfsp_tables_build(&tv[0], inst); rc != TSB_OK) return rc;
-  return three_step_search(PfspSearch(tv[0], inst, lb_kind, ub, devpool, pools), m, M, D, part, device, on, out,
-                           ck);
+  std::vector<Tables> tv(1);
+  if (int rc = pfsp_tables_for(&tv[0], inst); rc != TSB_OK) return rc;
+  return three_step_search(PfspSearch<Node, Tables>(tv[0], inst, lb_kind, ub, devpool, pools), m, M, D, part, device,
+                           on, out, ck);
 }
 
 // the resumable searches: resume from `path` if a checkpoint is there (refused before any device call if it is damaged
@@ -1283,6 +1313,23 @@ int tsb_pfsp_search_device_ckpt(int inst, int lb_kind, int ub, int m, int M, int
   const tsb::ckpt::Params p{tsb::ckpt::kPfsp, sizeof(tsb_pfsp_node), inst, lb_kind, ub, m, M, D, pools};
   return ckpt_search(path, seconds, p, [&](SearchCkpt* ck) {
     return pfsp_search(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out, pools, ck);
+  });
+}
+int tsb_pfsp_search_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, tsb_search_stats* out) {
+  if (max_jobs != TSB_MAX_JOBS_WIDE) return TSB_EINVAL;
+  return pfsp_search<tsb_pfsp_node50>(inst, lb_kind, ub, m, M, D, false, -1, 0, nullptr, out);
+}
+int tsb_pfsp_search_device_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, int pools,
+                                tsb_search_stats* out) {
+  if (max_jobs != TSB_MAX_JOBS_WIDE) return TSB_EINVAL;
+  return pfsp_search<tsb_pfsp_node50>(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out, pools);
+}
+int tsb_pfsp_search_device_ckpt_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, int pools,
+                                     const char* path, double seconds, tsb_search_stats* out) {
+  if (max_jobs != TSB_MAX_JOBS_WIDE) return TSB_EINVAL;
+  const tsb::ckpt::Params p{tsb::ckpt::kPfsp, sizeof(tsb_pfsp_node50), inst, lb_kind, ub, m, M, D, pools};
+  return ckpt_search(path, seconds, p, [&](SearchCkpt* ck) {
+    return pfsp_search<tsb_pfsp_node50>(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out, pools, ck);
   });
 }
 void tsb_search_request_stop(void) { g_stop_request.store(1); }

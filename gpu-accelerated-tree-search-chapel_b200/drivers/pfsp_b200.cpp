@@ -1,6 +1,7 @@
 // pfsp_b200 — C++ stand-in for pfsp_gpu_chpl / pfsp_multigpu_chpl.  Same CLI (--inst --lb --ub --m --M
 // --D; README.md:47-87), same defaults (pfsp_multigpu_chpl.chpl:24-30: inst 14, lb "lb1", ub 1), same
-// result lines (pfsp_gpu_chpl.chpl:66-77).  --lb takes the Chapel spelling lb1 | lb1_d | lb2.
+// result lines (pfsp_gpu_chpl.chpl:66-77).  --lb takes the Chapel spelling lb1 | lb1_d | lb2.  --max-jobs 50 runs
+// the program as the reference built with MAX_JOBS = 50 (lib/pfsp/PFSP_node.chpl:7): ta031..ta060.
 #include <csignal>
 #include <cstdio>
 #include <cstdlib>
@@ -20,7 +21,7 @@ static void on_stop_signals() {
 }
 
 int main(int argc, char** argv) {
-  int inst = 14, ub = 1, m = 25, M = 50000, D = 1, lb = TSB_LB1, devpool = 0, pools = 1;
+  int inst = 14, ub = 1, m = 25, M = 50000, D = 1, lb = TSB_LB1, devpool = 0, pools = 1, max_jobs = TSB_MAX_JOBS;
   const char* lbs = "lb1";
   const char* ckpt = nullptr;
   double limit = -1;
@@ -35,7 +36,8 @@ int main(int argc, char** argv) {
                   "   --checkpoint str  (with --devpool 1) resumable search: continue from FILE if it exists; on a stop\n"
                   "                     (--time-limit, SIGINT, SIGTERM) write FILE and exit with 4; rerun the same\n"
                   "                     command to resume; FILE is removed when the search ends\n"
-                  "   --time-limit real seconds of this run before it stops (0: after one call per task)\n\n");
+                  "   --time-limit real seconds of this run before it stops (0: after one call per task)\n"
+                  "   --max-jobs int   MAX_JOBS of the build (20, 50): 50 solves ta031..ta060 on 208-byte nodes\n\n");
       return 1;
     }
     if (i + 1 >= argc) break;
@@ -57,7 +59,7 @@ int main(int argc, char** argv) {
              : !std::strcmp(argv[i], "--m") ? &m : !std::strcmp(argv[i], "--M") ? &M
              : !std::strcmp(argv[i], "--D") ? &D
              : !std::strcmp(argv[i], "--devpool") ? &devpool  // 1: pool(s) of step 2 resident on the GPU
-             : !std::strcmp(argv[i], "--pools") ? &pools : nullptr;
+             : !std::strcmp(argv[i], "--pools") ? &pools : !std::strcmp(argv[i], "--max-jobs") ? &max_jobs : nullptr;
     if (dst) *dst = std::atoi(argv[++i]);
   }
   if (m <= 0 || M <= 0) { std::fprintf(stderr, "Error: m and M must be positive integers.\n"); return 2; }
@@ -70,6 +72,10 @@ int main(int argc, char** argv) {
     return 2;
   }
   if (inst < 1 || inst > 120) { std::fprintf(stderr, "Error: unsupported Taillard's instance\n"); return 2; }
+  if (max_jobs != TSB_MAX_JOBS && max_jobs != TSB_MAX_JOBS_WIDE) {
+    std::fprintf(stderr, "Error: --max-jobs must be %d or %d\n", TSB_MAX_JOBS, TSB_MAX_JOBS_WIDE);
+    return 2;
+  }
   if (lb < 0) { std::fprintf(stderr, "Error - Unsupported lower bound\n"); return 2; }
   if (ub != 0 && ub != 1) { std::fprintf(stderr, "Error: unsupported upper bound initialization\n"); return 2; }
   std::printf("\n=================================================\n%s H100 (tsb200)\n\n"
@@ -79,7 +85,11 @@ int main(int argc, char** argv) {
               ub ? "opt" : "inf", lbs);
   tsb_search_stats st;
   if (ckpt) on_stop_signals();
-  const int rc = ckpt        ? tsb_pfsp_search_device_ckpt(inst, lb, ub, m, M, D, pools, ckpt, limit, &st)
+  const bool wide = max_jobs == TSB_MAX_JOBS_WIDE;
+  const int rc = wide ? (ckpt       ? tsb_pfsp_search_device_ckpt_wide(max_jobs, inst, lb, ub, m, M, D, pools, ckpt, limit, &st)
+                         : !devpool ? tsb_pfsp_search_wide(max_jobs, inst, lb, ub, m, M, D, &st)
+                                    : tsb_pfsp_search_device_wide(max_jobs, inst, lb, ub, m, M, D, pools, &st))
+                 : ckpt      ? tsb_pfsp_search_device_ckpt(inst, lb, ub, m, M, D, pools, ckpt, limit, &st)
                  : !devpool  ? tsb_pfsp_search(inst, lb, ub, m, M, D, &st)
                  : pools > 1 ? tsb_pfsp_search_device_pools(inst, lb, ub, m, M, D, pools, &st)
                              : tsb_pfsp_search_device(inst, lb, ub, m, M, D, &st);

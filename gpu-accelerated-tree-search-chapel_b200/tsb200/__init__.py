@@ -17,10 +17,10 @@ from ._lib import (LB1, LB1_D, LB2, ROUTE_LB2, ROUTE_LB2U, ROUTE_MT_MASK, ROUTE_
 from .nqueens import (NQ_NODE_DTYPE, NQ_NODE24_DTYPE, NQueensEvaluator, nq_node_dtype, nqueens_search, nqueens_search_device,
                       nqueens_pool_run_multi, nqueens_search_device_part, nqueens_warmup)
 from .pfsp import (PFSP_NODE_DTYPE, PFSP_NODE50_DTYPE, LB_NAMES, LB2_VARIANTS, PfspEvaluator, taillard_tables50, pfsp_search, pfsp_search_device,
-                   pfsp_search_device_part, pfsp_pool_run_multi, taillard_tables)
+                   pfsp_search_device_part, pfsp_search_device_wide, pfsp_search_wide, pfsp_pool_run_multi, taillard_tables)
 
 __all__ = ["NQueensEvaluator", "PfspEvaluator", "nqueens_warmup", "nqueens_pool_run_multi", "nqueens_search", "nqueens_search_device", "nqueens_search_device_part", "pfsp_search", "pfsp_search_device",
-           "pfsp_search_device_part", "pfsp_pool_run_multi",
+           "pfsp_search_device_part", "pfsp_search_wide", "pfsp_search_device_wide", "pfsp_pool_run_multi",
            "taillard_tables",
            "NQ_NODE_DTYPE", "NQ_NODE24_DTYPE", "nq_node_dtype", "PFSP_NODE_DTYPE", "PFSP_NODE50_DTYPE", "LB2_VARIANTS", "taillard_tables50", "LB_NAMES", "LB1", "LB1_D", "LB2", "TsbError", "SearchStopped", "request_stop", "lib", "check",
            "PfspTables", "PfspTables50", "SearchStats", "XFER_AUTO", "XFER_MEMCPY", "XFER_ZEROCOPY",

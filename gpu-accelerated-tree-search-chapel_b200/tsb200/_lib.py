@@ -160,6 +160,10 @@ SYMBOLS = {
     "tsb_pfsp_search_on_pools": (_i, [_vp, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
     "tsb_nq_search_device_ckpt": (_i, [_i, _i, _i, _i, _i, _i, C.c_char_p, C.c_double, C.POINTER(SearchStats)]),
     "tsb_pfsp_search_device_ckpt": (_i, [_i, _i, _i, _i, _i, _i, _i, C.c_char_p, C.c_double, C.POINTER(SearchStats)]),
+    "tsb_pfsp_search_wide": (_i, [_i, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
+    "tsb_pfsp_search_device_wide": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, C.POINTER(SearchStats)]),
+    "tsb_pfsp_search_device_ckpt_wide": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, C.c_char_p, C.c_double,
+                                              C.POINTER(SearchStats)]),
     "tsb_search_request_stop": (None, []),
 }
 

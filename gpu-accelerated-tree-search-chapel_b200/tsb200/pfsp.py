@@ -213,6 +213,34 @@ def pfsp_search(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: int = 500
     return st
 
 
+MAX_JOBS_WIDE = 50
+
+
+def pfsp_search_wide(inst: int = 31, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1) -> SearchStats:
+    """pfsp_search as the reference built with MAX_JOBS = 50 runs it (tsb_pfsp_search_wide): ta031..ta060, 208-byte
+    nodes"""
+    kind = _lb(lb)
+    st = SearchStats()
+    check(lib().tsb_pfsp_search_wide(MAX_JOBS_WIDE, inst, kind, ub, m, M, D, C.byref(st)), "tsb_pfsp_search_wide")
+    return st
+
+
+def pfsp_search_device_wide(inst: int = 31, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1,
+                            pools: int = 1, checkpoint=None, time_limit: float | None = None) -> SearchStats:
+    """pfsp_search_device as the reference built with MAX_JOBS = 50 runs it (tsb_pfsp_search_device_wide; with
+    checkpoint / time_limit the resumable tsb_pfsp_search_device_ckpt_wide)"""
+    kind = _lb(lb)
+    st = SearchStats()
+    if checkpoint is not None:
+        check_search(lib().tsb_pfsp_search_device_ckpt_wide(MAX_JOBS_WIDE, inst, kind, ub, m, M, D, pools,
+                                                            *ckpt_args(checkpoint, time_limit), C.byref(st)),
+                     "tsb_pfsp_search_device_ckpt_wide", st)
+    else:
+        check(lib().tsb_pfsp_search_device_wide(MAX_JOBS_WIDE, inst, kind, ub, m, M, D, pools, C.byref(st)),
+              "tsb_pfsp_search_device_wide")
+    return st
+
+
 def pfsp_search_device_part(inst: int, lb, ub: int, m: int, M: int, D: int, part: int, device: int = 0,
                             pools: int = 1) -> SearchStats:
     kind = _lb(lb)

@@ -253,8 +253,10 @@ int tsb_pfsp_create(tsb_pfsp** h, int device, int jobs, int machines, int M_max,
                     const int32_t* mp_order);
 /* SURVEY §8(f4): the reference built with MAX_JOBS = max_jobs.  max_jobs == 20: tsb_pfsp_create.  max_jobs == 50:
  * nodes are 208-byte tsb_pfsp_node50 records, jobs must be 50 (ta031..ta060), bounds[p*50 + k]; tsb_pfsp_evaluate /
- * tsb_pfsp_evaluate_device work on such a handle (general kernels, csrc/pfsp_wide.cuh), the fused expand / pool
- * entry points return TSB_EUNSUPPORTED.  Table layouts as for tsb_pfsp_create with jobs = 50. */
+ * tsb_pfsp_evaluate_device work on such a handle (general kernels, csrc/pfsp_wide.cuh), the fused expand, pool,
+ * sibling and run_multi entry points return TSB_EUNSUPPORTED.  The 50-job searches (tsb_pfsp_search_*_wide) run
+ * device pools of 208-byte nodes on handles of their own, through functions internal to the library
+ * (csrc/pfsp_search_pool.h).  Table layouts as for tsb_pfsp_create with jobs = 50. */
 int tsb_pfsp_create_wide(tsb_pfsp** h, int device, int max_jobs, int jobs, int machines, int M_max, const int32_t* p_times,
                          const int32_t* min_heads, const int32_t* min_tails, int nb_pairs, const int32_t* johnson,
                          const int32_t* lags, const int32_t* mp0, const int32_t* mp1, const int32_t* mp_order);
@@ -478,6 +480,22 @@ int tsb_nq_search_device_ckpt(int max_queens, int N, int g, int m, int M, int D,
                               tsb_search_stats* out);
 int tsb_pfsp_search_device_ckpt(int inst, int lb_kind, int ub, int m, int M, int D, int pools, const char* path,
                                 double seconds, tsb_search_stats* out);
+/* The PFSP searches as the reference built with MAX_JOBS = max_jobs runs them: only 50 (TSB_EINVAL otherwise), on
+ * ta031..ta060 (TSB_EUNSUPPORTED for any other inst, after the checks of the other arguments): 208-byte
+ * tsb_pfsp_node50 nodes, the bounds of steps 1 and 3 on 50 jobs, and 50-job handles (tsb_pfsp_create_wide) in step 2.
+ * Every other argument is checked as by the 20-job twin.
+ *   - tsb_pfsp_search_wide: host pools (tsb_pfsp_search);
+ *   - tsb_pfsp_search_device_wide: device pools (tsb_pfsp_search_device_pools): D tasks with the static split, `pools`
+ *     device pools per task, stealing under ub = 1.  Every round is one evaluate + generate_children pair of kernels
+ *     (csrc/pfsp_wide_expand.cuh); a task's pools run one after the other, never in a shared launch;
+ *   - tsb_pfsp_search_device_ckpt_wide: the resumable form of tsb_pfsp_search_device_wide, as
+ *     tsb_pfsp_search_device_ckpt is of tsb_pfsp_search_device_pools.  Its checkpoints hold 208-byte nodes, so a
+ *     20-job checkpoint is refused (TSB_EINVAL), and a 50-job one is refused by tsb_pfsp_search_device_ckpt. */
+int tsb_pfsp_search_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, tsb_search_stats* out);
+int tsb_pfsp_search_device_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, int pools,
+                                tsb_search_stats* out);
+int tsb_pfsp_search_device_ckpt_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, int pools,
+                                     const char* path, double seconds, tsb_search_stats* out);
 /* async-signal-safe: every resumable search running in the process (or the next one to start) stops at its next call
  * boundary; the search that stops on it clears it */
 void tsb_search_request_stop(void);
