@@ -21,4 +21,18 @@ constexpr long long pf_pool_capacity(int sms, int pools) {
   return static_cast<long long>(pf_ctas_per_pool(sms, pools)) * PFR_SLICE;
 }
 
+// The persistent kernel of 50-job pools (pfsp_wide_rounds.cuh) has the same slice, so the same capacities.  What it
+// takes is what tools/pfsp50_rounds.py measured faster than the step loop on an H100 (DESIGN §7): one pool up to its
+// capacity (measured to 50 688), two pools sharing a launch up to M = 20 000 (measured to there), never three or four
+// (not measured; their pools take the one-pool kernel in turn).
+constexpr int PFW_MAX_M_ONE = 50688;
+constexpr int PFW_MAX_M_SHARED = 20000;
+constexpr int PFW_MAX_POOLS_SHARED = 2;
+// whether one launch of that kernel takes `pools` pools with chunks of up to M parents (the occupancy of the kernel
+// itself aside).  Taking K >= 2 pools implies taking any 2..K of them: the shared launch's pools leave it one by one.
+constexpr bool pfw_takes(int sms, int pools, long long M) {
+  return pools >= 1 && pools <= PFW_MAX_POOLS_SHARED && M <= pf_pool_capacity(sms, pools) &&
+         M <= (pools == 1 ? PFW_MAX_M_ONE : PFW_MAX_M_SHARED);
+}
+
 }  // namespace tsb

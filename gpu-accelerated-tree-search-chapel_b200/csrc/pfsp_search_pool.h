@@ -1,7 +1,9 @@
 // pfsp_search_pool.h — the PFSP device-pool calls of the searches in tsb_host.cpp.  On a 20-job handle each is the
 // exported call of the same name (tsb_pfsp_pool_push, tsb_pfsp_sibling, tsb_pfsp_pool_run_multi).  On a 50-job handle
 // (tsb_pfsp_create_wide), which those refuse with TSB_EUNSUPPORTED, each runs the same operation on the handle's
-// 208-byte pool: rounds of pfsp_wide_expand.cuh, one pool after the other (no persistent kernel takes these nodes).
+// 208-byte pool: for lb1 and lb1_d, launches of the persistent kernel of pfsp_wide_rounds.cuh that serve all the pools
+// (one pool per launch, in turn, or the step loop, where pfw_takes does not take M); for lb2, rounds of
+// pfsp_wide_expand.cuh, one pool after the other.
 #pragma once
 #include <cstdint>
 

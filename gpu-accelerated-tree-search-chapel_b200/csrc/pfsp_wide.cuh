@@ -16,6 +16,7 @@
 //     add_front_and_bound (:197-222), lb2 with the scheduled set as a 64-bit mask and the reference's early exit.
 #pragma once
 #include <cstddef>
+#include <type_traits>
 
 #include "pfsp_kernels.cuh"
 #include "tsb_ptx.cuh"
@@ -56,12 +57,14 @@ struct PfspWideSmem {
   int32_t fc[PW_MAXM * PW_THREADS];  // lb2: the child's front, [machine][thread] (dynamically indexed by pair)
 };
 
-// The bound of every child slot k = limit1+1 .. jobs-1 of one parent (`node`: depth, limit1, prmu) into out[k]:
-// the parent's front / remain once, then one child at a time.  fc: the calling thread's column of
-// PfspWideSmem::fc (lb2 only, stride PW_THREADS).  Shared by the evaluator and the expand count kernel.
-template <int KIND, int M>
+// The bound of every child slot k = limit1+1 .. jobs-1 of one parent (`node`: depth, limit1, prmu) into out[k], or,
+// when `out` is a callable, to out(k, bound): the parent's front / remain once, then one child at a time.  fc: the
+// calling thread's column of PfspWideSmem::fc (lb2 only, stride PW_THREADS).  Shared by the evaluator, the expand count
+// kernel and the persistent kernel (pfsp_wide_rounds.cuh, which keeps no bound array: it folds each bound into the
+// parent's child mask as it comes).
+template <int KIND, int M, class Out>
 __device__ __forceinline__ void pw_parent_bounds(const PfspWideTables& tab, const int32_t* node, int32_t* fc, int best,
-                                                 int32_t* out) {
+                                                 Out&& out) {
   const int jobs = tab.jobs;
   const int limit1 = min(max(node[1], -1), jobs - 1);
   const int32_t* prmu = node + 2;
@@ -139,7 +142,10 @@ __device__ __forceinline__ void pw_parent_bounds(const PfspWideTables& tab, cons
         if (lb > best) break;  // :232-236
       }
     }
-    out[k] = lb;
+    if constexpr (std::is_pointer_v<std::decay_t<Out>>)
+      out[k] = lb;
+    else
+      out(k, lb);
   }
 }
 

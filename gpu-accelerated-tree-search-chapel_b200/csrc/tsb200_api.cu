@@ -28,6 +28,7 @@
 #include "pfsp_kernels.cuh"
 #include "pfsp_wide.cuh"
 #include "pfsp_wide_expand.cuh"
+#include "pfsp_wide_rounds.cuh"
 #include "pfsp_search_pool.h"
 #include "tsb200.h"
 
@@ -1849,6 +1850,73 @@ struct PfspRounds {
   PfspRounds of_pool(int i) const { return {lb_kind, best + i}; }
 };
 
+// ---- the same for 50-job handles: pfsp_wide_rounds_kernel (pfsp_wide_rounds.cuh) on 208-byte records
+constexpr size_t kPfWideRoundsSmem = sizeof(tsb::PfWideRoundsSmem) + 128;
+template <class F>
+int with_pfsp_wide_rounds_kernel(const tsb_pfsp* h, int lb_kind, F&& f) {
+  return with_machines(h->tab->mt, [&](auto mt) -> int {
+    constexpr int MT = decltype(mt)::value;
+    return lb_kind == TSB_LB1 ? f(tsb::pfsp_wide_rounds_kernel<1, MT>) : f(tsb::pfsp_wide_rounds_kernel<0, MT>);
+  });
+}
+// CTAs per pool of a launch that serves `pools` 50-job pools with chunks of up to M parents (pf_ctas_per_pool, fewer
+// for small M, as in pfsp_rounds_grid); 0: the pools run the step loop of pfsp_step instead (lb2, no cooperative
+// launch, env TSB200_NO_ROUNDS=1, M beyond pfw_takes, or, for several pools, the kernel does not fit twice on an SM)
+int pfsp_wide_grid(tsb_pfsp* h, int lb_kind, int M, int pools) {
+  if (lb_kind == TSB_LB2 || !h->di.coop || env_no_rounds() || !tsb::pfw_takes(h->di.sms, pools, M)) return 0;
+  int per_sm = 0;
+  if (with_pfsp_wide_rounds_kernel(h, lb_kind, [&](auto kernel) -> int {
+        return h->per_sm(kernel, tsb::PFW_THREADS, kPfWideRoundsSmem, &per_sm);
+      }) != TSB_OK || per_sm < (pools == 1 ? 1 : 2)) {
+    (void)cudaGetLastError();
+    return 0;
+  }
+  return static_cast<int>(std::min<long long>(tsb::pf_ctas_per_pool(h->di.sms, pools),
+                                              (static_cast<long long>(M) + tsb::PFW_TILE - 1) / tsb::PFW_TILE));
+}
+// The 50-job side of rounds_run: PfspRounds with the wide kernel, tables and launch shape
+struct PfspWideRounds : PfspRounds {
+  using Params = tsb::PfWideRoundsMultiParams;
+  static constexpr const char* kKernel = "pfsp_wide_rounds_kernel";
+
+  int grid(tsb_pfsp* h0, int M, int pools, int*) const { return pfsp_wide_grid(h0, lb_kind, M, pools); }
+  int prepare(tsb_pfsp* h, int i, int64_t, long long need, tsb::PfWideRoundsParams* prm, bool* queued) const {
+    DevicePool& p = h->pool;
+    const int rc = p.make_stack(h->stream, need);  // room for the worst case of the next round
+    prm->arena = p.arena[p.cur];
+    prm->tables = h->d_wtab;
+    prm->cap = p.cap;
+    prm->best = clamp_best(best[i]);
+    *queued = true;  // (a pfsp_step round may still be storing on h's stream)
+    return rc;
+  }
+  int launch(tsb_pfsp* h0, const tsb::PfWideRoundsMultiParams& mp, int grid, int pools, int) const {
+    return with_pfsp_wide_rounds_kernel(h0, lb_kind, [&](auto kernel) -> int {
+      int rc = h0->configure(kernel, kPfWideRoundsSmem);
+      if (rc != TSB_OK) return rc;
+      void* args[] = {const_cast<tsb::PfWideRoundsMultiParams*>(&mp)};
+      // cooperative: every CTA of every pool co-resident (the exchanges wait for all of a pool's CTAs), or the launch fails
+      TSB_CUDA(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(grid, pools), dim3(tsb::PFW_THREADS),
+                                           args, kPfWideRoundsSmem, h0->stream));
+      h0->launches++;
+      return TSB_OK;
+    });
+  }
+  // TSB200_ROUNDS_PROF: CTA 0's phases of each pool
+  void report(const tsb::RoundsState* pace, const int*, int n_act, int grid) const {
+    for (int a = 0; a < n_act; a++) {
+      const tsb::RoundsState& st = pace[a];
+      const double r = static_cast<double>(std::max<unsigned long long>(1, st.rounds));
+      std::fprintf(stderr, "[tsb200] PFSP 50-job rounds kernel (pool %d of %d, %d CTAs): %llu rounds (exit %d); CTA 0 "
+                   "cycles per round: load %.0f bounds %.0f publish %.0f gather %.0f store %.0f store-exchange %.0f\n",
+                   a, n_act, grid, static_cast<unsigned long long>(st.rounds), st.exit_code,
+                   st.prof[tsb::PFR_PROF_LOAD] / r, st.prof[tsb::PFR_PROF_BOUND] / r, st.prof[tsb::PFR_PROF_PUBLISH] / r,
+                   st.prof[tsb::PFR_PROF_GATHER] / r, st.prof[tsb::PFR_PROF_STORE] / r, st.prof[tsb::PFR_PROF_BARRIER] / r);
+    }
+  }
+  PfspWideRounds of_pool(int i) const { return {{lb_kind, best + i}}; }
+};
+
 // A handle with chunks of up to M_max parents on `device`, an empty pool and the tables `tab` (its own, or its owner's
 // for a sibling).  Tables with an index out of range give TSB_EINVAL, after the errors of the device itself.
 int pfsp_open(int device, int M_max, std::shared_ptr<const PfspPacked> tab, tsb_pfsp** out) {
@@ -2375,8 +2443,7 @@ int pfsp_pool_run_multi(tsb_pfsp* const* handles, int n_pools, int lb_kind, int 
     if (int rc = pfsp_check(handles[i], false, lb_kind); rc != TSB_OK) return rc;
   if (!one_group(handles, n_pools, M, [](const tsb_pfsp& h, const tsb_pfsp& h0) { return h.tab->wide == h0.tab->wide; }))
     return TSB_EINVAL;
-  // (no persistent kernel takes 208-byte nodes: PfspRounds::grid is 0, and the pools run their rounds in turn)
-  return pool_run_multi(PfspRounds{lb_kind, best}, handles, n_pools, m, M, max_rounds, out);
+  return pool_run_multi(PfspWideRounds{{lb_kind, best}}, handles, n_pools, m, M, max_rounds, out);
 }
 
 }  // namespace tsb::search

@@ -171,6 +171,7 @@ struct GpuTaskResult {
   uint64_t tree = 0, sol = 0, offloads = 0, parents = 0, launches = 0;
   int64_t best = 0;
   int rc = 0;
+  double t_pool_calls = 0;  // seconds inside the library's device-pool calls (TSB200_TRACE)
 };
 
 inline void bind_task(int device) {  // one host thread per GPU: next to its GPU (env TSB200_NO_NUMA=1: no)
@@ -332,6 +333,11 @@ inline int64_t rounds_per_call(bool moves, int M) { return !moves ? INT64_MAX : 
 // rounds per call of a resumable search where the search above makes one unbounded call: a stop waits for the call
 // in flight, and pool_run resumes bit-exactly, so the cap changes no chunk sequence
 constexpr int64_t kCkptRoundsPerCall = 1024;
+// (env TSB200_CKPT_ROUNDS overrides that cap, so that tests can stop a search after a few rounds of large chunks)
+inline int64_t ckpt_rounds_per_call() {
+  const char* v = std::getenv("TSB200_CKPT_ROUNDS");
+  return v && std::atoll(v) > 0 ? std::atoll(v) : kCkptRoundsPerCall;
+}
 
 // (env set: nodes never move between the device pools of a search, the static split alone)
 inline bool steal_allowed() { return !std::getenv("TSB200_NO_STEAL"); }
@@ -422,7 +428,9 @@ bool devpool_rounds(const S& s, const std::vector<H*>& hs, int m, int M, int64_t
       if (got == 0) break;
       continue;
     }
+    const double c0 = now_s();
     r.rc = s.run_multi(hs.data(), P, m, M, rounds, best, out.data());
+    r.t_pool_calls += now_s() - c0;
     if (r.rc != TSB_OK) break;
     for (int i = 0; i < P; i++) {
       r.offloads += out[4 * i];
@@ -445,7 +453,7 @@ bool devpool_rounds(const S& s, const std::vector<H*>& hs, int m, int M, int64_t
 // pool) back to the task's pool.  Each of several pools is one reference task with its own incumbent
 // (pfsp_multigpu_chpl.chpl:384), min-reduced here, and hands its leftovers back as a reference task does (popBack).
 // `ck` (a resumable search): the task resumes its pools and incumbents from a checkpoint instead of splitting its pool,
-// caps unbounded calls at kCkptRoundsPerCall rounds, and when it stops leaves its pools in ck->pools.
+// caps unbounded calls at ckpt_rounds_per_call() rounds, and when it stops leaves its pools in ck->pools.
 template <class S, class H, class Node>
 void devpool_on(const S& s, H* h, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me,
                 TaskCkpt* ck) {
@@ -479,11 +487,14 @@ void devpool_on(const S& s, H* h, int m, int M, Pool<Node>& pool, GpuTaskResult&
   }
   if (sb) sb->publish_handle(me, r.rc == TSB_OK ? h : nullptr, most);
   int64_t rounds = s.rounds(P, sb != nullptr, M);
-  if (ck && rounds == INT64_MAX) rounds = kCkptRoundsPerCall;
+  if (ck && rounds == INT64_MAX) rounds = ckpt_rounds_per_call();
   bool stopped = false;
   if (r.rc == TSB_OK)
     stopped = devpool_rounds(s, hs, m, M, rounds, s.balance, sb, me, best.get(), r, ck ? ck->stop : nullptr);
   r.best = *std::min_element(best.get(), best.get() + P);
+  if (std::getenv("TSB200_TRACE"))  // (the rounds alone: no handle set-up, pool push or drain)
+    std::fprintf(stderr, "[tsb200] task %d: %d pools, %llu rounds in %.3f ms of pool calls\n", me, P,
+                 static_cast<unsigned long long>(r.offloads), r.t_pool_calls * 1e3);
   if (stopped) {  // every pool with its incumbent, in logical order, for the checkpoint
     ck->stopped = true;
     ck->pools.resize(P);
@@ -881,7 +892,7 @@ inline int pfsp_create_for(tsb_pfsp** h, int device, int M, const tsb_pfsp_table
 
 // PFSP on the tables of a Taillard instance; `pools` device pools per task, as many as the caller asks for.
 // Node / Tables: tsb_pfsp_node / tsb_pfsp_tables (MAX_JOBS = 20) or tsb_pfsp_node50 / tsb_pfsp_tables50 (MAX_JOBS = 50:
-// 50-job handles, whose device pools run one after the other, with no shared launch)
+// 50-job handles, whose device pools share the launches of their own persistent kernel, pfsp_wide_rounds.cuh)
 template <class NodeT, class Tables>
 struct PfspSearch {
   using Node = NodeT;

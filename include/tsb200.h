@@ -486,8 +486,11 @@ int tsb_pfsp_search_device_ckpt(int inst, int lb_kind, int ub, int m, int M, int
  * Every other argument is checked as by the 20-job twin.
  *   - tsb_pfsp_search_wide: host pools (tsb_pfsp_search);
  *   - tsb_pfsp_search_device_wide: device pools (tsb_pfsp_search_device_pools): D tasks with the static split, `pools`
- *     device pools per task, stealing under ub = 1.  Every round is one evaluate + generate_children pair of kernels
- *     (csrc/pfsp_wide_expand.cuh); a task's pools run one after the other, never in a shared launch;
+ *     device pools per task, stealing under ub = 1.  Under lb1 and lb1_d a task's pools run their rounds in launches
+ *     of a persistent kernel (csrc/pfsp_wide_rounds.cuh) that serve all of them where its K-pool capacity and measured
+ *     cutoffs take M (csrc/pfr_tiers.h), or one pool after the other in launches that serve one; otherwise (lb2, larger
+ *     M, TSB200_NO_ROUNDS=1) every round is one evaluate + generate_children pair of kernels
+ *     (csrc/pfsp_wide_expand.cuh), one pool after the other.  The counts are the same on every route;
  *   - tsb_pfsp_search_device_ckpt_wide: the resumable form of tsb_pfsp_search_device_wide, as
  *     tsb_pfsp_search_device_ckpt is of tsb_pfsp_search_device_pools.  Its checkpoints hold 208-byte nodes, so a
  *     20-job checkpoint is refused (TSB_EINVAL), and a 50-job one is refused by tsb_pfsp_search_device_ckpt. */
