@@ -1,5 +1,5 @@
-// search_ckpt.cpp — the checkpoint file of a resumable device-pool search.  Layout (version 1), every field
-// little-endian and fixed-width, no padding:
+// search_ckpt.cpp — the checkpoint file of a resumable search, on device or host pools.  Layout (version 1), every
+// field little-endian and fixed-width, no padding:
 //   "TSB200CK"  u32 version  u32 problem  u32 rec
 //   i32 a, b, c, m, M, D, pools                               (the call's parameters, search_ckpt.h)
 //   u64 tree1, sol1  i64 best1  f64 t_step1, t_step2  u64 steals
@@ -196,6 +196,7 @@ int load(const char* path, const Params& want, State* st) {
     t.best = r.i64();
     const uint32_t finished = r.u32(), pools = r.u32();
     if (finished > 1 || pools > 4) return TSB_EINVAL;
+    if (p.host() && pools != (finished ? 0u : 1u)) return TSB_EINVAL;  // (a host task: its one pool, or its leftovers)
     t.finished = finished == 1;
     r.records(r.u64(), p.rec, t.left);
     t.pools.resize(pools);

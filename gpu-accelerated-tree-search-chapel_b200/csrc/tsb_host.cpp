@@ -156,8 +156,9 @@ void nq_generate_children(int N, const Node* parents, int size, const uint8_t* l
 std::atomic<int> g_stop_request{0};
 static_assert(std::atomic<int>::is_always_lock_free, "tsb_search_request_stop must be async-signal-safe");
 
-// The stop condition of a resumable search (tsb_*_search_device_ckpt): its deadline or a stop request.  A task asks
-// between two library calls, after its first one; once one task sees it, every task stops at its next boundary.
+// The stop condition of a resumable search (tsb_*_search[_device]_ckpt): its deadline or a stop request.  A task asks
+// between two library calls (device pools) or two offloads (host pools), after its first one; once one task sees it,
+// every task stops at its next boundary.
 struct StopCtl {
   double deadline = 0;                // now_s() + seconds at the call (infinity: no time limit)
   std::atomic<bool> stopping{false};  // latched
@@ -378,14 +379,57 @@ int drain_to_bytes(H* h, size_t rec, std::vector<uint8_t>& out) {
   return rc;
 }
 
-// one task's share of a resumable search: the device pools it resumes from (nullptr: it starts from its host pool),
-// the search's stop condition, and, when it stopped, the pools it left
+// one task's share of a resumable search: the pools it resumes from (nullptr: it starts from its share of step 1; a
+// host-pool task has exactly one), the search's stop condition, and, when it stopped, the pools it left
 struct TaskCkpt {
   const std::vector<tsb::ckpt::PoolState>* resume = nullptr;
   StopCtl* stop = nullptr;
   bool stopped = false;
   std::vector<tsb::ckpt::PoolState> pools;
 };
+
+// a host pool's nodes, front to back, as records of a checkpoint, and back
+template <class Node>
+std::vector<uint8_t> pool_records(const Pool<Node>& pool) {
+  const auto* b = reinterpret_cast<const uint8_t*>(pool.el.data() + pool.front);
+  return std::vector<uint8_t>(b, b + pool.size * sizeof(Node));
+}
+template <class Node>
+void push_records(const std::vector<uint8_t>& rec, Pool<Node>& pool) {
+  for (size_t i = 0; i + sizeof(Node) <= rec.size(); i += sizeof(Node)) {
+    Node n;
+    std::memcpy(&n, &rec[i], sizeof(Node));
+    pool.pushBack(n);
+  }
+}
+
+// The offload loop of one host-pool task (the drivers' step 2: nqueens_gpu_chpl.chpl:197-215, pfsp_gpu_chpl.chpl:
+// 373-395): popBackBulk(m, M), `offload` the chunk (one library call: evaluate, then generate_children on the host),
+// until the pool holds fewer than m nodes.  `ck` (a resumable search): the task resumes its pool and incumbent from
+// the checkpoint, and asks for a stop after every offload, never before its first one; when it stops it leaves its
+// pool, front to back, and its incumbent in ck->pools.  A host task never steals, so the chunk sequence across stops
+// is the uninterrupted one.
+template <class Node, class Offload>
+void host_pool_loop(int m, int M, Pool<Node>& pool, Node* parents, GpuTaskResult& r, TaskCkpt* ck, Offload&& offload) {
+  if (ck && ck->resume) {
+    const tsb::ckpt::PoolState& in = ck->resume->front();  // (load: exactly one per unfinished host task)
+    push_records(in.nodes, pool);
+    r.best = in.best;
+  }
+  for (;;) {
+    const int n = pool.popBackBulk(m, M, parents);
+    if (n <= 0) break;
+    r.rc = offload(n);
+    if (r.rc != TSB_OK) break;
+    ++r.offloads;
+    r.parents += static_cast<uint64_t>(n);
+    if (ck && ck->stop->check()) {
+      ck->stopped = true;
+      ck->pools.assign(1, tsb::ckpt::PoolState{r.best, pool_records(pool)});
+      break;
+    }
+  }
+}
 
 // The offload loop of one task whose P >= 1 pools (a handle and its siblings) are resident on the device: all rounds
 // of step 2 inside the library (one persistent kernel for small M, two kernels per round otherwise; the pools' rounds
@@ -836,7 +880,7 @@ struct NqSearch {
     nq_decompose(N, parent, tree, sol, pool);
   }
   // one GPU task's offload loop (nqueens_gpu_chpl.chpl:197-215; nqueens_multigpu_chpl.chpl:234-253)
-  void host_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r) const {
+  void host_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, TaskCkpt* ck) const {
     tsb_nq* h = nullptr;
     r.rc = nq_create_for<Node>(&h, device, N, g, M);
     if (r.rc != TSB_OK) return;
@@ -845,16 +889,12 @@ struct NqSearch {
     // the chunk arrays live for the whole step 2 (nqueens_gpu_chpl.chpl:191-192): page-lock them once
     tsb_nq_register_host(h, parents.data(), parents.size() * sizeof(Node));
     tsb_nq_register_host(h, labels.data(), labels.size());
-    for (;;) {
-      const int n = pool.popBackBulk(m, M, parents.data());
-      if (n <= 0) break;
-      r.rc = tsb_nq_evaluate(h, parents.data(), n, labels.data());
-      if (r.rc != TSB_OK) break;
-      ++r.offloads;
-      r.parents += static_cast<uint64_t>(n);
-      nq_generate_children(N, parents.data(), n, labels.data(), r.tree, r.sol, pool);
-    }
-    r.launches = tsb_nq_kernel_launches(h);
+    host_pool_loop(m, M, pool, parents.data(), r, ck, [&](int n) {
+      const int rc = tsb_nq_evaluate(h, parents.data(), n, labels.data());
+      if (rc == TSB_OK) nq_generate_children(N, parents.data(), n, labels.data(), r.tree, r.sol, pool);
+      return rc;
+    });
+    r.launches += tsb_nq_kernel_launches(h);
     tsb_nq_destroy(h);
   }
   void device_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me,
@@ -917,7 +957,7 @@ struct PfspSearch {
   void decompose(const Node& parent, uint64_t& tree, uint64_t& sol, int64_t& best, Pool<Node>& pool) const {
     pfsp_decompose(hb, lb_kind, parent, tree, sol, best, pool);
   }
-  void host_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r) const {
+  void host_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, TaskCkpt* ck) const {
     tsb_pfsp* h = nullptr;
     r.rc = pfsp_create_for(&h, device, M, &hb.t);
     if (r.rc != TSB_OK) return;
@@ -927,16 +967,12 @@ struct PfspSearch {
     // the chunk arrays live for the whole step 2 (pfsp_gpu_chpl.chpl:355-356): page-lock them once
     tsb_pfsp_register_host(h, parents.data(), parents.size() * sizeof(Node));
     tsb_pfsp_register_host(h, bounds.data(), bounds.size() * sizeof(int32_t));
-    for (;;) {
-      const int n = pool.popBackBulk(m, M, parents.data());
-      if (n <= 0) break;
-      r.rc = tsb_pfsp_evaluate(h, lb_kind, parents.data(), n, r.best, bounds.data());
-      if (r.rc != TSB_OK) break;
-      ++r.offloads;
-      r.parents += static_cast<uint64_t>(n);
-      pfsp_generate_children(jobs, parents.data(), n, bounds.data(), r.tree, r.sol, r.best, pool);
-    }
-    r.launches = tsb_pfsp_kernel_launches(h);
+    host_pool_loop(m, M, pool, parents.data(), r, ck, [&](int n) {
+      const int rc = tsb_pfsp_evaluate(h, lb_kind, parents.data(), n, r.best, bounds.data());
+      if (rc == TSB_OK) pfsp_generate_children(jobs, parents.data(), n, bounds.data(), r.tree, r.sol, r.best, pool);
+      return rc;
+    });
+    r.launches += tsb_pfsp_kernel_launches(h);
     tsb_pfsp_destroy(h);
   }
   void device_task(int device, int m, int M, Pool<Node>& pool, GpuTaskResult& r, StealBoard* sb, int me,
@@ -972,8 +1008,8 @@ struct SearchCkpt {
 // process-per-GPU launch): the step-1 tree is credited to part 0 and every part drains its own leftovers, so the
 // per-part counts add up to the whole search's.  `on` != nullptr: D = 1 on device pools of a handle the caller created
 // (set-up outside the search's timers, as the Chapel drivers' `on device var` declarations are).
-// `ck` (D tasks on device pools, part < 0): a resumed search skips step 1 and continues step 2 from the checkpoint; a
-// search that stops writes the checkpoint and returns TSB_ESTOPPED with the counts so far.
+// `ck` (D tasks on device or host pools, part < 0): a resumed search skips step 1 and continues step 2 from the
+// checkpoint; a search that stops writes the checkpoint and returns TSB_ESTOPPED with the counts so far.
 template <class S>
 int three_step_search(const S& s, int m, int M, int D, int part, int device, typename S::Handle* on,
                       tsb_search_stats* out, SearchCkpt* ck = nullptr) {
@@ -1020,16 +1056,11 @@ int three_step_search(const S& s, int m, int M, int D, int part, int device, typ
   const auto finished = [&](int gid) { return from && from->tasks[gid].finished; };
   const auto task = [&](int dev, Pool<Node>& own, GpuTaskResult& r, StealBoard* sb, int me) {
     if (finished(me)) {
-      const std::vector<uint8_t>& left = from->tasks[me].left;
-      for (size_t i = 0; i + sizeof(Node) <= left.size(); i += sizeof(Node)) {
-        Node n;
-        std::memcpy(&n, &left[i], sizeof(Node));
-        own.pushBack(n);
-      }
+      push_records(from->tasks[me].left, own);
     } else if (s.devpool) {
       s.device_task(dev, m, M, own, r, sb, me, ck ? &tck[me] : nullptr);
     } else {
-      s.host_task(dev, m, M, own, r);
+      s.host_task(dev, m, M, own, r, ck ? &tck[me] : nullptr);
     }
   };
   // a task's leftovers back to the global pool (:315-320); several pools per task already handed theirs back to the
@@ -1085,7 +1116,7 @@ int three_step_search(const S& s, int m, int M, int D, int part, int device, typ
   }
   double t2 = now_s();
   out->t_step2 = (from ? from->t_step2 : 0) + (t2 - t1);
-  if (stopped) {  // the checkpoint: step 1, every task's counters, and its device pools or (finished) its leftovers
+  if (stopped) {  // the checkpoint: step 1, every task's counters, and its pools or (finished) its leftovers
     tsb::ckpt::State st;
     st.p = ck->params;
     st.tree1 = tree1, st.sol1 = sol1, st.best1 = best1;
@@ -1098,9 +1129,7 @@ int three_step_search(const S& s, int m, int M, int D, int part, int device, typ
       t.best = r.best;
       t.finished = !tck[gid].stopped;
       if (t.finished) {
-        const Pool<Node>& own = D == 1 ? pool : multi[gid];
-        const auto* b = reinterpret_cast<const uint8_t*>(own.el.data() + own.front);
-        t.left.assign(b, b + own.size * sizeof(Node));
+        t.left = pool_records(D == 1 ? pool : multi[gid]);
       } else {
         t.pools = std::move(tck[gid].pools);
       }
@@ -1202,6 +1231,30 @@ int nq_warmup(int N, int min_size, void* nodes, int64_t capacity, int64_t* n, ui
 template <class F>
 int with_nq_node(bool wide, F&& f) {
   return wide ? f(tsb_nq_node24{}) : f(tsb_nq_node{});
+}
+
+// tsb_nq_search[_device]_ckpt: max_queens = 20 runs N <= 20 on 21-byte nodes and N > 20 on 25-byte nodes, 24 every N
+// on 25-byte nodes.  (N-Queens has no pools argument: how many device pools a task runs is checked against the
+// checkpoint per task; c = 1 marks the host-pool search, search_ckpt.h)
+int nq_search_ckpt(bool devpool, int max_queens, int N, int g, int m, int M, int D, const char* path, double seconds,
+                   tsb_search_stats* out) {
+  if (max_queens != TSB_MAX_QUEENS && max_queens != TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
+  return with_nq_node(max_queens == TSB_MAX_QUEENS_WIDE || N > TSB_MAX_QUEENS, [&](auto node) {
+    using Node = decltype(node);
+    const tsb::ckpt::Params p{tsb::ckpt::kNQueens, sizeof(Node), N, g, devpool ? 0 : 1, m, M, D, 0};
+    return ckpt_search(path, seconds, p, [&](SearchCkpt* ck) {
+      return nq_search<Node>(N, g, m, M, D, devpool, -1, 0, nullptr, out, ck);
+    });
+  });
+}
+// tsb_pfsp_search[_device]_ckpt[_wide]: the host-pool search has one pool per task and writes pools = 0
+template <class Node>
+int pfsp_search_ckpt(bool devpool, int inst, int lb_kind, int ub, int m, int M, int D, int pools, const char* path,
+                     double seconds, tsb_search_stats* out) {
+  const tsb::ckpt::Params p{tsb::ckpt::kPfsp, sizeof(Node), inst, lb_kind, ub, m, M, D, devpool ? pools : 0};
+  return ckpt_search(path, seconds, p, [&](SearchCkpt* ck) {
+    return pfsp_search<Node>(inst, lb_kind, ub, m, M, D, devpool, -1, 0, nullptr, out, pools, ck);
+  });
 }
 }  // namespace
 
@@ -1309,22 +1362,19 @@ int tsb_pfsp_search_on_pools(tsb_pfsp* h, int inst, int lb_kind, int ub, int m, 
 
 int tsb_nq_search_device_ckpt(int max_queens, int N, int g, int m, int M, int D, const char* path, double seconds,
                               tsb_search_stats* out) {
-  if (max_queens != TSB_MAX_QUEENS && max_queens != TSB_MAX_QUEENS_WIDE) return TSB_EINVAL;
-  return with_nq_node(max_queens == TSB_MAX_QUEENS_WIDE || N > TSB_MAX_QUEENS, [&](auto node) {
-    using Node = decltype(node);
-    // (N-Queens has no pools argument: how many pools a task runs is checked against the checkpoint per task)
-    const tsb::ckpt::Params p{tsb::ckpt::kNQueens, sizeof(Node), N, g, 0, m, M, D, 0};
-    return ckpt_search(path, seconds, p, [&](SearchCkpt* ck) {
-      return nq_search<Node>(N, g, m, M, D, true, -1, 0, nullptr, out, ck);
-    });
-  });
+  return nq_search_ckpt(true, max_queens, N, g, m, M, D, path, seconds, out);
+}
+int tsb_nq_search_ckpt(int max_queens, int N, int g, int m, int M, int D, const char* path, double seconds,
+                       tsb_search_stats* out) {
+  return nq_search_ckpt(false, max_queens, N, g, m, M, D, path, seconds, out);
 }
 int tsb_pfsp_search_device_ckpt(int inst, int lb_kind, int ub, int m, int M, int D, int pools, const char* path,
                                 double seconds, tsb_search_stats* out) {
-  const tsb::ckpt::Params p{tsb::ckpt::kPfsp, sizeof(tsb_pfsp_node), inst, lb_kind, ub, m, M, D, pools};
-  return ckpt_search(path, seconds, p, [&](SearchCkpt* ck) {
-    return pfsp_search(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out, pools, ck);
-  });
+  return pfsp_search_ckpt<tsb_pfsp_node>(true, inst, lb_kind, ub, m, M, D, pools, path, seconds, out);
+}
+int tsb_pfsp_search_ckpt(int inst, int lb_kind, int ub, int m, int M, int D, const char* path, double seconds,
+                         tsb_search_stats* out) {
+  return pfsp_search_ckpt<tsb_pfsp_node>(false, inst, lb_kind, ub, m, M, D, 1, path, seconds, out);
 }
 int tsb_pfsp_search_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, tsb_search_stats* out) {
   if (max_jobs != TSB_MAX_JOBS_WIDE) return TSB_EINVAL;
@@ -1338,10 +1388,12 @@ int tsb_pfsp_search_device_wide(int max_jobs, int inst, int lb_kind, int ub, int
 int tsb_pfsp_search_device_ckpt_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, int pools,
                                      const char* path, double seconds, tsb_search_stats* out) {
   if (max_jobs != TSB_MAX_JOBS_WIDE) return TSB_EINVAL;
-  const tsb::ckpt::Params p{tsb::ckpt::kPfsp, sizeof(tsb_pfsp_node50), inst, lb_kind, ub, m, M, D, pools};
-  return ckpt_search(path, seconds, p, [&](SearchCkpt* ck) {
-    return pfsp_search<tsb_pfsp_node50>(inst, lb_kind, ub, m, M, D, true, -1, 0, nullptr, out, pools, ck);
-  });
+  return pfsp_search_ckpt<tsb_pfsp_node50>(true, inst, lb_kind, ub, m, M, D, pools, path, seconds, out);
+}
+int tsb_pfsp_search_ckpt_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, const char* path,
+                              double seconds, tsb_search_stats* out) {
+  if (max_jobs != TSB_MAX_JOBS_WIDE) return TSB_EINVAL;
+  return pfsp_search_ckpt<tsb_pfsp_node50>(false, inst, lb_kind, ub, m, M, D, 1, path, seconds, out);
 }
 void tsb_search_request_stop(void) { g_stop_request.store(1); }
 

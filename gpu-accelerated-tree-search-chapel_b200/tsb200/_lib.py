@@ -165,6 +165,9 @@ SYMBOLS = {
     "tsb_pfsp_search_device_ckpt_wide": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, C.c_char_p, C.c_double,
                                               C.POINTER(SearchStats)]),
     "tsb_search_request_stop": (None, []),
+    "tsb_nq_search_ckpt": (_i, [_i, _i, _i, _i, _i, _i, C.c_char_p, C.c_double, C.POINTER(SearchStats)]),
+    "tsb_pfsp_search_ckpt": (_i, [_i, _i, _i, _i, _i, _i, C.c_char_p, C.c_double, C.POINTER(SearchStats)]),
+    "tsb_pfsp_search_ckpt_wide": (_i, [_i, _i, _i, _i, _i, _i, _i, C.c_char_p, C.c_double, C.POINTER(SearchStats)]),
 }
 
 _lib = None
@@ -198,7 +201,7 @@ def check_search(code: int, where: str, stats) -> None:
 
 
 def ckpt_args(checkpoint, time_limit):
-    """the path and seconds arguments of tsb_*_search_device_ckpt (time_limit None: no limit)"""
+    """the path and seconds arguments of tsb_*_search[_device]_ckpt (time_limit None: no limit)"""
     return os.fsencode(os.fspath(checkpoint)), -1.0 if time_limit is None else float(time_limit)
 
 

@@ -128,12 +128,17 @@ def nqueens_warmup(N: int, min_size: int = 25):
 
 
 def nqueens_search(N: int = 14, g: int = 1, m: int = 25, M: int = 50000, D: int = 1,
-                   max_queens: int | None = None) -> SearchStats:
+                   max_queens: int | None = None, checkpoint=None, time_limit: float | None = None) -> SearchStats:
     """the 3-step search of nqueens_gpu_chpl.chpl:152-248 (D = 1) / nqueens_multigpu_chpl.chpl:158-352
     (static split, D GPUs), run by the C++ emulation driver inside libtsb200.so.  N in 1..24 (N > 20 with 25-byte
-    nodes); max_queens=24: every N as a MAX_QUEENS = 24 build runs it (tsb_nq_search_wide)"""
+    nodes); max_queens=24: every N as a MAX_QUEENS = 24 build runs it (tsb_nq_search_wide).  checkpoint /
+    time_limit: the resumable search (tsb_nq_search_ckpt), as for nqueens_search_device"""
     st = SearchStats()
-    if max_queens is None:
+    if checkpoint is not None:
+        mq = MAX_QUEENS if max_queens is None else max_queens
+        check_search(lib().tsb_nq_search_ckpt(mq, N, g, m, M, D, *ckpt_args(checkpoint, time_limit), C.byref(st)),
+                     "tsb_nq_search_ckpt", st)
+    elif max_queens is None:
         check(lib().tsb_nq_search(N, g, m, M, D, C.byref(st)), "tsb_nq_search")
     else:
         check(lib().tsb_nq_search_wide(max_queens, N, g, m, M, D, C.byref(st)), "tsb_nq_search_wide")

@@ -205,23 +205,35 @@ def pfsp_search_device(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: in
     return st
 
 
-def pfsp_search(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1) -> SearchStats:
-    """pfsp_gpu_chpl.chpl:306-431 (D = 1) / pfsp_multigpu_chpl.chpl (static split), C++ emulation driver"""
+def pfsp_search(inst: int = 14, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1,
+                checkpoint=None, time_limit: float | None = None) -> SearchStats:
+    """pfsp_gpu_chpl.chpl:306-431 (D = 1) / pfsp_multigpu_chpl.chpl (static split), C++ emulation driver.
+    checkpoint / time_limit: the resumable search (tsb_pfsp_search_ckpt), as for nqueens_search_device"""
     kind = _lb(lb)
     st = SearchStats()
-    check(lib().tsb_pfsp_search(inst, kind, ub, m, M, D, C.byref(st)), "tsb_pfsp_search")
+    if checkpoint is not None:
+        check_search(lib().tsb_pfsp_search_ckpt(inst, kind, ub, m, M, D, *ckpt_args(checkpoint, time_limit),
+                                                C.byref(st)), "tsb_pfsp_search_ckpt", st)
+    else:
+        check(lib().tsb_pfsp_search(inst, kind, ub, m, M, D, C.byref(st)), "tsb_pfsp_search")
     return st
 
 
 MAX_JOBS_WIDE = 50
 
 
-def pfsp_search_wide(inst: int = 31, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1) -> SearchStats:
+def pfsp_search_wide(inst: int = 31, lb="lb1", ub: int = 1, m: int = 25, M: int = 50000, D: int = 1,
+                     checkpoint=None, time_limit: float | None = None) -> SearchStats:
     """pfsp_search as the reference built with MAX_JOBS = 50 runs it (tsb_pfsp_search_wide): ta031..ta060, 208-byte
-    nodes"""
+    nodes (with checkpoint / time_limit the resumable tsb_pfsp_search_ckpt_wide)"""
     kind = _lb(lb)
     st = SearchStats()
-    check(lib().tsb_pfsp_search_wide(MAX_JOBS_WIDE, inst, kind, ub, m, M, D, C.byref(st)), "tsb_pfsp_search_wide")
+    if checkpoint is not None:
+        check_search(lib().tsb_pfsp_search_ckpt_wide(MAX_JOBS_WIDE, inst, kind, ub, m, M, D,
+                                                     *ckpt_args(checkpoint, time_limit), C.byref(st)),
+                     "tsb_pfsp_search_ckpt_wide", st)
+    else:
+        check(lib().tsb_pfsp_search_wide(MAX_JOBS_WIDE, inst, kind, ub, m, M, D, C.byref(st)), "tsb_pfsp_search_wide")
     return st
 
 

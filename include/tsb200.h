@@ -499,8 +499,26 @@ int tsb_pfsp_search_device_wide(int max_jobs, int inst, int lb_kind, int ub, int
                                 tsb_search_stats* out);
 int tsb_pfsp_search_device_ckpt_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, int pools,
                                      const char* path, double seconds, tsb_search_stats* out);
+/* Resumable host-pool searches: the searches of tsb_nq_search (max_queens = 20: N <= 20 on 21-byte nodes, N > 20 on
+ * 25-byte nodes) or tsb_nq_search_wide (max_queens = 24), tsb_pfsp_search and tsb_pfsp_search_wide (max_jobs = 50),
+ * whose step-2 pools stay on the host and call only tsb_*_evaluate.  Every other argument is checked as by that twin,
+ * and `path`, `seconds`, TSB_ESTOPPED, the summed stats and the removal of the file at the end are as for
+ * tsb_*_search_device_ckpt, with one difference: a task asks for a stop between two offloads (after generate_children
+ * of a chunk, before the next popBackBulk), never before its first one, so seconds = 0 stops as soon as every task has
+ * made one offload.  A stopped task leaves its host pool, front to back, and its incumbent in the checkpoint; a resumed
+ * one rebuilds that pool in the same order and continues with popBackBulk.
+ * Host tasks never steal, so a resumed search equals the uninterrupted one in every field but the times and
+ * kernel_launches, for any D and for ub 0 and 1 alike (stronger than the device-pool forms promise).
+ * Their checkpoints are marked as host-pool ones: a device-pool checkpoint is refused here, and a host-pool checkpoint
+ * by the tsb_*_search_device_ckpt forms (TSB_EINVAL before any device call, the file unchanged). */
+int tsb_nq_search_ckpt(int max_queens, int N, int g, int m, int M, int D, const char* path, double seconds,
+                       tsb_search_stats* out);
+int tsb_pfsp_search_ckpt(int inst, int lb_kind, int ub, int m, int M, int D, const char* path, double seconds,
+                         tsb_search_stats* out);
+int tsb_pfsp_search_ckpt_wide(int max_jobs, int inst, int lb_kind, int ub, int m, int M, int D, const char* path,
+                              double seconds, tsb_search_stats* out);
 /* async-signal-safe: every resumable search running in the process (or the next one to start) stops at its next call
- * boundary; the search that stops on it clears it */
+ * boundary (host pools: its next offload); the search that stops on it clears it */
 void tsb_search_request_stop(void);
 
 #ifdef __cplusplus

@@ -1,7 +1,7 @@
-"""What the resumable device-pool searches (tsb_*_search_device_ckpt) cost when they do not stop, what a stop costs,
-and how large their checkpoints are.
+"""What the resumable searches (tsb_*_search_device_ckpt on device pools, tsb_*_search_ckpt on host pools) cost when
+they do not stop, what a stop costs, and how large their checkpoints are.
 
-  python tools/search_ckpt_time.py [--reps 3] [--out DIR]
+  python tools/search_ckpt_time.py [--reps 3] [--parts whole,capped,checkpoints,host] [--out DIR]
 
 1. Whole searches, the twin and the resumable search without a time limit alternated `reps` times on warm handles
    (step-2 seconds and kernel launches): N = 17 at M = 50 000 (four pools per task, 2048 rounds per call in both) and
@@ -12,6 +12,9 @@ and how large their checkpoints are.
 3. Checkpoints: N = 17, the whole N = 21 search and ta014 lb1, all at M = 50 000, stopped after `--stop` seconds
    (N = 17, ta014: after one call), with the file's size, the time from the stop to the return, the write and read
    times (TSB200_TRACE lines of a child process) and the time of the resumed invocation.
+4. Host pools: the twin (tsb_pfsp_search, tsb_nq_search) and its resumable form without a time limit alternated `reps`
+   times, ta014 lb1 and N = 17 (--host-N; about three minutes per search on an H100), both at M = 50 000 (step-2
+   seconds): the resumable form asks for a stop once per chunk.
 Prints one JSON line per measurement after the name and power limit of the card; --out DIR also writes them to
 DIR/search_ckpt_time.jsonl."""
 import argparse
@@ -73,6 +76,25 @@ def whole(reps, tmp):
             emit({"what": "whole search", "case": name, "rep": rep, "twin_step2_s": round(a.t_step2, 5),
                   "ckpt_step2_s": round(b.t_step2, 5), "twin_launches": a.kernel_launches,
                   "ckpt_launches": b.kernel_launches, "offloads": a.offloads})
+
+
+def host_whole(reps, tmp, N):
+    cases = {
+        "host_ta014_lb1_M50000": (lambda: tsb200.pfsp_search(14, "lb1", 1, 25, 50000, 1),
+                                  lambda p: tsb200.pfsp_search(14, "lb1", 1, 25, 50000, 1, checkpoint=p)),
+        f"host_nq{N}_M50000": (lambda: tsb200.nqueens_search(N, 1, 25, 50000, 1),
+                               lambda p: tsb200.nqueens_search(N, 1, 25, 50000, 1, checkpoint=p)),
+    }
+    for name, (twin, ckpt) in cases.items():
+        for rep in range(reps):
+            a = twin()
+            b = ckpt(os.path.join(tmp, name))
+            assert (a.explored_tree, a.explored_sol, a.best, a.offloads) == \
+                (b.explored_tree, b.explored_sol, b.best, b.offloads)
+            emit({"what": "whole host-pool search", "case": name, "rep": rep, "twin_step2_s": round(a.t_step2, 4),
+                  "ckpt_step2_s": round(b.t_step2, 4), "offloads": a.offloads,
+                  "twin_Mnodes_per_s": round(a.explored_tree / a.t_step2 / 1e6, 2),
+                  "ckpt_Mnodes_per_s": round(b.explored_tree / b.t_step2 / 1e6, 2)})
 
 
 def capped(reps):
@@ -147,13 +169,21 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--stop", type=float, default=5.0, help="seconds of the N = 21 search before it stops")
+    ap.add_argument("--host-N", type=int, default=17, help="board size of the host-pool N-Queens case")
+    ap.add_argument("--parts", default="whole,capped,checkpoints,host", help="which measurements, comma-separated")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
+    parts = a.parts.split(",")
     emit({"card": card()})
     with tempfile.TemporaryDirectory() as tmp:
-        whole(a.reps, tmp)
-        capped(a.reps)
-        checkpoints(tmp, a.stop)
+        if "whole" in parts:
+            whole(a.reps, tmp)
+        if "capped" in parts:
+            capped(a.reps)
+        if "checkpoints" in parts:
+            checkpoints(tmp, a.stop)
+        if "host" in parts:
+            host_whole(a.reps, tmp, a.host_N)
     if a.out:
         os.makedirs(a.out, exist_ok=True)
         with open(os.path.join(a.out, "search_ckpt_time.jsonl"), "w") as f:
